@@ -3,7 +3,7 @@
 
     metric   : embed+top-k query images/sec  (whole job: embed gallery + queries with the descriptor network,
                L2-normalise, all-pairs dot-product similarity, per-query top-k)
-    default  : configs[1] (C2) "10k query x 100k gallery, SSCD ResNet-50 embed+top-k on 1 B200"; at N > 1 every rank
+    default  : configs[1] (C2) "10k query x 100k gallery, SSCD ResNet-50 embed+top-k on 1 H100"; at N > 1 every rank
                holds a 100k-image gallery shard and a 10k block of queries (weak scaling), all queries are scored against
                every shard, per-shard top-k lists are all-gathered and merged (dcr_b200/dist.py).
     --config c3      configs[2]: DINO ViT-S/16 instead of the SSCD ResNet-50, same sizes
@@ -49,7 +49,8 @@ def load_peaks():
             d = json.load(f)
         return {"burst": float(d["bf16_tflops"]), "sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                 "hbm": float(d["hbm_gbs"]), "src": "measured"}
-    return {"burst": 1590.0, "sustained": 1400.0, "hbm": 6650.0, "src": "fallback"}
+    # NVIDIA's H100 SXM data sheet (700 W): dense bf16 and HBM3 bandwidth -- an upper bound, not a measured rate
+    return {"burst": 989.0, "sustained": 989.0, "hbm": 3350.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler(threading.Thread):
@@ -181,8 +182,7 @@ _CPU_THREADS = None
 def _cpu_threads() -> int:
     """SURVEY.md 8d: the CPU baseline uses every host core.  torchrun exports OMP_NUM_THREADS=1, so torch's default
     would be one thread under the multi-GPU launch; the count is set explicitly.  On a hyper-threaded host one thread per
-    LOGICAL cpu can be several times slower than one per physical core for MKL/oneDNN kernels (measured on the B200 box:
-    2.6 img/s with 128 threads against 18.8 with 64), so both are tried on a small ResNet-50 forward and the FASTER one is
+    LOGICAL cpu can be several times slower than one per physical core for MKL/oneDNN kernels, so both are tried on a small ResNet-50 forward and the FASTER one is
     used and reported -- the baseline is the reference path at its best on this host."""
     global _CPU_THREADS
     if _CPU_THREADS is not None:
@@ -295,11 +295,12 @@ def parse_args():
     ap.add_argument("--other-modes", default="bf16x3,parity",
                     help="comma-separated network modes measured after the headline one (same full workload)")
     ap.add_argument("--batch", type=int, default=384,
-                    help="images per network launch (measured on B200: 73.5k img/s at 256, 79.9k at 384 -- wave quantisation of the "
-                         "persistent kernels over 148 SMs)")
+                    help="images per network launch")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--cpu-embed-sample", type=int, default=128)
     ap.add_argument("--cpu-sim-sample", type=int, default=1000)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed to DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     args = ap.parse_args()
     if args.net is None:
         args.net = "dino" if args.config == "c3" else "sscd"
@@ -336,16 +337,16 @@ def make_config(args, world, q_total, g_total, d_desc, precision):
     return {"workload": f"{net_name} embed + dot-product top-{K_TOP}: {q_total} query x {g_total} gallery "
                         f"synthetic 256x256 images ({per})",
             "baseline_config": args.config, "network": net_name, "precision": precision,
-            "precision_note": ("networks in bf16 (one plane) on tcgen05, fp32 accumulate; similarity scores are exact "
+            "precision_note": ("networks in bf16 (one plane) on wgmma, fp32 accumulate; similarity scores are exact "
                                "fp64-accumulated dot products of the fp32 descriptors the network produced.  bf16 descriptors "
-                               "deviate from the fp32 reference path by more than the 1e-4 score tolerance (see "
-                               "precision_modes.measured_deviation_from_fp32); the fp32-level modes are reported beside it"
+                               "deviate from the fp32 reference path by more than the 1e-4 score tolerance; "
+                               "the fp32-level modes are reported beside it"
                                if precision == "fast" else
-                               "networks in split-bf16 (two / three planes) on tcgen05: fp32-level descriptors"),
+                               "networks in split-bf16 (two / three planes) on wgmma: fp32-level descriptors"),
             "queries": q_total, "gallery": g_total, "descriptor_dim": d_desc, "k": K_TOP,
             "images_embedded_per_step": q_total + g_total, "parallelism": f"gallery-shard x{world}",
             "l2": f"inputs ({imgs_per_gpu * IMG * IMG * 3 / 1e9:.1f} GB of images per GPU) are larger than "
-                  "the 126 MB L2; no explicit flush"}
+                  "the 50 MB L2; no explicit flush"}
 
 
 def run_reference(args, rank, world):
@@ -422,6 +423,38 @@ def check_result(values, indices, qf_all_fn, gf, g_base, world, dev, n_check: in
             "against": "per-rank fp64 torch matmul + stable sort on a query subsample, merged on the host"}
 
 
+def _row_sample(x, max_rows: int, seed: int):
+    """All rows of x, or a fixed seeded sample of max_rows of them (sorted row numbers, returned beside the rows)."""
+    n = x.shape[0]
+    if n <= max_rows:
+        return None, x
+    rows = torch.from_numpy(np.sort(np.random.default_rng(seed).choice(n, max_rows, replace=False)))
+    return rows, x[rows.to(x.device)]
+
+
+def save_arrays(out_dir, arrays):
+    total = sum(a.numel() * a.element_size() for a in arrays.values())
+    assert total <= 64 << 20, f"--dump-outputs: {total / 2**20:.1f} MB exceeds 64 MB"
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.cpu().numpy())
+
+
+def dump_outputs(out_dir, topk, qf, gf, max_query_rows: int = 12288, max_gallery_rows: int = 8192):
+    """What the last timed step returned (top-k scores and gallery indices per query) and the descriptors it matched:
+    the query and gallery rows, or fixed seeded samples of them where all rows would exceed the 64 MB budget."""
+    values, indices = topk
+    arrays = {"topk_values": values.float(), "topk_indices": indices.double()}
+    for name, x, cap, seed in (("query", qf, max_query_rows, 1), ("gallery", gf, max_gallery_rows, 0)):
+        rows, sample = _row_sample(x, cap, seed)
+        if rows is None:
+            arrays[f"{name}_features"] = sample.float()
+        else:
+            arrays[f"{name}_feature_rows"] = rows.double()
+            arrays[f"{name}_features_sample"] = sample.float()
+    save_arrays(out_dir, arrays)
+
+
 def run_retrieval_bench(args, rank, local_rank, world):
     import torch.distributed as dist
     from dcr_b200 import dist as ddist
@@ -434,7 +467,7 @@ def run_retrieval_bench(args, rank, local_rank, world):
         dist.init_process_group("nccl", device_id=dev)
     q_total, g_total, q_local, g_local, g_base = shard_sizes(args, rank, world)
     need_gb = (q_local + g_local) * IMG * IMG * 3 / 1e9
-    if need_gb > 150:
+    if need_gb > 0.6 * torch.cuda.get_device_properties(dev).total_memory / 1e9:
         raise SystemExit(f"this rank would hold {need_gb:.0f} GB of images: use more GPUs for --config {args.config}")
     q_sizes = [shard_sizes(args, r, world)[2] for r in range(world)]
 
@@ -463,13 +496,15 @@ def run_retrieval_bench(args, rank, local_rank, world):
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = {}
+
     def timed(fn, steps):
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         barrier()
         ev0.record()
         kms = []
         for _ in range(steps):
-            fn()
+            last["out"] = fn()
             kms.append(similarity.sim_topk_stats()["kernel_ms"])
         ev1.record()
         barrier()
@@ -492,6 +527,8 @@ def run_retrieval_bench(args, rank, local_rank, world):
     if rank == 0:
         sampler.stop_flag.set()
         sampler.join(timeout=2)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, last["out"], keep["qf"], keep["gf"])
 
     # ---- the step validates its own output (all ranks take part: collectives inside) -------------------------------
     out_v, out_i = step(gal_u8, qry_u8)
@@ -570,7 +607,7 @@ def run_retrieval_bench(args, rank, local_rank, world):
             pj = json.load(f)
         if pj.get("shape", [10000, 100000, 512, 10]) == [q_total, g_local, d_desc, K_TOP]:
             traffic = pj.get("dram_bytes_per_launch")
-    roofline = {"kernel": "sim_topk_kernel<2> (fused Q.G^T + per-query top-k, tcgen05 cta_group::2)",
+    roofline = {"kernel": "sim_topk_kernel (fused Q.G^T + per-query top-k, wgmma)",
                 "bound": "tensor", "achieved": achieved, "peak": peaks["sustained"], "unit": "TFLOP/s",
                 "frac": achieved / peaks["sustained"], "frac_of_burst_peak": achieved / peaks["burst"],
                 "peak_source": f"{peaks['src']} bf16_tflops_sustained (kernel timed inside a long step)",
@@ -593,10 +630,6 @@ def run_retrieval_bench(args, rank, local_rank, world):
         line["precision_modes"] = {args.precision: {"value": value, "unit": "query images/s", "ms_per_step": ms_per_step,
                                                     "note": notes.get(args.precision, "")}}
         line["precision_modes"].update(others)
-        line["precision_modes"]["measured_deviation_from_fp32"] = (
-            "tests/test_round2_gpu.py::test_precision_mode_contracts_against_fp32_mode (B200, 2304 images): max |score error| "
-            "fast 9.7e-5 / bf16x3 3.6e-7 / parity 5.6e-7 on contractive random-init weights; fast 2.1e-1 / bf16x3 9.2e-4 / parity "
-            "9.1e-4 on THIS benchmark's calibrated (chaotic) synthetic weights; every replicated image is found in every mode")
     if world == 1:
         v, det = cpu_reference_sample(args.net, args.cpu_embed_sample, args.cpu_sim_sample, g_total, q_total, d_desc)
         line["cpu_baseline"] = {"value": v, "unit": "query images/s", "cores": det["cores"], "kind": "port",
@@ -628,8 +661,10 @@ def run_fid_bench(args, rank, local_rank, world):
     gen = gen_images_cuda(n_gen, seed=400 + rank, device=dev, size=FID_IMG)
     result = {}
 
-    def step(r, g):
-        result["fid"] = dfid.fid_from_images(net, r, g, batch_size=bs)
+    def step(r, g):   # dfid.fid_from_images, keeping the statistics for --dump-outputs
+        m1, s1 = dfid.statistics_of_images(net, r, bs)
+        m2, s2 = dfid.statistics_of_images(net, g, bs)
+        result.update(fid=dfid.frechet_distance(m1, s1, m2, s2), mu_real=m1, sigma_real=s1, mu_gen=m2, sigma_gen=s2)
 
     def barrier():
         if world > 1:
@@ -656,6 +691,11 @@ def run_fid_bench(args, rank, local_rank, world):
         sampler.start()
     l0 = similarity.kernel_launch_count()
     ms = timed(lambda: step(real, gen), args.steps) / args.steps
+    if rank == 0 and args.dump_outputs:
+        t = lambda x: torch.as_tensor(np.asarray(x))   # noqa: E731
+        save_arrays(args.dump_outputs, {"fid": torch.tensor([float(result["fid"])], dtype=torch.float64),
+                                        "mu_real": t(result["mu_real"]).double(), "mu_gen": t(result["mu_gen"]).double(),
+                                        "sigma_real": t(result["sigma_real"]).float(), "sigma_gen": t(result["sigma_gen"]).float()})
     launches = similarity.kernel_launch_count() - l0
     n_total = (n_gen + n_real) * world
     e2e = None
@@ -682,7 +722,7 @@ def run_fid_bench(args, rank, local_rank, world):
             "config": {"workload": f"FID: {n_gen * world} generated vs {n_real * world} real synthetic 299x299 images, "
                                    "Inception-v3 pool3 + streaming fp64 mean/covariance + Frechet distance",
                        "baseline_config": "c4", "precision": args.precision, "batch": bs,
-                       "l2": "inputs (tens of GB of images) are larger than the 126 MB L2; no explicit flush"},
+                       "l2": "inputs (tens of GB of images) are larger than the 50 MB L2; no explicit flush"},
             "fid_value": result.get("fid"), "gpu_launches": int(launches), "clocks": sampler.summary(),
             "roofline": {"kernel": "FID Inception-v3 forward (all conv GEMMs, per GPU)", "bound": "tensor",
                          "achieved": tfl / world, "peak": peaks["sustained"], "unit": "TFLOP/s",
@@ -703,6 +743,8 @@ def main():
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.impl == "reference":
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs writes what the GPU path computed; --impl reference times a CPU sample")
         run_reference(args, rank, world)
         return
     if not torch.cuda.is_available():

@@ -1,4 +1,4 @@
-"""In-tree build of libdcr_b200.so (sm_100a) and of the CPU oracle's C helpers.
+"""In-tree build of libdcr_b200.so (sm_90a, NVIDIA H100).
 
 `python -m dcr_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles without a GPU.  Objects are cached by
 source mtime so a rebuild after touching one .cu file takes seconds.
@@ -18,7 +18,7 @@ BUILD_DIR = PKG_DIR / "_build"
 LIB_PATH = PKG_DIR / "libdcr_b200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -66,7 +66,7 @@ def build(verbose: bool = False, force: bool = False) -> Path:
     if jobs or force or _needs(LIB_PATH, objs):
         # cudart linked statically: the .so only needs libcuda (driver) at run time, resolved lazily by cudart
         run([nvcc, "-shared", "-o", str(LIB_PATH), *map(str, objs), "-cudart", "static",
-             "-gencode", "arch=compute_100a,code=sm_100a"])
+             "-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB_PATH
 
 

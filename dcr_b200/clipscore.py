@@ -1,4 +1,4 @@
-"""CLIP score on the B200 path: the host mirror of `gen_clipscore` (utils_ret.py:1046-1066; called by
+"""CLIP score on the H100 path: the host mirror of `gen_clipscore` (utils_ret.py:1046-1066; called by
 diff_retrieval.py:485-487 for the query and the gallery loaders).
 
     for images, caps in loader:                                   utils_ret.py:1053

@@ -1,24 +1,24 @@
-// Cross-layer fusion of the ResNet bottleneck's 1x1 pair (sm_100a, tcgen05 + TMA):
+// Cross-layer fusion of the ResNet bottleneck's 1x1 pair (sm_90a, wgmma + TMA):
 //
 //     Y  = relu(scale3 * (T2 @ W3^T) + bias3 + X)        conv3 (1x1 expand) + BN + residual + ReLU of block i
 //     T1 = relu(scale1 * (Y  @ W1^T) + bias1)            conv1 (1x1 reduce) + BN + ReLU of block i+1
 //
 // as ONE kernel.  Unfused, the expanded activation Y (B*H*W x 4*width bf16: 411 MB at 56x56, batch 256) is written by the
-// first GEMM and read again by the second -- and both GEMMs already run at the HBM roofline (profiles/r01_layers_sscd.txt:
-// 5.9 / 6.5 TB/s of algorithmic bytes).  Here a CTA keeps the 128 rows of T2 it works on resident, walks the column
+// first GEMM and read again by the second, and both GEMMs are HBM bound.  Here a CTA keeps the 128 rows of T2 it works on resident, walks the column
 // blocks of Y, and every finished 128x128 block of Y is (a) stored to HBM (block i+1 still needs it as its residual) and
 // (b) consumed IN PLACE from the store's 128B-swizzled staging tile as the A operand of the second GEMM, whose
-// accumulator lives in its own TMEM columns.  Y is never read back: per row 2*(K1 + 2*N1 + N2) bytes instead of
+// accumulator stays in registers for the whole m-tile.  Y is never read back: per row 2*(K1 + 2*N1 + N2) bytes instead of
 // 2*(K1 + 3*N1 + N2) -- 1028 instead of 1439 MB per layer1 block pair.
 //
 // Reference call sites replaced (through `model(samples)`, utils_ret.py:751): torchvision Bottleneck.forward's
 // conv3/bn3/+identity/relu of one block and conv1/bn1/relu of the next (SSCD trunk, SURVEY.md 8a4).
 //
-// Roles (320 threads, persistent over 128-row m-tiles):  warp 0 TMA producer, warp 1 tcgen05.mma issuer, warps 2-9 epilogue.
+// Roles (288 threads, persistent over 128-row m-tiles):  warps 0-7 two consumer warpgroups (warpgroup h: wgmma and epilogue
+// of the 64-column slab h of every Y block and of columns [h N2/2, (h+1) N2/2) of T1), warp 8 TMA producer.
 //   shared memory   A1 (T2 rows, all of K1; 1-2 buffers) | W ring (16 KB stages: W3 tiles and W1 slabs in issue order) |
 //                   3 rotating X tiles (128 x 128 bf16: residual lands here by TMA, the epilogue overwrites it in place
 //                   with Y, the TMA store and the second GEMM read it) | T1 staging | BN tables | mbarriers
-//   tensor memory   [0,256) two accumulators of the first GEMM, [256, 256+N2) accumulator of the second
+//   registers       per warpgroup a 128 x 64 accumulator of the first GEMM and a 128 x N2/2 one of the second
 // Results are bit-identical to the two separate launches of conv_gemm.cu (same K order, same epilogue arithmetic).
 #include <cuda_bf16.h>
 
@@ -33,15 +33,14 @@ namespace dcr {
 
 namespace {
 
-constexpr int kFM = 128;                 // rows per m-tile (TMEM lanes)
+constexpr int kFM = 128;                 // rows per m-tile
 constexpr int kFN = 128;                 // columns of Y per n-block
 constexpr int kFK = 64;                  // bf16 per 128-byte swizzled row
-constexpr int kFThreads = 320;
+constexpr int kFThreads = 288;
 constexpr int kSlab = kFM * 128;         // one [128 rows x 64 bf16] slab, 16 KB
 constexpr int kXTile = 2 * kSlab;        // one 128 x 128 tile of X / Y
 constexpr int kXBufs = 3;
 constexpr int kWStage = kSlab;           // 16 KB: a W3 tile [128 x 64] or a W1 slab [N2 <= 128 x 64]
-constexpr uint32_t kAcc2Col = 256;       // TMEM column of the second accumulator
 
 struct FuseMaps {
   CUtensorMap a;      // T2   [M, K1]   box 128 x 64
@@ -99,17 +98,10 @@ __global__ void __launch_bounds__(kFThreads, 1) expand_reduce_kernel(const __gri
   uint64_t* a_empty = bars + 2;       // [2]
   uint64_t* w_full = bars + 4;        // [8]
   uint64_t* w_empty = bars + 12;      // [8]
-  uint64_t* t_full = bars + 20;       // [2]
-  uint64_t* t_empty = bars + 22;      // [2]
   uint64_t* r_full = bars + 24;       // [3] residual tile landed in X buffer b
-  uint64_t* y_ready = bars + 27;      // [3] epilogue finished writing Y into X buffer b
-  uint64_t* y_free = bars + 30;       // [3] second GEMM finished reading X buffer b
-  uint64_t* acc2_full = bars + 33;
-  uint64_t* acc2_empty = bars + 34;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 35);
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&maps.a);
     tma_prefetch_desc(&maps.w3);
     tma_prefetch_desc(&maps.res);
@@ -117,37 +109,22 @@ __global__ void __launch_bounds__(kFThreads, 1) expand_reduce_kernel(const __gri
     tma_prefetch_desc(&maps.w1);
     tma_prefetch_desc(&maps.out2);
   }
-  if (warp == 1 && lane == 0) {
+  if (warp == 0 && lane == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], 1);
-      mbar_init(&t_full[s], 1);
-      mbar_init(&t_empty[s], 8);
+      mbar_init(&a_empty[s], 8);   // one arrive per consumer warp
     }
     for (int s = 0; s < 8; ++s) {
       mbar_init(&w_full[s], 1);
-      mbar_init(&w_empty[s], 1);
+      mbar_init(&w_empty[s], 8);
     }
-    for (int s = 0; s < kXBufs; ++s) {
-      mbar_init(&r_full[s], 1);
-      mbar_init(&y_ready[s], 1);
-      mbar_init(&y_free[s], 1);
-    }
-    mbar_init(acc2_full, 1);
-    mbar_init(acc2_empty, 8);
+    for (int s = 0; s < kXBufs; ++s) mbar_init(&r_full[s], 1);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc<1>(tmem_slot, 512);
-    tmem_relinquish<1>();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int num_m_tiles = p.num_m_tiles;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================================== TMA producer =====================================
     PipeState ws(p.w_stages), as(p.a_bufs);
     for (int tile = blockIdx.x; tile < num_m_tiles; tile += gridDim.x, as.next()) {
@@ -156,102 +133,53 @@ __global__ void __launch_bounds__(kFThreads, 1) expand_reduce_kernel(const __gri
       if (elect_one()) {
         mbar_arrive_expect_tx(&a_full[as.s], a_buf_bytes);
         for (int ki = 0; ki < k_iters1; ++ki)
-          tma_load_2d<1>(smem_a + as.s * a_buf_bytes + ki * kSlab, &maps.a, &a_full[as.s], ki * kFK, m0, kEvictFirst);
+          tma_load_2d(smem_a + as.s * a_buf_bytes + ki * kSlab, &maps.a, &a_full[as.s], ki * kFK, m0, kEvictFirst);
       }
       __syncwarp();
-      for (int j = 0; j <= nb; ++j) {
-        if (j < nb) {   // W3 tiles of column block j
+      for (int j = 0; j < nb; ++j) {
+        {   // W3 tiles of column block j
           for (int ki = 0; ki < k_iters1; ++ki, ws.next()) {
             mbar_wait(&w_empty[ws.s], ws.ph ^ 1);
             if (elect_one()) {
               mbar_arrive_expect_tx(&w_full[ws.s], kFN * 128);
-              tma_load_2d<1>(smem_w + ws.s * kWStage, &maps.w3, &w_full[ws.s], ki * kFK, j * kFN, kEvictLast);
+              tma_load_2d(smem_w + ws.s * kWStage, &maps.w3, &w_full[ws.s], ki * kFK, j * kFN, kEvictLast);
             }
             __syncwarp();
           }
         }
-        if (kSecond && j >= 1) {   // W1 slabs matching the two 64-column slabs of Y block j-1
+        if (kSecond) {   // W1 slabs matching the two 64-column slabs of Y block j
           for (int sl = 0; sl < 2; ++sl, ws.next()) {
             mbar_wait(&w_empty[ws.s], ws.ph ^ 1);
             if (elect_one()) {
               mbar_arrive_expect_tx(&w_full[ws.s], N2 * 128);
-              tma_load_2d<1>(smem_w + ws.s * kWStage, &maps.w1, &w_full[ws.s], ((j - 1) * 2 + sl) * kFK, 0, kEvictLast);
+              tma_load_2d(smem_w + ws.s * kWStage, &maps.w1, &w_full[ws.s], (j * 2 + sl) * kFK, 0, kEvictLast);
             }
             __syncwarp();
           }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================== MMA issuer =====================================
-    constexpr uint32_t idesc1 = umma_idesc_bf16(kFM, kFN);
-    constexpr uint32_t idesc2 = umma_idesc_bf16(kFM, kSecond ? N2 : 64);
-    PipeState ws(p.w_stages), as(p.a_bufs), xs(kXBufs);
-    const uint64_t da0 = umma_desc_sw128(smem_u32(smem_a));
-    const uint64_t dw0 = umma_desc_sw128(smem_u32(smem_w));
-    const uint64_t dx0 = umma_desc_sw128(smem_u32(smem_x));
-    const uint32_t tmem_acc2 = tmem_base + kAcc2Col;
-    uint32_t g = 0, mt = 0;
-    for (int tile = blockIdx.x; tile < num_m_tiles; tile += gridDim.x, ++mt, as.next()) {
-      mbar_wait(&a_full[as.s], as.ph);
-      tc_fence_after();
-      const uint64_t da_buf = da0 + static_cast<uint64_t>(as.s * (a_buf_bytes >> 4));
-      for (int j = 0; j <= nb; ++j) {
-        if (j < nb) {   // first GEMM, column block j -> accumulator g & 1
-          const uint32_t buf = g & 1;
-          mbar_wait(&t_empty[buf], ((g >> 1) & 1) ^ 1);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + buf * kFN;
-          for (int ki = 0; ki < k_iters1; ++ki, ws.next()) {
-            mbar_wait(&w_full[ws.s], ws.ph);
-            tc_fence_after();
-            const uint64_t da = da_buf + static_cast<uint64_t>(ki * (kSlab >> 4));
-            const uint64_t db = dw0 + static_cast<uint64_t>(ws.s * (kWStage >> 4));
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < kFK / 16; ++k) umma_f16<1>(tmem_d, da + 2 * k, db + 2 * k, idesc1, (ki | k) != 0);
-              umma_commit<1>(&w_empty[ws.s]);
-              if (ki == k_iters1 - 1) {
-                umma_commit<1>(&t_full[buf]);
-                if (j == nb - 1) umma_commit<1>(&a_empty[as.s]);
-              }
-            }
-            __syncwarp();
-          }
-          ++g;
-        }
-        if (kSecond && j >= 1) {   // second GEMM: acc2 += Y block j-1 (in X buffer xs.s) x W1 slabs
-          mbar_wait(&y_ready[xs.s], xs.ph);
-          if (j == 1) mbar_wait(acc2_empty, (mt & 1) ^ 1);   // previous m-tile's T1 epilogue has drained acc2
-          tc_fence_after();
-          for (int sl = 0; sl < 2; ++sl, ws.next()) {
-            mbar_wait(&w_full[ws.s], ws.ph);
-            tc_fence_after();
-            const uint64_t da = dx0 + static_cast<uint64_t>(xs.s * (kXTile >> 4) + sl * (kSlab >> 4));
-            const uint64_t db = dw0 + static_cast<uint64_t>(ws.s * (kWStage >> 4));
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < kFK / 16; ++k) umma_f16<1>(tmem_acc2, da + 2 * k, db + 2 * k, idesc2, (j > 1) || (sl | k) != 0);
-              umma_commit<1>(&w_empty[ws.s]);
-              if (sl == 1) {
-                umma_commit<1>(&y_free[xs.s]);
-                if (j == nb) umma_commit<1>(acc2_full);
-              }
-            }
-            __syncwarp();
-          }
-          xs.next();
         }
       }
     }
   } else {
-    // ===================================== epilogue warps =====================================
-    const uint32_t ewarp = warp - 2;               // 0..7
-    const uint32_t quad = warp & 3;                // TMEM lane quadrant
-    const uint32_t half = ewarp >> 2;              // which 64-column slab of a 128-column tile
+    // ===================================== consumer warpgroups =====================================
+    const uint32_t ewarp = warp;                   // 0..7
+    const uint32_t quad = warp & 3;                // rows quad*32 .. +31 of the m-tile
+    const uint32_t half = ewarp >> 2;              // which 64-column slab of a 128-column tile (= warpgroup)
     const uint32_t row = quad * 32 + lane;
     const uint32_t etid = ewarp * 32 + lane;
-    const uint32_t tmem_row = tmem_base + ((quad * 32u) << 16);
+    const uint32_t a0 = smem_u32(smem_a), w0 = smem_u32(smem_w);
+    PipeState ws(p.w_stages), as(p.a_bufs);
+    // one k-block of 64 from shared memory: A rows at a_addr (128 x 64), B rows at b_addr (N x 64), then release the W stage
+    auto kblock = [&](auto& acc, uint32_t a_addr, uint32_t b_addr, bool first) {
+      mbar_wait(&w_full[ws.s], ws.ph);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kFK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), (first && k == 0) ? 0u : 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc.fence_regs();
+      if (lane == 0) mbar_arrive(&w_empty[ws.s]);
+      ws.next();
+    };
     const uint32_t sb_addr = smem_u32(sb), x_addr = smem_u32(smem_x), o2_addr = smem_u32(smem_o2);
     const int N1 = p.N1;
     for (int c = etid; c < N1; c += 256) {
@@ -266,133 +194,78 @@ __global__ void __launch_bounds__(kFThreads, 1) expand_reduce_kernel(const __gri
     if (etid == 0 && static_cast<int>(blockIdx.x) < num_m_tiles) {
       mbar_arrive_expect_tx(&r_full[0], kXTile);
       for (int sl = 0; sl < 2; ++sl)
-        tma_load_2d<1>(smem_x + sl * kSlab, &maps.res, &r_full[0], sl * kFK, blockIdx.x * kFM, kEvictFirst);
+        tma_load_2d(smem_x + sl * kSlab, &maps.res, &r_full[0], sl * kFK, blockIdx.x * kFM, kEvictFirst);
     }
     asm volatile("bar.sync 1, 256;" ::: "memory");
     PipeState xs(kXBufs);
-    uint32_t g = 0, mt = 0;
-    const uint32_t sw = row & 7;
-    for (int tile = blockIdx.x; tile < num_m_tiles; tile += gridDim.x, ++mt) {
+    uint32_t g = 0;
+    for (int tile = blockIdx.x; tile < num_m_tiles; tile += gridDim.x, as.next()) {
       const int m0 = tile * kFM;
+      mbar_wait(&a_full[as.s], as.ph);
+      const uint32_t a_buf = a0 + as.s * a_buf_bytes;
+      WgAcc<kSecond ? N2 / 2 : 32> acc2;
       for (int j = 0; j < nb; ++j, ++g, xs.next()) {
-        const uint32_t buf = g & 1;
         const uint32_t xb = xs.s;
         if (etid == 0) {
           // prefetch the residual of the NEXT n-tile (possibly the first of this CTA's next m-tile) into the buffer
-          // tile g-2 used: its TMA store must have finished reading it and the second GEMM must have consumed it
+          // tile g-2 used: its TMA store must have finished reading it (the second GEMM of tile g-2 completed before
+          // every consumer thread passed the end-of-block barrier of tile g-1)
           const bool has_next = (j + 1 < nb) || (tile + static_cast<int>(gridDim.x) < num_m_tiles);
           if (has_next) {
             const uint32_t xn = (xb + 1 == kXBufs) ? 0 : xb + 1;
-            if (g >= 2) {
-              store_wait_read_1();
-              if constexpr (kSecond) {
-                const uint32_t ph_prev = (xb >= 2) ? xs.ph : (xs.ph ^ 1);   // parity of use (g-2)/3 of buffer xn
-                mbar_wait(&y_free[xn], ph_prev);
-              }
-            }
+            if (g >= 2) store_wait_read_1();
             const int nm0 = (j + 1 < nb) ? m0 : (tile + static_cast<int>(gridDim.x)) * kFM;
             const int nn0 = (j + 1 < nb) ? (j + 1) * kFN : 0;
             mbar_arrive_expect_tx(&r_full[xn], kXTile);
             for (int sl = 0; sl < 2; ++sl)
-              tma_load_2d<1>(smem_x + xn * kXTile + sl * kSlab, &maps.res, &r_full[xn], nn0 + sl * kFK, nm0, kEvictFirst);
+              tma_load_2d(smem_x + xn * kXTile + sl * kSlab, &maps.res, &r_full[xn], nn0 + sl * kFK, nm0, kEvictFirst);
           }
         }
-        mbar_wait(&t_full[buf], (g >> 1) & 1);
-        tc_fence_after();
+        // first GEMM, column block j: this warpgroup's 64-column slab
+        WgAcc<64> acc;
+        for (int ki = 0; ki < k_iters1; ++ki) kblock(acc, a_buf + ki * kSlab, w0 + ws.s * kWStage + half * 64 * 128, ki == 0);
+        if (j == nb - 1 && lane == 0) mbar_arrive(&a_empty[as.s]);
         mbar_wait(&r_full[xb], xs.ph);
-        const uint32_t taddr = tmem_row + buf * kFN + half * 64;
-        const uint32_t xrow = x_addr + xb * kXTile + half * kSlab + row * 128;
+        // epilogue straight from the accumulator layout: per pair of adjacent columns one 4-byte residual word is read
+        // and overwritten in place with Y (each word belongs to exactly one thread)
+        const uint32_t xslab = x_addr + xb * kXTile + half * kSlab;
         const uint32_t s_scale = sb_addr + (j * kFN + half * 64) * 4;
         const uint32_t s_bias = s_scale + N1 * 4;
-#pragma unroll 1
-        for (int ci = 0; ci < 2; ++ci) {
-          uint32_t r[32];
-          tmem_ld_32x32(taddr + ci * 32, r);
-          tmem_ld_wait_regs(r);
-          if (ci == 1) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&t_empty[buf]);
-          }
-          float y[32];
-#pragma unroll
-          for (int c = 0; c < 32; c += 4) {
-            const float4 sc = ld_shared_f4(s_scale + (ci * 32 + c) * 4);
-            const float4 bi = ld_shared_f4(s_bias + (ci * 32 + c) * 4);
-            y[c + 0] = fmaf(__uint_as_float(r[c + 0]), sc.x, bi.x);
-            y[c + 1] = fmaf(__uint_as_float(r[c + 1]), sc.y, bi.y);
-            y[c + 2] = fmaf(__uint_as_float(r[c + 2]), sc.z, bi.z);
-            y[c + 3] = fmaf(__uint_as_float(r[c + 3]), sc.w, bi.w);
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {   // residual: this thread's 16-byte chunks of its row, read then overwritten in place
-            const uint32_t addr = xrow + (((ci * 4 + q) ^ sw) << 4);
-            const uint4 rv = ld_shared_v4(addr);
-            const uint32_t w[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              y[q * 8 + 2 * e] += __uint_as_float(w[e] << 16);
-              y[q * 8 + 2 * e + 1] += __uint_as_float(w[e] & 0xffff0000u);
-            }
-            uint4 v;
-            v.x = pack2(fmaxf(y[q * 8 + 0], 0.f), fmaxf(y[q * 8 + 1], 0.f));
-            v.y = pack2(fmaxf(y[q * 8 + 2], 0.f), fmaxf(y[q * 8 + 3], 0.f));
-            v.z = pack2(fmaxf(y[q * 8 + 4], 0.f), fmaxf(y[q * 8 + 5], 0.f));
-            v.w = pack2(fmaxf(y[q * 8 + 6], 0.f), fmaxf(y[q * 8 + 7], 0.f));
-            st_shared_v4(addr, v);
-          }
-        }
-        fence_proxy_async();   // generic-proxy writes -> visible to the TMA store and to tcgen05.mma (async proxy)
+        acc.for_each_pair(lane, [&](uint32_t r, uint32_t c, float v0, float v1) {
+          const uint32_t rr = quad * 32 + r;
+          const uint32_t addr = xslab + rr * 128 + (((c >> 3) ^ (rr & 7)) << 4) + (c & 7) * 2;
+          const float2 sc = ld_shared_f2(s_scale + c * 4), bi = ld_shared_f2(s_bias + c * 4);
+          const uint32_t w = ld_shared_u32(addr);
+          float y0 = fmaf(v0, sc.x, bi.x), y1 = fmaf(v1, sc.y, bi.y);
+          y0 += __uint_as_float(w << 16);
+          y1 += __uint_as_float(w & 0xffff0000u);
+          st_shared_u32(addr, pack2(fmaxf(y0, 0.f), fmaxf(y1, 0.f)));
+        });
+        fence_proxy_async();   // generic-proxy writes -> visible to the TMA store and to wgmma (async proxy)
         asm volatile("bar.sync 2, 256;" ::: "memory");
         if (etid == 0) {
           for (int sl = 0; sl < 2; ++sl)
             tma_store_2d_(&maps.out, x_addr + xb * kXTile + sl * kSlab, j * kFN + sl * kFK, m0);
           store_commit();
-          if constexpr (kSecond) mbar_arrive(&y_ready[xb]);
+        }
+        if constexpr (kSecond) {   // second GEMM: acc2 += Y block j (in place in X buffer xb) x W1 slabs
+          for (int sl = 0; sl < 2; ++sl)
+            kblock(acc2, x_addr + xb * kXTile + sl * kSlab, w0 + ws.s * kWStage + half * (N2 / 2) * 128, j == 0 && sl == 0);
         }
       }
       if constexpr (!kSecond) continue;
       // ---- T1 tile of this m-tile: acc2 -> BN + ReLU -> bf16 -> staging -> TMA store ----
       if (etid == 0) store_wait_read_1();   // the previous m-tile's T1 store has finished reading the staging slabs
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      mbar_wait(acc2_full, mt & 1);
-      tc_fence_after();
       {
-        constexpr int kCh = N2 / 64;   // 32-column chunks per warp
         const uint32_t s_scale2 = sb_addr + 2 * N1 * 4;
         const uint32_t s_bias2 = s_scale2 + N2 * 4;
-#pragma unroll 1
-        for (int ci = 0; ci < kCh; ++ci) {
-          const int ch = half * kCh + ci;
-          uint32_t r[32];
-          tmem_ld_32x32(tmem_row + kAcc2Col + ch * 32, r);
-          tmem_ld_wait_regs(r);
-          if (ci == kCh - 1) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(acc2_empty);
-          }
-          float y[32];
-#pragma unroll
-          for (int c = 0; c < 32; c += 4) {
-            const float4 sc = ld_shared_f4(s_scale2 + (ch * 32 + c) * 4);
-            const float4 bi = ld_shared_f4(s_bias2 + (ch * 32 + c) * 4);
-            y[c + 0] = fmaxf(fmaf(__uint_as_float(r[c + 0]), sc.x, bi.x), 0.f);
-            y[c + 1] = fmaxf(fmaf(__uint_as_float(r[c + 1]), sc.y, bi.y), 0.f);
-            y[c + 2] = fmaxf(fmaf(__uint_as_float(r[c + 2]), sc.z, bi.z), 0.f);
-            y[c + 3] = fmaxf(fmaf(__uint_as_float(r[c + 3]), sc.w, bi.w), 0.f);
-          }
-          const uint32_t orow = o2_addr + (ch >> 1) * kSlab + row * 128;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint4 v;
-            v.x = pack2(y[q * 8 + 0], y[q * 8 + 1]);
-            v.y = pack2(y[q * 8 + 2], y[q * 8 + 3]);
-            v.z = pack2(y[q * 8 + 4], y[q * 8 + 5]);
-            v.w = pack2(y[q * 8 + 6], y[q * 8 + 7]);
-            st_shared_v4(orow + ((((ch & 1) * 4 + q) ^ sw) << 4), v);
-          }
-        }
+        acc2.for_each_pair(lane, [&](uint32_t r, uint32_t cl, float v0, float v1) {
+          const uint32_t rr = quad * 32 + r, c = half * (N2 / 2) + cl;
+          const float2 sc = ld_shared_f2(s_scale2 + c * 4), bi = ld_shared_f2(s_bias2 + c * 4);
+          const uint32_t addr = o2_addr + (c >> 6) * kSlab + rr * 128 + ((((c & 63) >> 3) ^ (rr & 7)) << 4) + (c & 7) * 2;
+          st_shared_u32(addr, pack2(fmaxf(fmaf(v0, sc.x, bi.x), 0.f), fmaxf(fmaf(v1, sc.y, bi.y), 0.f)));
+        });
       }
       fence_proxy_async();
       asm volatile("bar.sync 2, 256;" ::: "memory");
@@ -404,9 +277,6 @@ __global__ void __launch_bounds__(kFThreads, 1) expand_reduce_kernel(const __gri
     if (etid == 0) store_wait_all();
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<1>(tmem_base, 512);
 }
 
 }  // namespace
@@ -461,7 +331,8 @@ int launch_fused(const FuseMaps& maps, const FuseParams& p, int grid, size_t sme
 static int expand_reduce_impl(const ConvGemmDesc& a, const ConvGemmDesc* b, cudaStream_t stream) {
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  DCR_REQUIRE(di->cc_major == 10, "expand_reduce: this build targets sm_100a; device reports sm_%d%d", di->cc_major, di->cc_minor);
+  DCR_REQUIRE(di->cc_major == 9 && di->cc_minor == 0, "expand_reduce: this build targets sm_90a; device reports sm_%d%d", di->cc_major,
+              di->cc_minor);
   const long long M = static_cast<long long>(a.B) * a.H * a.W;
   DCR_REQUIRE(M > 0 && M < (1ll << 31), "expand_reduce: M out of range");
   const int n2 = b ? b->N : 0;

@@ -6,14 +6,13 @@
 // one image and the producer loads, per 64-channel block, ONE halo block
 //       [(R + 2) input rows] x [(W + 2) pixels, the two extra ones zero-filled by the TMA unit] x [64 channels]
 // as a single 4-D tiled TMA box.  In shared memory that is a width-padded raster of 128-byte rows, so the A operand of
-// filter tap (r, s) is the SAME buffer read from a start address shifted by (r * (W + 2) + s) rows: nine UMMA descriptor
+// filter tap (r, s) is the SAME buffer read from a start address shifted by (r * (W + 2) + s) rows: nine wgmma descriptor
 // start addresses instead of nine loads.  (The 128-byte swizzle is a function of the absolute shared-memory address
-// on both the TMA write and the UMMA read side, so a start address that is a multiple of 128 B but not of 1024 B is
+// on both the TMA write and the wgmma read side, so a start address that is a multiple of 128 B but not of 1024 B is
 // fine.)  MMA row m of the tile is padded-raster position m = pl * (W + 2) + ql; positions with ql >= W (2 per row)
 // and the rows past R * (W + 2) are junk that the epilogue drops when it compacts the tile into the [R x W] staging
 // box of the TMA store.  W + 2 <= 64 and R = 128 / (W + 2) rows: 2 rows at 56 wide (87.5 % useful MMA rows), 4 at 28,
-// 8 at 14.  Used for N <= 128 (measured on B200: 171 -> 89 us at 56x56x64->64, 74 -> 55 us at 28x28x128->128, batch
-// 256; at N = 256 only two 32 KB weight stages fit beside the halo buffers and the generic kernel is faster).
+// 8 at 14.  Used for N <= 128 (at N = 256 only two 32 KB weight stages fit beside the halo buffers).
 //
 // Weights are streamed per (tap, channel block) exactly as in the generic kernel (all SMs read the same tiles; that
 // traffic is served at several times the rate of per-SM-unique data).  Fast (single-plane bf16) mode only, no residual:
@@ -34,12 +33,7 @@ namespace {
 constexpr int kHM = 128;                    // MMA rows (padded-raster positions) per tile
 constexpr int kHK = 64;                     // channels per block = one 128-byte swizzled row
 constexpr int kSlabBytes = kHM * 128;       // one 64-channel slab of the output staging tile
-constexpr int kHThreads = 352;              // warp 0 producer, warp 1 (and 10) MMA issuers, warps 2..9 epilogue
-// Timing experiments (garbage results), compile-time only: bit 0 = no weight loads, bit 1 = no halo loads.
-#ifndef DCR_HALO_TIMING_MODE
-#define DCR_HALO_TIMING_MODE 0
-#endif
-constexpr int kHaloTimingMode = DCR_HALO_TIMING_MODE;
+constexpr int kHThreads = 288;              // warps 0-7 two consumer warpgroups (MMA + epilogue), warp 8 producer
 
 struct HaloMaps {
   CUtensorMap a;     // input  [B][H][W][C]   box 64 x (W+2) x (R+2) x 1
@@ -67,176 +61,95 @@ DCR_DEVICE uint32_t pack_bf16_(float a, float b) {
 }
 
 // kRW: ALL filter taps stay resident in shared memory (9 * cblocks tiles of [BN x 64]; fits for the 64 -> 64 convolutions of
-// ResNet layer1: 72 KB) and TWO warps issue the MMAs, alternating tiles on the two TMEM accumulators.  One thread issues a
-// 128 x 64 x 16 tcgen05.mma every ~90 cycles in this loop while the tensor core needs 32 (tools/microbench/umma_rate.cu), and
-// with the weight ring gone the two issuers only share the halo buffers, one per tile.
+// ResNet layer1: 72 KB): no weight ring, the producer only streams halo boxes.
 template <int BN, bool kRW>
 __global__ void __launch_bounds__(kHThreads, 1)
     conv3x3_halo_kernel(const __grid_constant__ HaloMaps maps, const HaloParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int kWStage = BN * 128;
-  constexpr uint32_t kTmemCols = (2 * BN <= 128) ? 128 : (2 * BN <= 256 ? 256 : 512);
   constexpr int kChunksPerWarp = BN / 64;
   uint8_t* a_ring = smem;
   uint8_t* w_ring = a_ring + p.a_bufs * p.a_buf_bytes;                // kRW: 9 * cblocks resident tiles, tap-major
   uint8_t* out_stage = w_ring + (kRW ? 9 * p.cblocks : p.w_stages) * kWStage;                 // BN/64 slabs
-  float* sb = reinterpret_cast<float*>(out_stage + (BN / 64) * kSlabBytes);   // [scale | bias][BN]
+  uint8_t* acc_xpose = out_stage + (BN / 64) * kSlabBytes;                  // [8 warps] accumulator transposes
+  float* sb = reinterpret_cast<float*>(acc_xpose + 8 * kAccXposeWarpBytes);   // [scale | bias][BN]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sb + 2 * BN);
   uint64_t* a_full = bars;          // [4]
   uint64_t* a_empty = bars + 4;     // [4]
   uint64_t* w_full = bars + 8;      // [8]
   uint64_t* w_empty = bars + 16;    // [8]
-  uint64_t* t_full = bars + 24;     // [2]
-  uint64_t* t_empty = bars + 26;    // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 28);
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&maps.a);
     tma_prefetch_desc(&maps.w);
     tma_prefetch_desc(&maps.out);
   }
-  if (warp == 1 && lane == 0) {
+  if (warp == 0 && lane == 0) {
     for (int s = 0; s < p.a_bufs; ++s) {
       mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_empty[s], 8);   // one arrive per consumer warp
     }
     for (int s = 0; s < (kRW ? 1 : p.w_stages); ++s) {
       mbar_init(&w_full[s], 1);
-      mbar_init(&w_empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&t_full[b], 1);
-      mbar_init(&t_empty[b], 8);
+      mbar_init(&w_empty[s], 8);
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc<1>(tmem_slot, kTmemCols);
-    tmem_relinquish<1>();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================================== TMA producer =====================================
     // (whole warp walks the loop, one elected lane issues: see conv_gemm.cu)
     {
-      uint32_t ai = 0, wi = 0;
       PipeState as(p.a_bufs), ws(kRW ? 1 : p.w_stages);
       if constexpr (kRW) {   // every filter tap once
         if (elect_one()) {
           mbar_arrive_expect_tx(&w_full[0], 9 * p.cblocks * kWStage);
           for (int t = 0; t < 9 * p.cblocks; ++t)
-            tma_load_2d<1>(w_ring + t * kWStage, &maps.w, &w_full[0], t * kHK, 0, kEvictLast);
+            tma_load_2d(w_ring + t * kWStage, &maps.w, &w_full[0], t * kHK, 0, kEvictLast);
         }
         __syncwarp();
       }
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         const int b = tile / p.tiles_per_img;
         const int p0 = (tile - b * p.tiles_per_img) * p.R;
-        for (int cb = 0; cb < p.cblocks; ++cb, ++ai, as.next()) {
+        for (int cb = 0; cb < p.cblocks; ++cb, as.next()) {
           const uint32_t sa = as.s, pha = as.ph;
           mbar_wait(&a_empty[sa], pha ^ 1);
           if (elect_one()) {
-            if ((kHaloTimingMode & 2) && ai >= static_cast<uint32_t>(p.a_bufs)) {
-              mbar_arrive(&a_full[sa]);    // timing experiment: reuse stale halo data, no load
-            } else {
-              mbar_arrive_expect_tx(&a_full[sa], p.halo_bytes);
-              // rows p0-1 .. p0+R, columns -1 .. W: everything outside the image arrives as zeros (the padding)
-              tma_load_4d(a_ring + sa * p.a_buf_bytes, &maps.a, &a_full[sa], cb * kHK, -1, p0 - 1, b, kEvictNormal);
-            }
+            mbar_arrive_expect_tx(&a_full[sa], p.halo_bytes);
+            // rows p0-1 .. p0+R, columns -1 .. W: everything outside the image arrives as zeros (the padding)
+            tma_load_4d(a_ring + sa * p.a_buf_bytes, &maps.a, &a_full[sa], cb * kHK, -1, p0 - 1, b, kEvictNormal);
           }
           __syncwarp();
           if constexpr (kRW) continue;
-          for (int tap = 0; tap < 9; ++tap, ++wi, ws.next()) {
+          for (int tap = 0; tap < 9; ++tap, ws.next()) {
             const uint32_t sw = ws.s, phw = ws.ph;
             mbar_wait(&w_empty[sw], phw ^ 1);
             if (elect_one()) {
-              if ((kHaloTimingMode & 1) && wi >= static_cast<uint32_t>(p.w_stages)) {
-                mbar_arrive(&w_full[sw]);  // timing experiment: stale weights, no load
-              } else {
-                mbar_arrive_expect_tx(&w_full[sw], kWStage);
-                tma_load_2d<1>(w_ring + sw * kWStage, &maps.w, &w_full[sw], (tap * p.cblocks + cb) * kHK, 0, kEvictLast);
-              }
+              mbar_arrive_expect_tx(&w_full[sw], kWStage);
+              tma_load_2d(w_ring + sw * kWStage, &maps.w, &w_full[sw], (tap * p.cblocks + cb) * kHK, 0, kEvictLast);
             }
             __syncwarp();
           }
         }
       }
     }
-  } else if (warp == 1 || (kRW && warp == 10)) {
-    // ===================================== MMA issuer(s) =====================================
-    {
-      constexpr uint32_t idesc = umma_idesc_bf16(kHM, BN);
-      const uint32_t issuer = (warp == 1) ? 0u : 1u;
-      uint32_t tc = 0;
-      PipeState as(p.a_bufs), ws(kRW ? 1 : p.w_stages);
-      const uint64_t da0 = umma_desc_sw128(smem_u32(a_ring));
-      const uint64_t db0 = umma_desc_sw128(smem_u32(w_ring));
-      const uint32_t row_step = static_cast<uint32_t>(p.Wp) * 8u;   // one padded image row in 16-byte units (128 B / pixel)
-      if constexpr (kRW) {
-        mbar_wait(&w_full[0], 0);
-        tc_fence_after();
-      }
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tc) {
-        const uint32_t buf = tc & 1;
-        if (kRW && buf != issuer) {   // the other issuer's tile: only keep the halo ring position in step
-          for (int cb = 0; cb < p.cblocks; ++cb) as.next();
-          continue;
-        }
-        mbar_wait(&t_empty[buf], ((tc >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + buf * BN;
-        uint32_t accumulate = 0;
-        for (int cb = 0; cb < p.cblocks; ++cb, as.next()) {
-          const uint32_t sa = as.s;
-          mbar_wait(&a_full[sa], as.ph);
-          tc_fence_after();
-          const uint64_t da_buf = da0 + static_cast<uint64_t>(sa * (p.a_buf_bytes >> 4));
-#pragma unroll
-          for (int r = 0; r < 3; ++r) {
-#pragma unroll
-            for (int s = 0; s < 3; ++s) {
-              uint32_t sw = 0;
-              if constexpr (!kRW) {
-                sw = ws.s;
-                mbar_wait(&w_full[sw], ws.ph);
-                tc_fence_after();
-              } else {
-                sw = static_cast<uint32_t>((r * 3 + s) * p.cblocks + cb);   // resident tile of this (tap, channel block)
-              }
-              // the tap's view of the halo block: same buffer, start shifted by r padded rows + s pixels (128 B each)
-              const uint64_t da = da_buf + static_cast<uint64_t>(r * row_step + s * 8);
-              const uint64_t db = db0 + static_cast<uint64_t>(sw * (kWStage >> 4));
-              if (elect_one()) {
-#pragma unroll
-                for (int k = 0; k < kHK / 16; ++k) umma_f16<1>(tmem_d, da + 2 * k, db + 2 * k, idesc, accumulate | k);
-                if constexpr (!kRW) umma_commit<1>(&w_empty[sw]);
-                if (r == 2 && s == 2) {
-                  umma_commit<1>(&a_empty[sa]);
-                  if (cb == p.cblocks - 1) umma_commit<1>(&t_full[buf]);
-                }
-              }
-              __syncwarp();
-              accumulate = 1;
-              if constexpr (!kRW) ws.next();
-            }
-          }
-        }
-      }
-    }
-  } else if (warp < 10) {
-    // ===================================== epilogue warps =====================================
-    const uint32_t ewarp = warp - 2;
+  } else {
+    // ===================================== consumer warpgroups =====================================
+    const uint32_t ewarp = warp;
     const uint32_t quad = warp & 3;
-    const uint32_t half = ewarp >> 2;
+    const uint32_t half = ewarp >> 2;                    // column half of the tile (= warpgroup)
     const uint32_t m = quad * 32 + lane;                 // padded-raster position of this thread's accumulator row
     const uint32_t etid = ewarp * 32 + lane;
-    const uint32_t tmem_row = tmem_base + ((quad * 32u) << 16);
+    const uint32_t xacc = smem_u32(acc_xpose) + warp * kAccXposeWarpBytes;
+    const uint32_t a_base = smem_u32(a_ring);
+    const uint32_t w_base = smem_u32(w_ring) + half * (BN / 2) * 128;
+    const uint32_t row_bytes = static_cast<uint32_t>(p.Wp) * 128u;   // one padded image row (128 B per pixel)
+    PipeState as(p.a_bufs), ws(kRW ? 1 : p.w_stages);
+    if constexpr (kRW) mbar_wait(&w_full[0], 0);
     const int pl = static_cast<int>(m) / p.Wp, ql = static_cast<int>(m) - pl * p.Wp;
     const bool valid = ql < p.W && pl < p.R;
     const uint32_t srow = static_cast<uint32_t>(pl * p.W + ql);          // row of the compact [R x W] staging box
@@ -245,27 +158,50 @@ __global__ void __launch_bounds__(kHThreads, 1)
       st_shared_f32(sb_addr + c * 4, (p.scale && c < p.N) ? p.scale[c] : 1.f);
       st_shared_f32(sb_addr + (BN + c) * 4, (p.bias && c < p.N) ? p.bias[c] : 0.f);
     }
-    uint32_t tc = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tc) {
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const int b = tile / p.tiles_per_img;
       const int p0 = (tile - b * p.tiles_per_img) * p.R;
-      const uint32_t buf = tc & 1;
       if (etid == 0) tma_store_wait_read_();     // the previous tile's store has finished reading the staging box
       asm volatile("bar.sync 1, 256;" ::: "memory");   // (also orders the scale/bias staging before its first use)
-      mbar_wait(&t_full[buf], (tc >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_row + buf * BN;
+      // main loop: per channel block one halo box, nine taps = nine start addresses into it
+      WgAcc<BN / 2> acc;
+      uint32_t accumulate = 0;
+      for (int cb = 0; cb < p.cblocks; ++cb, as.next()) {
+        const uint32_t sa = as.s;
+        mbar_wait(&a_full[sa], as.ph);
+        const uint32_t a_buf = a_base + sa * p.a_buf_bytes;
 #pragma unroll 1
+        for (int tap = 0; tap < 9; ++tap) {
+          const int r = tap / 3, s = tap - 3 * r;
+          uint32_t sw = 0;
+          if constexpr (!kRW) {
+            sw = ws.s;
+            mbar_wait(&w_full[sw], ws.ph);
+          } else {
+            sw = static_cast<uint32_t>(tap * p.cblocks + cb);   // resident tile of this (tap, channel block)
+          }
+          // the tap's view of the halo block: same buffer, start shifted by r padded rows + s pixels (128 B each)
+          const uint32_t a_addr = a_buf + r * row_bytes + s * 128u;
+          const uint32_t b_addr = w_base + sw * kWStage;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kHK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), accumulate | k);
+          wgmma_commit();
+          wgmma_wait<0>();
+          accumulate = 1;
+          if constexpr (!kRW) {
+            if (lane == 0) mbar_arrive(&w_empty[sw]);
+            ws.next();
+          }
+        }
+        if (lane == 0) mbar_arrive(&a_empty[sa]);
+      }
+      acc.fence_regs();
+#pragma unroll
       for (int ci = 0; ci < kChunksPerWarp; ++ci) {
         const int ch = half * kChunksPerWarp + ci;
         uint32_t r[32];
-        tmem_ld_32x32(taddr + ch * 32, r);
-        tmem_ld_wait_regs(r);
-        if (ci == kChunksPerWarp - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&t_empty[buf]);
-        }
+        acc.rows32(ci, r, xacc, lane);
         if (ch * 32 >= p.N) continue;   // warp-uniform
         float y[32];
 #pragma unroll
@@ -305,15 +241,12 @@ __global__ void __launch_bounds__(kHThreads, 1)
     if (etid == 0) tma_store_wait_all_();
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<1>(tmem_base, kTmemCols);
 }
 
 template <int BN, bool kRW>
 int launch_halo(const HaloMaps& maps, HaloParams& p, int num_sms, size_t max_smem, cudaStream_t stream) {
   constexpr size_t kWStage = static_cast<size_t>(BN) * 128;
-  const size_t fixed = 1024 + static_cast<size_t>(BN / 64) * kSlabBytes + 2 * BN * 4 + 256;
+  const size_t fixed = 1024 + static_cast<size_t>(BN / 64) * kSlabBytes + 8 * kAccXposeWarpBytes + 2 * BN * 4 + 256;
   const size_t abuf = p.a_buf_bytes;
   size_t smem = 0;
   if constexpr (kRW) {
@@ -382,7 +315,7 @@ int conv3x3_halo(const ConvGemmDesc& d, cudaStream_t stream) {
   const int ktot = 9 * p.cblocks * 64;
   if (int rc = make_tmap_2d_bf16(&maps.w, d.weight, d.N, ktot, ktot, BN, 64)) return rc;
   if (int rc = make_tmap_nhwc_box_bf16(&maps.out, d.out, d.B, d.H, d.W, d.ld_out, d.ld_out, d.W, p.R)) return rc;
-  // all taps resident + two MMA issuers when the weights are small (ResNet layer1: 9 x [64 x 64] = 72 KB)
+  // all taps resident when the weights are small (ResNet layer1: 9 x [64 x 64] = 72 KB)
   const bool resident = BN == 64 && static_cast<size_t>(9) * p.cblocks * BN * 128 <= 80 * 1024 && !tuning_flag("DCR_HALO_NO_RESIDENT");
   if (BN == 64) return resident ? launch_halo<64, true>(maps, p, di->num_sms, di->max_smem_optin, stream)
                                 : launch_halo<64, false>(maps, p, di->num_sms, di->max_smem_optin, stream);

@@ -1,4 +1,4 @@
-// tcgen05 GEMM / implicit-GEMM convolution with fused epilogue (sm_100a).
+// wgmma GEMM / implicit-GEMM convolution with fused epilogue (sm_90a).
 //
 // One kernel family computes   Y[m, n] = act( scale[n] * sum_k A[m, k] * W[n, k] + bias[n] (+ R[m, n]) )
 // for every dense contraction of the descriptor networks:
@@ -12,13 +12,14 @@
 //
 // Precision: operands are bf16 "planes".  Fast mode uses one plane (plain bf16 x bf16 -> fp32).  Parity mode
 // stores every activation / weight as 2-3 bf16 planes (hi, mid, lo with x = hi + mid + lo to ~2^-24) and
-// accumulates the listed cross terms into the same TMEM accumulator, which reproduces fp32 arithmetic on the
+// accumulates the listed cross terms into the same register accumulator, which reproduces fp32 arithmetic on the
 // tensor cores (DESIGN.md section 5).
 //
-// Structure per CTA (192 threads, persistent over output tiles of 128 x BN):
-//   warp 0 : TMA producer (A tile 128x64, W tile BNx64 per stage, 128B swizzle)
-//   warp 1 : tcgen05.mma issuer (cta_group::1, UMMA 128 x BN x 16), accumulators double-buffered in TMEM
-//   warps 2-5 : epilogue (tcgen05.ld -> scale/bias/residual/activation -> bf16 planes / fp32 -> global)
+// Structure per CTA (288 threads, persistent over output tiles of 128 x BN):
+//   warps 0-7 : two consumer warpgroups; warpgroup h issues the wgmma for columns [h BN/2, (h+1) BN/2) of the tile
+//               (two m64 x BN/2 x k16 per k16 step, fp32 accumulators in registers) and runs the epilogue of those
+//               columns (scale/bias/residual/activation -> bf16 planes / fp32 -> global)
+//   warp 8    : TMA producer (A tile 128x64, W tile BNx64 per stage, 128B swizzle)
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -34,14 +35,9 @@ namespace {
 
 constexpr int kBM = 128;
 constexpr int kBK = 64;
-constexpr int kThreads = 320;   // warp 0 TMA, warp 1 MMA, warps 2-9 epilogue
+constexpr int kThreads = 288;   // warps 0-7 MMA + epilogue (two warpgroups), warp 8 TMA
+constexpr int kAccXposeBytes = 8 * kAccXposeWarpBytes;
 constexpr int kAStage = kBM * kBK * 2;   // 16 KB
-// Timing experiments (results are garbage), compile-time only: 1 = loads only (no MMA, no epilogue), 2 = loads only and
-// every im2col request replaced by a tiled request of the same size (row-shifted view).
-#ifndef DCR_GEMM_TIMING_MODE
-#define DCR_GEMM_TIMING_MODE 0
-#endif
-constexpr int kGemmTimingMode = DCR_GEMM_TIMING_MODE;
 // direct epilogue: per epilogue warp a [32 rows][64 B + 16 B pad] buffer through which the bf16 planes are transposed, so that
 // one warp instruction touches 8 rows x 64 contiguous bytes of global memory instead of 32 rows x 16 bytes
 constexpr int kXposePitch = 80;
@@ -53,7 +49,6 @@ struct GemmMaps {
   CUtensorMap w[3];
   CUtensorMap out;   // TMA-store epilogue (single-plane bf16 output)
   CUtensorMap res;   // residual tile loads for that epilogue
-  CUtensorMap a_flat; // timing experiment DCR_GEMM_DEBUG=2 only: the im2col input viewed as a plain [pixels, C] matrix
 };
 
 struct GemmParams {
@@ -86,8 +81,8 @@ struct GemmParams {
 };
 
 // exact-erf GELU of the tensor-core epilogues: erf by Abramowitz-Stegun 7.1.26 (|error| <= 2e-7 absolute: below the bf16
-// rounding of a stored activation and at the level of the split-bf16 modes' own accumulation error) -- about half the instructions of erff(), whose two-branch evaluation made
-// the fc1 + GELU layers of the ViTs ALU bound in their epilogue (129 us at 461 TFLOP/s for 50k x 1536 x 384).
+// rounding of a stored activation and at the level of the split-bf16 modes' own accumulation error) -- about half the instructions of erff(), whose two-branch evaluation makes
+// the fc1 + GELU layers of the ViTs ALU bound in their epilogue.
 DCR_DEVICE float gelu_erf_fast(float y) {
   const float ax = fabsf(y) * 0.70710678118654752440f;
   float t;
@@ -106,7 +101,7 @@ DCR_DEVICE float gelu_erf_fast(float y) {
 // five FMA-pipe instructions and one MUFU per element.  It differs from the erf form by <= 4.7e-4 absolute (the form itself) plus
 // <= 5e-4 |y| / 2 (tanh.approx.f32), below the bf16 rounding of the stored activation (2^-9 relative) for every |y| >= 0.1 and
 // within two bf16 ulps below that.  The erf polynomial above costs 16 instructions and TWO MUFU ops per element: over a 128 x 256
-// tile that is 4096 MUFU cycles against 3072 MMA cycles, which made fc1 + GELU epilogue bound (95 us at 627 TFLOP/s on ViT-S/16).
+// tile that is 4096 MUFU cycles against 3072 MMA cycles, which makes fc1 + GELU epilogue bound.
 // The split-bf16 (fp32-level) modes and the float64 mode keep the erf forms.
 DCR_DEVICE float gelu_tanh_fast(float y) {
   const float u = y * y;
@@ -129,15 +124,6 @@ DCR_DEVICE uint32_t pack_bf16(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&p);
 }
 
-DCR_DEVICE void tmem_ld_wait_dep32(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]),
-                 "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]),
-                 "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]),
-                 "+r"(r[29]), "+r"(r[30]), "+r"(r[31])::"memory");
-}
-
 DCR_DEVICE void tma_store_2d(const void* tmap, const void* src_smem, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(tmap)),
@@ -146,38 +132,27 @@ DCR_DEVICE void tma_store_2d(const void* tmap, const void* src_smem, int c0, int
 }
 DCR_DEVICE void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 DCR_DEVICE void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-DCR_DEVICE void tma_store_wait_read_1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 DCR_DEVICE void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // kEpi: 0 = direct epilogue (any number of planes, optional fp32 output, runtime activation; parity mode and final
 //           layers), 1/2/3/4 = TMA-store epilogue with compile-time activation none / ReLU / GELU / QuickGELU (fast mode hot path).
-// Eight epilogue warps: warps w and w+4 share a TMEM lane quadrant and split the tile's columns, so every SM
-// sub-partition has two epilogue warps to switch between (the epilogue is latency bound, not issue bound).
-//
-// kCG == 2: two CTAs of a cluster (a TPC's SM pair) work one 256 x BN tile with UMMA 256 x BN x 16 (cta_group::2): each CTA
-// loads its own 128 A rows and HALF of the W tile (BN/2 rows), the leader CTA issues the MMAs for both, each CTA's TMEM
-// holds the accumulators of its own 128 rows and each runs its own epilogue.  Per CTA and k-block that is 16 KB + BN*64 B
-// through the L2 -> shared-memory port instead of 16 KB + BN*128 B, and 4 KB + BN*16 B of operand reads per UMMA instead of
-// 4 KB + BN*32 B -- the two resources the 128-wide single-CTA tiles are short of (DESIGN.md section 5d).  Plain (1x1 /
-// Linear) single-term GEMMs with the TMA-store epilogue only; no A-resident mode.
-template <int BN, bool kIm2col, int kEpi, int kCG>
+// Eight MMA + epilogue warps: warps w and w+4 own the same 32 rows and split the tile's columns, so every SM
+// sub-partition has two warps to switch between (the epilogue is latency bound, not issue bound).
+template <int BN, bool kIm2col, int kEpi>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm_bf16_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
-  static_assert(kCG == 1 || (!kIm2col && kEpi != 0), "the CTA-pair form covers plain GEMMs with the TMA-store epilogue");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr bool kTma = kEpi != 0;
-  constexpr int kBRows = BN / kCG;          // W rows this CTA loads per stage
-  constexpr int kBStage = kBRows * kBK * 2;
+  constexpr int kBStage = BN * kBK * 2;
   constexpr int kStageBytes = kAStage + kBStage;
-  constexpr uint32_t kTmemCols = (2 * BN <= 128) ? 128 : (2 * BN <= 256 ? 256 : 512);
   constexpr int kStagingBytes = (BN / 64) * kBM * 128;   // BN/64 slabs of [128 rows x 64 bf16], 128B swizzle
   constexpr int kChunksPerWarp = BN / 64;                // 32-column chunks each epilogue warp handles per tile
   const int stages = p.stages;
   const int k_iters = p.n_terms * p.taps * p.cblocks;
   // A-resident mode (wide 1x1 convolutions / Linear layers with small K): [k_iters x 16 KB A rows of the current m-tile]
   // first, then stages that carry only the W tile; the per-channel affine of ALL column blocks is staged once.
-  const bool a_res = (kCG == 1) && p.a_resident != 0;
+  const bool a_res = p.a_resident != 0;
   const int stage_bytes = a_res ? kBStage : kStageBytes;
   const int num_n_tiles = p.num_n_tiles;
   uint8_t* smem_ares = smem;
@@ -185,14 +160,12 @@ __global__ void __launch_bounds__(kThreads, 1)
   uint8_t* out_stage = smem_ab + stages * stage_bytes;                      // n_out_bufs tiles, 1024-aligned
   // direct epilogue (kEpi == 0): no staging tiles; one 32-row x 64-byte transpose buffer per epilogue warp instead
   uint8_t* res_stage = out_stage + (kTma ? p.n_out_bufs * kStagingBytes : kXposeBytes);   // n_res_bufs tiles
-  float* sb = reinterpret_cast<float*>(res_stage + p.n_res_bufs * kStagingBytes);   // [2 bufs][2 (scale,bias)][BN] | a_res: [2][n_tiles*BN]
+  uint8_t* acc_xpose = res_stage + p.n_res_bufs * kStagingBytes;   // [8 warps] accumulator transpose buffers
+  float* sb = reinterpret_cast<float*>(acc_xpose + kAccXposeBytes);   // [2 bufs][2 (scale,bias)][BN] | a_res: [2][n_tiles*BN]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sb + (a_res ? 2 * num_n_tiles * BN : 4 * BN));
   uint64_t* full = bars;          // [stages] (<= 12)
   uint64_t* empty = bars + 12;    // [stages]
-  uint64_t* t_full = bars + 24;   // [2]
-  uint64_t* t_empty = bars + 26;  // [2]
   uint64_t* res_full = bars + 28;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 30);
   uint64_t* a_full = bars + 10;    // A-resident mode (stages <= 8, so full[10..11] are free)
   uint64_t* a_empty = bars + 11;
 
@@ -200,24 +173,19 @@ __global__ void __launch_bounds__(kThreads, 1)
   // hoist everything the tile loops need out of the constant bank once
   const int M = p.M, N = p.N, num_m_tiles = p.num_m_tiles;
   const bool has_res = p.res != nullptr;
-  // CTA pair: tiles are 2 m-tiles tall, the pair (cluster) is the scheduling unit and CTA rank r works m-tile 2*pm + r (an
-  // odd last m-tile leaves rank 1 a tile past M: its loads are zero filled, its stores skipped)
-  const uint32_t cta_rank = (kCG == 2) ? cluster_ctarank() : 0;
-  const bool leader = cta_rank == 0;
-  const int pair_m_tiles = (num_m_tiles + kCG - 1) / kCG;
-  const int num_tiles = pair_m_tiles * p.num_n_tiles;
-  const int unit = static_cast<int>(blockIdx.x) / kCG, n_units = static_cast<int>(gridDim.x) / kCG;
+  const int num_tiles = num_m_tiles * p.num_n_tiles;
+  const int unit = static_cast<int>(blockIdx.x), n_units = static_cast<int>(gridDim.x);
   // tile sequence of this CTA: m-fastest round robin (default) or a contiguous range of the n-fastest order (A-resident)
   const int t_first = a_res ? static_cast<int>(static_cast<long long>(num_tiles) * blockIdx.x / gridDim.x) : unit;
   const int t_end = a_res ? static_cast<int>(static_cast<long long>(num_tiles) * (blockIdx.x + 1) / gridDim.x) : num_tiles;
   const int t_step = a_res ? 1 : n_units;
   const bool n_fast = p.n_fastest != 0;
   auto tile_m = [&](int t) {
-    return a_res ? t / num_n_tiles : ((n_fast ? t / num_n_tiles : t % pair_m_tiles) * kCG + static_cast<int>(cta_rank));
+    return a_res ? t / num_n_tiles : (n_fast ? t / num_n_tiles : t % num_m_tiles);
   };
-  auto tile_n = [&](int t) { return (a_res || n_fast) ? t % num_n_tiles : t / pair_m_tiles; };
+  auto tile_n = [&](int t) { return (a_res || n_fast) ? t % num_n_tiles : t / num_m_tiles; };
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&maps.out);
     tma_prefetch_desc(&maps.res);
     for (int i = 0; i < 3; ++i) {
@@ -225,35 +193,21 @@ __global__ void __launch_bounds__(kThreads, 1)
       tma_prefetch_desc(&maps.w[i]);
     }
   }
-  if (warp == 1 && lane == 0) {
+  if (warp == 0 && lane == 0) {
     for (int s = 0; s < stages; ++s) {
-      mbar_init(&full[s], kCG);        // pair: the leader's barrier takes one arrive per CTA and both CTAs' bytes
-      mbar_init(&empty[s], 1);         // pair: tcgen05.commit multicasts the arrive to both CTAs
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);         // one arrive per consumer warp once its wgmma on the stage have completed
     }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&t_full[b], 1);
-      mbar_init(&t_empty[b], 8 * kCG);   // pair: the leader's MMA warp waits for both CTAs' epilogue warps
-      mbar_init(&res_full[b], 1);
-    }
+    for (int b = 0; b < 2; ++b) mbar_init(&res_full[b], 1);
     mbar_init(a_full, 1);
-    mbar_init(a_empty, 1);
+    mbar_init(a_empty, 8);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc<kCG>(tmem_slot, kTmemCols);
-    tmem_relinquish<kCG>();
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (kCG == 2) cluster_sync();   // the peer's barriers are initialised before any remote arrive / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // Producer and MMA roles: the WHOLE warp walks the loops (so that every value is provably warp-uniform and lives
-  // in uniform registers) and one elected lane issues the TMA / tcgen05 instructions.  Running the loops under
-  // `if (lane == 0)` makes the compiler wrap every UTMALDG / UTCHMMA in an ELECT + R2UR.BROADCAST + BRA.U.ANY loop
-  // (8-20 extra instructions each) -- and the single-thread instruction stream IS the pipeline's critical path.
-  if (warp == 0) {
+  // Producer: the WHOLE warp walks the loops (so that every value is provably warp-uniform and lives in uniform
+  // registers) and one elected lane issues the TMA instructions.
+  if (warp == 8) {
     {
       const int n_terms = p.n_terms, taps = p.taps, kw = p.kw, cblocks = p.cblocks;
       PipeState st(stages);
@@ -269,7 +223,7 @@ __global__ void __launch_bounds__(kThreads, 1)
             if (elect_one()) {
               mbar_arrive_expect_tx(a_full, k_iters * kAStage);
               for (int ki = 0; ki < k_iters; ++ki)
-                tma_load_2d<1>(smem_ares + ki * kAStage, &maps.a[p.term_a[0]], a_full, ki * kBK, m0, kEvictFirst);
+                tma_load_2d(smem_ares + ki * kAStage, &maps.a[p.term_a[0]], a_full, ki * kBK, m0, kEvictFirst);
             }
             __syncwarp();
             ++a_seg;
@@ -279,7 +233,7 @@ __global__ void __launch_bounds__(kThreads, 1)
             mbar_wait(&empty[s], st.ph ^ 1);
             if (elect_one()) {
               mbar_arrive_expect_tx(&full[s], kBStage);
-              tma_load_2d<1>(smem_ab + s * kBStage, &maps.w[p.term_w[0]], &full[s], ki * kBK, n0, kEvictLast);
+              tma_load_2d(smem_ab + s * kBStage, &maps.w[p.term_w[0]], &full[s], ki * kBK, n0, kEvictLast);
             }
             __syncwarp();
           }
@@ -303,19 +257,14 @@ __global__ void __launch_bounds__(kThreads, 1)
               const uint32_t s = st.s, ph = st.ph;
               mbar_wait(&empty[s], ph ^ 1);
               if (elect_one()) {
-                if (leader) mbar_arrive_expect_tx(&full[s], kStageBytes * kCG);
-                else mbar_arrive_cluster(&full[s], 0);
+                mbar_arrive_expect_tx(&full[s], kStageBytes);
                 uint8_t* sa = smem_ab + s * kStageBytes;
                 if constexpr (kIm2col) {
-                  if constexpr (kGemmTimingMode == 2)
-                    tma_load_2d<1>(sa, &maps.a_flat, &full[s], cb * kBK, max(0, m0 + (r - 1) * p.Q + sx - 1), kEvictNormal);
-                  else
-                    tma_load_im2col_4d<1>(sa, ma, &full[s], cb * kBK, w0, h0, img, static_cast<uint16_t>(sx),
+                  tma_load_im2col_4d(sa, ma, &full[s], cb * kBK, w0, h0, img, static_cast<uint16_t>(sx),
                                           static_cast<uint16_t>(r));
                 } else
-                  tma_load_2d<kCG>(sa, ma, &full[s], cb * kBK, m0, kEvictNormal);
-                tma_load_2d<kCG>(sa + kAStage, mw, &full[s], (tap * cblocks + cb) * kBK, n0 + static_cast<int>(cta_rank) * kBRows,
-                                 kEvictNormal);
+                  tma_load_2d(sa, ma, &full[s], cb * kBK, m0, kEvictNormal);
+                tma_load_2d(sa + kAStage, mw, &full[s], (tap * cblocks + cb) * kBK, n0, kEvictNormal);
               }
               __syncwarp();
             }
@@ -323,71 +272,20 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    if (leader) {
-      constexpr uint32_t idesc = umma_idesc_bf16(kBM * kCG, BN);
-      uint32_t tc = 0;
-      PipeState st(stages);
-      // descriptors of stage 0; stage s adds s * kStageBytes to the 16-byte-granular start-address field (no carry out
-      // of the field: shared memory addresses stay below 256 KB)
-      const uint64_t da0 = umma_desc_sw128(smem_u32(a_res ? smem_ares : smem_ab));
-      const uint64_t db0 = umma_desc_sw128(smem_u32(a_res ? smem_ab : smem_ab + kAStage));
-      const uint32_t a_step = a_res ? (kAStage >> 4) : (kStageBytes >> 4);     // A: per k-iteration (resident) / per stage
-      const uint32_t b_step = static_cast<uint32_t>(stage_bytes) >> 4;
-      int res_m = -1;
-      uint32_t a_seg = 0;
-      for (int tile = t_first; tile < t_end; tile += t_step, ++tc) {
-        const uint32_t buf = tc & 1;
-        bool last_of_m = false;
-        if (a_res) {
-          const int m = tile_m(tile);
-          if (m != res_m) {
-            res_m = m;
-            mbar_wait(a_full, a_seg & 1);
-            tc_fence_after();
-            ++a_seg;
-          }
-          last_of_m = (tile + 1 >= t_end) || tile_m(tile + 1) != m;
-        }
-        if constexpr (kGemmTimingMode != 0) {   // loads only: hand every stage straight back to the producer
-          for (int ki = 0; ki < k_iters; ++ki, st.next()) {
-            mbar_wait(&full[st.s], st.ph);
-            if (elect_one()) mbar_arrive(&empty[st.s]);
-            __syncwarp();
-          }
-          continue;
-        }
-        mbar_wait(&t_empty[buf], ((tc >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + buf * BN;
-        for (int ki = 0; ki < k_iters; ++ki, st.next()) {
-          const uint32_t s = st.s;
-          mbar_wait(&full[s], st.ph);
-          tc_fence_after();
-          const uint64_t da = da0 + static_cast<uint64_t>((a_res ? static_cast<uint32_t>(ki) : s) * a_step);
-          const uint64_t db = db0 + static_cast<uint64_t>(s * b_step);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < kBK / 16; ++k) umma_f16<kCG>(tmem_d, da + 2 * k, db + 2 * k, idesc, (ki | k) != 0);
-            umma_commit<kCG>(&empty[s]);
-            if (ki == k_iters - 1) {
-              umma_commit<kCG>(&t_full[buf]);
-              if (last_of_m) umma_commit<kCG>(a_empty);
-            }
-          }
-          __syncwarp();
-        }
-      }
-    }
   } else {
-    const uint32_t ewarp = warp - 2;               // 0..7
-    const uint32_t quad = warp & 3;                // TMEM lane quadrant
-    const uint32_t half = ewarp >> 2;              // which half of the tile's columns
+    const uint32_t ewarp = warp;                   // 0..7
+    const uint32_t quad = warp & 3;                // rows quad*32 .. +31 of the tile
+    const uint32_t half = ewarp >> 2;              // which half of the tile's columns (= warpgroup)
     const uint32_t row = quad * 32 + lane;
-    const uint32_t etid = ewarp * 32 + lane;       // 0..255 among the epilogue threads
-    const uint32_t tmem_row = tmem_base + ((quad * 32u) << 16);
+    const uint32_t etid = ewarp * 32 + lane;       // 0..255 among the consumer threads
+    const uint32_t xacc = smem_u32(acc_xpose) + warp * kAccXposeWarpBytes;
     const int act = p.act;
     uint32_t tc = 0;
+    PipeState st(stages);
+    const uint32_t a_base = smem_u32(a_res ? smem_ares : smem_ab);
+    const uint32_t b_base = smem_u32(a_res ? smem_ab : smem_ab + kAStage) + half * (BN / 2) * 128;
+    int res_m_c = -1;
+    uint32_t a_seg = 0;
     auto load_residual = [&](int tile_idx, uint32_t rbuf) {   // one thread: residual tile -> res_stage[rbuf]
       const int rm0 = tile_m(tile_idx) * kBM;
       const int rn0 = tile_n(tile_idx) * BN;
@@ -397,10 +295,10 @@ __global__ void __launch_bounds__(kThreads, 1)
       mbar_arrive_expect_tx(&res_full[rbuf], slabs * kBM * 128);
       for (int sl = 0; sl < BN / 64; ++sl)
         if (rn0 + sl * 64 < N)
-          tma_load_2d<1>(res_stage + rbuf * kStagingBytes + sl * kBM * 128, &maps.res, &res_full[rbuf], rn0 + sl * 64, rm0,
+          tma_load_2d(res_stage + rbuf * kStagingBytes + sl * kBM * 128, &maps.res, &res_full[rbuf], rn0 + sl * 64, rm0,
                          kEvictFirst);
     };
-    if (kTma && has_res && etid == 0 && t_first < t_end && kGemmTimingMode == 0) load_residual(t_first, 0);
+    if (kTma && has_res && etid == 0 && t_first < t_end) load_residual(t_first, 0);
     const bool two_out = p.n_out_bufs == 2;
     const uint32_t sb_addr = smem_u32(sb), out_addr = smem_u32(out_stage), res_addr = smem_u32(res_stage);
     int staged_n0 = -1;
@@ -413,10 +311,9 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
     }
-    for (int tile = t_first; tile < t_end && kGemmTimingMode == 0; tile += t_step, ++tc) {
+    for (int tile = t_first; tile < t_end; tile += t_step, ++tc) {
       const int m0 = tile_m(tile) * kBM;
       const int n0 = tile_n(tile) * BN;
-      const uint32_t buf = tc & 1;
       uint8_t* ostage = out_stage + (two_out ? (tc & 1) : 0) * kStagingBytes;
       const uint32_t ostage_addr = out_addr + (two_out ? (tc & 1) : 0) * kStagingBytes;
       const uint32_t rstage_addr = res_addr + (tc & 1) * kStagingBytes;
@@ -445,26 +342,47 @@ __global__ void __launch_bounds__(kThreads, 1)
       if (restage || (kTma && !two_out)) asm volatile("bar.sync 1, 256;" ::: "memory");
       const uint32_t s_scale = a_res ? sb_addr + n0 * 4 : sb_addr + sbsel * 2 * BN * 4;
       const uint32_t s_bias = s_scale + (a_res ? num_n_tiles * BN : BN) * 4;
-      mbar_wait(&t_full[buf], (tc >> 1) & 1);
-      tc_fence_after();
+      // ---- main loop: this warpgroup's 128 x BN/2 accumulator over all k-iterations.  The stage of k-iteration i is
+      // released once wgmma_wait<1> in iteration i+1 has seen its MMAs complete.
+      bool last_of_m = false;
+      if (a_res) {
+        const int mt = tile_m(tile);
+        if (mt != res_m_c) {
+          res_m_c = mt;
+          mbar_wait(a_full, a_seg & 1);
+          ++a_seg;
+        }
+        last_of_m = (tile + t_step >= t_end) || tile_m(tile + t_step) != mt;
+      }
+      WgAcc<BN / 2> acc;
+      uint32_t prev_s = 0;
+      for (int ki = 0; ki < k_iters; ++ki, st.next()) {
+        const uint32_t s = st.s;
+        mbar_wait(&full[s], st.ph);
+        const uint32_t a_addr = a_base + (a_res ? static_cast<uint32_t>(ki) * kAStage : s * kStageBytes);
+        const uint32_t b_addr = b_base + s * static_cast<uint32_t>(stage_bytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), (ki | k) != 0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (ki > 0 && lane == 0) mbar_arrive(&empty[prev_s]);
+        prev_s = s;
+      }
+      wgmma_wait<0>();
+      acc.fence_regs();
+      if (lane == 0) {
+        mbar_arrive(&empty[prev_s]);
+        if (last_of_m) mbar_arrive(a_empty);
+      }
       if (kTma && has_res) mbar_wait(&res_full[tc & 1], (tc >> 1) & 1);
       const int m = m0 + static_cast<int>(row);
       const bool row_ok = m < M;
-      const uint32_t taddr = tmem_row + buf * BN;
-#pragma unroll 1
+#pragma unroll
       for (int ci = 0; ci < kChunksPerWarp; ++ci) {
         const int ch = half * kChunksPerWarp + ci;
         uint32_t r[32];
-        tmem_ld_32x32(taddr + ch * 32, r);
-        tmem_ld_wait_regs(r);
-        if (ci == kChunksPerWarp - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if constexpr (kCG == 2) mbar_arrive_cluster(&t_empty[buf], 0);
-            else mbar_arrive(&t_empty[buf]);
-          }
-        }
+        acc.rows32(ci, r, xacc, lane);
         const int nc = n0 + ch * 32;
         if (nc >= N) continue;
         float y[32];
@@ -507,9 +425,8 @@ __global__ void __launch_bounds__(kThreads, 1)
           }
         } else {
           // Direct epilogue (split-bf16 planes, fp32 outputs, final layers).  Thread = accumulator row, but a row's 32 columns
-          // are only 64 bytes per plane: written straight from the registers, one warp instruction touched 32 rows x 16 bytes
-          // (32 half-used sectors, 32 LSU wavefronts) and the 1x1 expansions of the fp32-level modes ran at 0.5 TB/s (layer1:
-          // 870 us against 97 us with the TMA-store epilogue in one-plane mode).  Every plane now goes through the warp's
+          // are only 64 bytes per plane: written straight from the registers, one warp instruction would touch 32 rows x 16 bytes
+          // (32 half-used sectors, 32 LSU wavefronts).  Every plane goes through the warp's
           // transpose buffer: rows -> shared memory, then 8 rows x 64 contiguous bytes per instruction to / from global memory.
           const int nvalid = min(32, N - nc);   // multiple of 8 (N % 8 == 0 enforced on the host)
           const uint32_t xw = smem_u32(out_stage) + ewarp * kXposeWarpBytes;
@@ -610,20 +527,14 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
   }
 
-  if (kTma && warp == 2 && lane == 0) tma_store_wait_all();   // etid 0 issued the stores
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (kCG == 2) cluster_sync();   // the peer's MMAs (issued by the leader) read this CTA's tiles and write its TMEM
-  if (warp == 2) tmem_dealloc<kCG>(tmem_base, kTmemCols);
+  if (kTma && warp == 0 && lane == 0) tma_store_wait_all();   // etid 0 issued the stores
 }
 
 // A-resident mode: plain (non-im2col) single-term GEMMs with several column blocks and K <= 256 -- the wide 1x1
 // expansions: the A rows of an m-tile are loaded once instead of once per column block (per-SM-unique data is what
 // the L2 -> shared-memory path is short of; the W tiles are shared by all SMs and cheap)
 // (the resident rows are single buffered: the next m-tile's rows wait for the last MMA on the current ones, a bubble
-// that only pays off when the epilogue is heavy (residual) or the m-tile has >= 4 column blocks; measured on B200,
-// batch 256: 177 -> 157 us for the layer1 expansion with residual, 98 -> 90 us layer2, but 103 -> 130 us for the
-// residual-free 2-block downsample)
+// that only pays off when the epilogue is heavy (residual) or the m-tile has >= 4 column blocks)
 bool wants_a_resident(const GemmParams& p, int BN, bool im2col, size_t max_smem) {
   const int k_iters_h = p.n_terms * p.taps * p.cblocks;
   if (!(!im2col && p.tma_epi && p.n_terms == 1 && p.num_n_tiles >= 2 && (p.res != nullptr || p.num_n_tiles >= 4) &&
@@ -633,24 +544,25 @@ bool wants_a_resident(const GemmParams& p, int BN, bool im2col, size_t max_smem)
   // the layer runs with the default schedule
   const size_t staging = static_cast<size_t>(BN / 64) * kBM * 128;
   const size_t need = 1024 + static_cast<size_t>(2) * p.num_n_tiles * BN * 4 + static_cast<size_t>(k_iters_h) * kAStage + 256 +
-                      static_cast<size_t>(1 + (p.res ? 2 : 0)) * staging + 3 * static_cast<size_t>(BN) * kBK * 2;
+                      static_cast<size_t>(1 + (p.res ? 2 : 0)) * staging + kAccXposeBytes + 3 * static_cast<size_t>(BN) * kBK * 2;
   return need <= max_smem;
 }
 
-template <int BN, bool kIm2col, int kEpi, int kCG>
+template <int BN, bool kIm2col, int kEpi>
 int launch(const GemmMaps& maps, GemmParams& p, int num_sms, size_t max_smem, cudaStream_t stream) {
-  constexpr int kStageBytes = kAStage + (BN / kCG) * kBK * 2;
+  constexpr int kStageBytes = kAStage + BN * kBK * 2;
   constexpr size_t kStagingBytes = static_cast<size_t>(BN / 64) * kBM * 128;
   // staging tiles: residual layers get 2 residual + 2 output tiles (prefetch / drain a full tile ahead) when they still
   // leave >= 3 pipeline stages, otherwise one output tile (plus two residual tiles if needed)
   p.n_res_bufs = (p.tma_epi && p.res) ? 2 : 0;
   p.n_out_bufs = p.tma_epi ? 2 : 0;
   const int k_iters_h = p.n_terms * p.taps * p.cblocks;
-  p.a_resident = (kCG == 1 && kEpi != 0 && wants_a_resident(p, BN, kIm2col, max_smem)) ? 1 : 0;
+  p.a_resident = (kEpi != 0 && wants_a_resident(p, BN, kIm2col, max_smem)) ? 1 : 0;
   const size_t sb_bytes = p.a_resident ? static_cast<size_t>(2) * p.num_n_tiles * BN * 4 : static_cast<size_t>(4) * BN * 4;
   const size_t ares_bytes = p.a_resident ? static_cast<size_t>(k_iters_h) * kAStage : 0;
   auto fixed_for = [&](int nout, int nres) {
-    return 1024 + sb_bytes + ares_bytes + 256 + static_cast<size_t>(nout + nres) * kStagingBytes + (p.tma_epi ? 0 : kXposeBytes);
+    return 1024 + sb_bytes + ares_bytes + 256 + static_cast<size_t>(nout + nres) * kStagingBytes + (p.tma_epi ? 0 : kXposeBytes) +
+           kAccXposeBytes;
   };
   const size_t stage_bytes = p.a_resident ? static_cast<size_t>(BN) * kBK * 2 : static_cast<size_t>(kStageBytes);
   if (p.tma_epi && (fixed_for(p.n_out_bufs, p.n_res_bufs) + 3 * stage_bytes > max_smem)) p.n_out_bufs = 1;
@@ -660,7 +572,7 @@ int launch(const GemmMaps& maps, GemmParams& p, int num_sms, size_t max_smem, cu
   stages = std::min(stages, 8);
   p.stages = stages;
   const size_t smem = fixed + static_cast<size_t>(stages) * stage_bytes;
-  auto kern = gemm_bf16_kernel<BN, kIm2col, kEpi, kCG>;
+  auto kern = gemm_bf16_kernel<BN, kIm2col, kEpi>;
   static bool attr_set_dev[64] = {};   // per template instantiation and device (the attribute is per device)
   int cur_dev = 0;
   DCR_CUDA_CHECK(cudaGetDevice(&cur_dev));
@@ -669,22 +581,7 @@ int launch(const GemmMaps& maps, GemmParams& p, int num_sms, size_t max_smem, cu
     DCR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(max_smem)));
     attr_set = true;
   }
-  if constexpr (kCG == 2) {
-    const int pair_tiles = ((p.num_m_tiles + 1) / 2) * p.num_n_tiles;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * std::min(pair_tiles, num_sms / 2));
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    DCR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, maps, p));
-  } else {
+  {
     const int tiles = p.num_m_tiles * p.num_n_tiles;
     const int grid = std::min(tiles, num_sms);
     kern<<<grid, kThreads, smem, stream>>>(maps, p);
@@ -699,7 +596,8 @@ int launch(const GemmMaps& maps, GemmParams& p, int num_sms, size_t max_smem, cu
 int conv_gemm(const ConvGemmDesc& d, cudaStream_t stream) {
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  DCR_REQUIRE(di->cc_major == 10, "conv_gemm: this build targets sm_100a; device reports sm_%d%d", di->cc_major, di->cc_minor);
+  DCR_REQUIRE(di->cc_major == 9 && di->cc_minor == 0, "conv_gemm: this build targets sm_90a; device reports sm_%d%d", di->cc_major,
+              di->cc_minor);
   DCR_REQUIRE(d.n_terms >= 1 && d.n_terms <= kMaxGemmTerms, "conv_gemm: bad n_terms %d", d.n_terms);
   DCR_REQUIRE(d.C % 8 == 0 && d.N % 8 == 0, "conv_gemm: C (%d) and N (%d) must be multiples of 8", d.C, d.N);
   DCR_REQUIRE(d.kh >= 1 && d.kw >= 1 && d.stride >= 1, "conv_gemm: bad filter geometry");
@@ -790,13 +688,10 @@ int conv_gemm(const ConvGemmDesc& d, cudaStream_t stream) {
   p.act = d.act;
   p.fast_gelu = (d.n_terms == 1 && p.out_planes <= 1 && !tuning_flag("DCR_GELU_ERF")) ? 1 : 0;
   // tile order: with several column blocks and an A matrix larger than what L2 keeps between the passes, m-fastest order
-  // streams A from HBM once per column block (ViT-S fc2: 155 MB x 3 = 83 us of HBM time for a 99 us layer)
+  // streams A from HBM once per column block
   const double a_bytes = 2.0 * a_planes * (im2col ? static_cast<double>(d.B) * d.H * d.W * d.C : static_cast<double>(M) * d.C);
   const int order = tuning_int("DCR_GEMM_TILE_ORDER", -1);   // tuning / tests: 0 = m-fastest, 1 = n-fastest, default by size
   p.n_fastest = (order >= 0) ? (order == 1 && p.num_n_tiles >= 2) : (p.num_n_tiles >= 2 && a_bytes > 48e6);
-  if (kGemmTimingMode == 2 && im2col && !windowed) {
-    if (int rc = make_tmap_2d_bf16(&maps.a_flat, d.in, static_cast<uint64_t>(d.B) * d.H * d.W, d.C, d.C, kBM, kBK)) return rc;
-  }
   p.tma_epi = (p.out != nullptr && p.out_planes == 1 && p.out_f32 == nullptr && (p.res == nullptr || p.res_planes == 1) &&
                (d.act != 2 || p.fast_gelu) &&   // the TMA-store epilogue's compile-time GELU is the tanh form
                !tuning_flag("DCR_GEMM_DIRECT_EPILOGUE"))
@@ -818,38 +713,11 @@ int conv_gemm(const ConvGemmDesc& d, cudaStream_t stream) {
   DCR_REQUIRE(p.res == nullptr || p.ld_res % 8 == 0, "conv_gemm: residual leading dim must be a multiple of 8");
   DCR_REQUIRE(p.out_f32 == nullptr || p.ld_out_f32 % 4 == 0, "conv_gemm: fp32 output leading dim must be a multiple of 4");
 
-  // ---- CTA-pair form (cta_group::2, 256-row tiles, half a W tile per CTA): plain single-term GEMMs with the TMA-store
-  // epilogue whose A rows are not kept resident and that have enough m-tiles to fill the pairs
-  const int want_cg2 = tuning_int("DCR_GEMM_CG2", -1);   // 0: never, 1: wherever the kernel form exists, default: policy
-  bool use_cg2 = !im2col && p.tma_epi && p.n_terms == 1 && (BN == 128 || BN == 256) && kGemmTimingMode == 0 && want_cg2 != 0;
-  if (use_cg2 && want_cg2 < 0) {
-    // measured per layer at batch 256 (tools/pair_bench.py, B200): 256-wide tiles gain 5-11 % from K = 384 up (ResNet layer3/4
-    // reductions 256<-1024, 512<-1024; ViT qkv 1152<-384, ViT-B qkv / fc1); 128-wide residual tiles gain only with many column
-    // blocks and K >= 512 (layer4 expansion 2048<-512: 9 %; ViT fc2 / proj with 3 column blocks: none); short K loses
-    const long long pair_tiles = static_cast<long long>((p.num_m_tiles + 1) / 2) * p.num_n_tiles;
-    const bool shape_ok = (BN == 256) ? ktot >= 384 : (ktot >= 512 && p.num_n_tiles >= 8);
-    use_cg2 = !wants_a_resident(p, BN, im2col, di->max_smem_optin) && shape_ok && pair_tiles >= di->num_sms;
-  }
-  if (use_cg2) {
-    for (int pl = 0; pl < 3; ++pl) {
-      const int pw = std::min(pl, w_planes - 1);
-      if (int rc = make_tmap_2d_bf16(&maps.w[pl], d.weight + pw * d.w_plane_stride, d.N, ktot, ktot, BN / 2, kBK)) return rc;
-    }
-  }
   const int epi = p.tma_epi ? 1 + p.act : 0;   // compile-time activation on the TMA-store path
-  if (use_cg2) {
-#define DCR_LAUNCH_PAIR(BNv)                                                                                     \
-  (epi == 1 ? launch<BNv, false, 1, 2>(maps, p, di->num_sms, di->max_smem_optin, stream)                         \
-            : (epi == 2 ? launch<BNv, false, 2, 2>(maps, p, di->num_sms, di->max_smem_optin, stream)             \
-                        : (epi == 3 ? launch<BNv, false, 3, 2>(maps, p, di->num_sms, di->max_smem_optin, stream) \
-                                    : launch<BNv, false, 4, 2>(maps, p, di->num_sms, di->max_smem_optin, stream))))
-    return BN == 128 ? DCR_LAUNCH_PAIR(128) : DCR_LAUNCH_PAIR(256);
-#undef DCR_LAUNCH_PAIR
-  }
 
 #define DCR_LAUNCH_E(BNv, E)                                                                      \
-  (im2col ? launch<BNv, true, E, 1>(maps, p, di->num_sms, di->max_smem_optin, stream)              \
-          : launch<BNv, false, E, 1>(maps, p, di->num_sms, di->max_smem_optin, stream))
+  (im2col ? launch<BNv, true, E>(maps, p, di->num_sms, di->max_smem_optin, stream)              \
+          : launch<BNv, false, E>(maps, p, di->num_sms, di->max_smem_optin, stream))
 #define DCR_LAUNCH(BNv)                                                                          \
   (epi == 0 ? DCR_LAUNCH_E(BNv, 0)                                                                \
             : (epi == 1 ? DCR_LAUNCH_E(BNv, 1) : (epi == 2 ? DCR_LAUNCH_E(BNv, 2) : (epi == 3 ? DCR_LAUNCH_E(BNv, 3) : DCR_LAUNCH_E(BNv, 4)))))

@@ -39,7 +39,7 @@ int topk_merge(const float* scores, const long long* idx, int nq, int nlists, in
                long long* out_idx, cudaStream_t stream);
 
 
-// ---- tcgen05 GEMM / implicit-GEMM convolution (conv_gemm.cu) ---------------------------------------------------
+// ---- wgmma GEMM / implicit-GEMM convolution (conv_gemm.cu) ---------------------------------------------------
 constexpr int kMaxGemmTerms = 6;
 
 // Y = act(scale * conv(X, W) + bias (+ R)).  X: NHWC bf16 planes [B,H,W,C] (row stride ld_in for the 1x1/linear
@@ -73,7 +73,7 @@ struct ConvGemmDesc {
 };
 int conv_gemm(const ConvGemmDesc& d, cudaStream_t stream);
 int conv_exact(const ConvGemmDesc& d, cudaStream_t stream);
-bool conv3x3_halo_eligible(const ConvGemmDesc& d);   // 3x3 / stride 1 / pad 1, fast mode, no residual, W <= 62, N <= 256
+bool conv3x3_halo_eligible(const ConvGemmDesc& d);   // 3x3 / stride 1 / pad 1, fast mode, no residual, W <= 62, N <= 128
 int conv3x3_halo(const ConvGemmDesc& d, cudaStream_t stream);
 // bottleneck_fuse.cu: `a` (1x1 expand + residual + ReLU) followed by `b` (1x1 reduce + ReLU) on a's output, fast mode
 bool expand_reduce_eligible(const ConvGemmDesc& a, const ConvGemmDesc& b, size_t max_smem);

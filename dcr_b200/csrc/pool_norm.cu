@@ -276,8 +276,7 @@ __global__ void pool_kernel(const PoolParams p) {
 
 // Single-plane 3x3 average pool, count_include_pad = False (the patched pools of the FID Inception blocks,
 // metrics/inception.py:241,269,302): nine clamped 16-byte loads in flight per thread, fp32 sum of the in-bounds taps in the
-// generic kernel's order (bit-identical results), one division.  The generic kernel walked the taps serially: 1.4 ms of a
-// 5.5 ms Inception forward at batch 128 (profiles/r02_layers_inception.txt) for data HBM moves in ~0.15 ms.
+// generic kernel's order (bit-identical results), one division (the generic kernel walks the taps serially).
 __global__ void __launch_bounds__(256) avgpool3_bf16_kernel(const PoolParams p) {
   const int cg = p.C / 8;
   const long long total = static_cast<long long>(p.B) * p.OH * p.OW * cg;
@@ -395,8 +394,7 @@ struct ReduceHWParams {
 };
 
 // block = 64 channel groups x kSlices position slices: every thread streams HW / kSlices positions of its 8 channels
-// (independent 16-byte loads, several in flight), the slices meet in shared memory.  (One thread per channel group walked
-// all HW positions serially before: 41 us for the 51 MB layer4 output of a ResNet-50 batch.)
+// (independent 16-byte loads, several in flight), the slices meet in shared memory.
 constexpr int kRedSlices = 4;
 // kCube: GeM with p = 3 (the SSCD head): t*t*t and cbrtf; the general exponent keeps powf out of this instantiation (inlined
 // into the unrolled loop it made the kernel instruction-fetch bound: 39 us, 26 % of the warp samples on `no_inst`).
@@ -466,8 +464,7 @@ struct LayerNormParams {
 
 // Single-plane fast path for C = kChunks * 128 (384, 512, 768, 1024): HALF a warp per row, kChunks 16-byte loads per lane
 // all in flight at once (balanced: the generic kernel gives C = 384 to 32 + 16 lanes), gamma / beta held in registers across
-// the rows a half-warp walks, 4-step reductions.  The generic kernel ran at ~2 TB/s (37 us for the 50k x 384 rows of a
-// ViT-S/16 batch); this one is a pure stream.
+// the rows a half-warp walks, 4-step reductions.  This one is a pure stream.
 template <int kChunks>
 __global__ void __launch_bounds__(256) layernorm_fast_kernel(const LayerNormParams p) {
   const int lane16 = threadIdx.x & 15;

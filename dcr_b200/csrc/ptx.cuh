@@ -1,5 +1,4 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (tiled + im2col), tcgen05 (alloc/mma/commit/ld),
-// cluster helpers.  Everything here is device-only and header-only.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (tiled + im2col), wgmma, cluster helpers.  Everything here is device-only and header-only.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -65,10 +64,8 @@ DCR_DEVICE bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// The producer and MMA-issuing roles are single threads whose instruction stream runs at one dependent instruction
-// every few cycles; everything between two tcgen05.mma / TMA issues is on the critical path of the whole pipeline
-// (tools/microbench/umma_rate.cu: a handful of extra compares and branches per 4 MMAs turn 54 cycles per 128x64x16 MMA
-// into 120).  So: the wait is one tight asm loop (no predicate -> register -> branch round trip per poll) ...
+// The producer role is a single thread whose instruction stream is on the critical path of the whole pipeline, so the
+// wait is one tight asm loop (no predicate -> register -> branch round trip per poll) ...
 DCR_DEVICE void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
       "{\n\t.reg .pred P;\n\t"
@@ -118,41 +115,21 @@ constexpr uint64_t kEvictNormal = 0x1000000000000000ull;
 constexpr uint64_t kEvictFirst = 0x12F0000000000000ull;
 constexpr uint64_t kEvictLast = 0x14F0000000000000ull;
 
-// kCG == 1 : plain load, completes on this CTA's barrier.
-// kCG == 2 : cta_group::2 load; completes on the barrier at the same offset in the even (leader) CTA of the pair.
-template <int kCG>
+// tiled loads, complete on this CTA's barrier
 DCR_DEVICE void tma_load_2d(void* dst, const void* tmap, uint64_t* bar, int c0, int c1, uint64_t hint) {
-  if constexpr (kCG == 1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
-        : "memory");
-  } else {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1), "l"(hint)
-        : "memory");
-  }
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
+      : "memory");
 }
 
-template <int kCG>
 DCR_DEVICE void tma_load_3d(void* dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2, uint64_t hint) {
-  if constexpr (kCG == 1) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(hint)
-        : "memory");
-  } else {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1), "r"(c2),
-        "l"(hint)
-        : "memory");
-  }
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(hint)
+      : "memory");
 }
 
 // 4-D tiled load / store (coordinates innermost first; loads may start at negative coordinates: zero fill)
@@ -171,101 +148,15 @@ DCR_DEVICE void tma_store_4d(const void* tmap, const void* src_smem, int c0, int
 }
 
 // im2col-mode load of an NHWC tensor: coordinates {c, w, h, n} of the first base pixel, filter-tap offsets {w, h}
-template <int kCG>
 DCR_DEVICE void tma_load_im2col_4d(void* dst, const void* tmap, uint64_t* bar, int c, int w, int h, int n,
                                    uint16_t off_w, uint16_t off_h) {
-  if constexpr (kCG == 1) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w),
-        "h"(off_h)
-        : "memory");
-  } else {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.im2col.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c), "r"(w), "r"(h), "r"(n),
-        "h"(off_w), "h"(off_h)
-        : "memory");
-  }
-}
-
-// ----------------------------------------------------------------------------------------------
-// tcgen05
-template <int kCG>
-DCR_DEVICE void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  if constexpr (kCG == 1)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-  else
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-}
-template <int kCG>
-DCR_DEVICE void tmem_relinquish() {
-  if constexpr (kCG == 1)
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  else
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int kCG>
-DCR_DEVICE void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (kCG == 1)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  else
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-DCR_DEVICE void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-DCR_DEVICE void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers fp16/bf16 inputs with fp32 accumulation.
-template <int kCG>
-DCR_DEVICE void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (kCG == 1)
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-  else
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// D[tmem] (+)= A[tmem] * B[smem desc], CTA pair.  A: K-major, lane = row, two bf16 per 32-bit column (K = 16 spans
-// 8 columns); each CTA of the pair holds its own 128 rows at the same column address.  The 8-register vector is the
-// disable-output-lane mask (all lanes enabled).
-DCR_DEVICE void umma_f16_ts_cg2(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  const uint32_t z = 0;
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(z)
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w),
+      "h"(off_h)
       : "memory");
 }
-
-// 32 registers per thread -> 32 lanes x 32 consecutive 32-bit columns (thread i of the warp writes TMEM lane base+i)
-DCR_DEVICE void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};" ::"r"(r[0]),
-      "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]),
-      "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]),
-      "r"(r[29]), "r"(r[30]), "r"(r[31]), "r"(taddr)
-      : "memory");
-}
-DCR_DEVICE void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // Explicit shared-state-space vector accesses (32-bit shared addresses): pointers into dynamically carved shared
 // memory whose buffer index is a run-time value otherwise compile to GENERIC loads/stores (LD.E / ST.E), which queue
@@ -283,79 +174,134 @@ DCR_DEVICE float4 ld_shared_f4(uint32_t saddr) {
 DCR_DEVICE void st_shared_v4(uint32_t saddr, const uint4& v) {
   asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
+DCR_DEVICE float2 ld_shared_f2(uint32_t saddr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(saddr));
+  return v;
+}
+DCR_DEVICE uint32_t ld_shared_u32(uint32_t saddr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(saddr));
+  return v;
+}
+DCR_DEVICE void st_shared_u32(uint32_t saddr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory");
+}
 DCR_DEVICE void st_shared_f32(uint32_t saddr, float v) {
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(saddr), "f"(v) : "memory");
 }
 
-// commit all previously issued MMAs of this thread to an mbarrier (arrive::one when they retire).
-// kCG == 2 multicasts the arrive to the barrier at the same offset in both CTAs of the pair.
-template <int kCG>
-DCR_DEVICE void umma_commit(uint64_t* bar) {
-  if constexpr (kCG == 1)
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-  else
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(static_cast<uint16_t>(3))
-        : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i of the warp reads TMEM lane base+i)
-DCR_DEVICE void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-DCR_DEVICE void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-DCR_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// wait for the outstanding tcgen05.ld and tie the destination registers to the wait so that no consumer of r[] can
-// be scheduled above it (the loads complete asynchronously)
-DCR_DEVICE void tmem_ld_wait_regs(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]),
-                 "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]),
-                 "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]),
-                 "+r"(r[29]), "+r"(r[30]), "+r"(r[31])::"memory");
-}
 
 // ----------------------------------------------------------------------------------------------
-// UMMA descriptors (layouts documented in DESIGN.md "tcgen05 operand layout")
-//
-// Shared-memory matrix descriptor for a K-major bf16 tile stored as rows of 128 B with the 128-byte swizzle
-// (8-row x 128 B atoms, atoms 1024 B apart).  start>>4 in [0,14), LBO>>4 in [16,30) (unused for swizzled K-major,
-// set to 1), SBO>>4 = 1024>>4 in [32,46), descriptor version 1 in [46,48), layout type 2 (SWIZZLE_128B) in [61,64).
-DCR_DEVICE uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// wgmma (Hopper warpgroup MMA): D[regs] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulation.
+// Executed by all 128 threads of an aligned warpgroup (warps 4i .. 4i+3).
+DCR_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+DCR_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+DCR_DEVICE void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory"); }
+
+// m64 x N x k16; kTransB: B is stored MN-major (N contiguous) instead of K-major
+template <int N, bool kTransB = false>
+DCR_DEVICE void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  static_assert(N == 32 || N == 64 || N == 128, "wgmma_bf16: N must be 32, 64 or 128");
+  if constexpr (N == 32) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, 0, %19;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(kTransB ? 1 : 0));
+  } else if constexpr (N == 64) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, %35;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(kTransB ? 1 : 0));
+  } else if constexpr (N == 128) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, %67;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(kTransB ? 1 : 0));
+  }
+
+}
+
+// Shared-memory matrix descriptor (wgmma) for a bf16 tile stored as rows of 128 B with the 128-byte swizzle (8-row x
+// 128 B atoms).  start>>4 in [0,14), LBO>>4 in [16,30) (unused for swizzled K-major, 1), SBO>>4 in [32,46) = distance of
+// consecutive 8-row groups, layout type 1 (SWIZZLE_128B) in [62,64); base offset 0: the swizzle is a function of the
+// absolute shared-memory address, so a start address that is a multiple of 128 B but not of 1024 B (conv3x3_halo.cu)
+// needs no correction.  K advances inside the atom by +32 B per k16.
+DCR_DEVICE uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_t sbo = 1024) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(sbo >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// Instruction descriptor for kind::f16: D=f32 (bits 4-5 = 1), A=B=bf16 (bits 7-9, 10-12 = 1), both K-major,
-// N>>3 in [17,23), M>>4 in [24,29).
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t m, uint32_t n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
+// A 128-row x N-column fp32 accumulator tile held by one warpgroup as two m64 wgmma accumulators.  The A descriptors take
+// the tile's 8-row groups two apart (SBO = 2048 B; the second accumulator starts one group, 1024 B, later), so warp w of
+// the warpgroup holds exactly rows 32w .. 32w+31 of the tile: the row block its epilogue owns.
+template <int N, bool kTransB = false>
+struct WgAcc {
+  float d[2][N / 2];
+
+  // one k16 step.  a_addr: smem address of row 0 of the 128-row K-major A tile (1024-aligned, plus the k offset);
+  // db: descriptor of B for the same k step
+  DCR_DEVICE void mma(uint32_t a_addr, uint64_t db, uint32_t accumulate) {
+    mma2(wgmma_desc_sw128(a_addr, 2048), wgmma_desc_sw128(a_addr + 1024, 2048), db, accumulate);
+  }
+  // the same with explicit A descriptors of the two 64-row halves (even / odd 8-row groups)
+  DCR_DEVICE void mma2(uint64_t da0, uint64_t da1, uint64_t db, uint32_t accumulate) {
+    wgmma_bf16<N, kTransB>(d[0], da0, db, accumulate);
+    wgmma_bf16<N, kTransB>(d[1], da1, db, accumulate);
+  }
+  // keep the compiler from moving accumulator accesses across wgmma_fence / wgmma_wait
+  DCR_DEVICE void fence_regs() {
+#pragma unroll
+    for (int s = 0; s < 2; ++s)
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) asm volatile("" : "+f"(d[s][i])::"memory");
+  }
+  // every pair of horizontally adjacent accumulator elements this thread holds: f(row, col, d[row][col], d[row][col + 1])
+  // with row in [0, 32) of this warp's row block and col even, in [0, N).  For epilogues that write straight from the
+  // accumulator layout (no transpose buffer).
+  template <class F>
+  DCR_DEVICE void for_each_pair(uint32_t lane, F&& f) const {
+    const uint32_t r0 = lane >> 2, c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int s = 0; s < 2; ++s)
+#pragma unroll
+      for (int i = 0; i < N / 2; i += 2) f(r0 + 8 * s + 16 * ((i >> 1) & 1), 8 * (i >> 2) + c0, d[s][i], d[s][i + 1]);
+  }
+  // columns [32c, 32c+32) of row `lane` of this warp's 32-row block -> r[0..31], through the warp's 32 x 33 float
+  // transpose buffer at shared address xbuf.  c must be a compile-time constant after unrolling (d stays in registers).
+  DCR_DEVICE void rows32(int c, uint32_t (&r)[32], uint32_t xbuf, uint32_t lane) const {
+    const uint32_t r0 = lane >> 2, c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int s = 0; s < 2; ++s)
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const uint32_t row = r0 + 8 * s + 16 * ((i >> 1) & 1);
+        const uint32_t col = 8 * (i >> 2) + c0 + (i & 1);
+        st_shared_f32(xbuf + (row * 33 + col) * 4, d[s][16 * c + i]);
+      }
+    __syncwarp();
+#pragma unroll
+    for (int j = 0; j < 32; ++j) asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r[j]) : "r"(xbuf + (lane * 33 + j) * 4));
+    __syncwarp();
+  }
+};
+constexpr int kAccXposeWarpBytes = 32 * 33 * 4;   // per-warp transpose buffer of WgAcc::rows32
 
 }  // namespace dcr

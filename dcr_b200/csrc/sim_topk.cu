@@ -1,4 +1,4 @@
-// Fused all-pairs similarity + per-query top-k for sm_100a.
+// Fused all-pairs similarity + per-query top-k for sm_90a.
 //
 // Replaces (reference = somepago/DCR):
 //   diff_retrieval.py:402      sim = torch.mm(values_features, query_features.T)          (fp32, [G,Q], CPU/MKL)
@@ -8,7 +8,7 @@
 //
 // The [Q,G] score matrix is never written.  Three stages, all on the caller's stream:
 //   1. to_bf16_rows_kernel   fp32 descriptors -> zero-padded bf16 rows + per-row norms of the rounding residual
-//   2. sim_topk_kernel       tcgen05 bf16 GEMM (fp32 accumulate in TMEM) whose epilogue keeps, per query, the
+//   2. sim_topk_kernel       wgmma bf16 GEMM (fp32 accumulate in registers) whose epilogue keeps, per query, the
 //                            kp (>= k) best approximate scores of its gallery segment (threshold filter on the
 //                            accumulator registers, warp-cooperative compaction in shared memory)
 //   3. rescore_select_kernel exact re-score (fp64 accumulate, fixed order) of the <= slots*kp candidates per query,
@@ -30,8 +30,8 @@ namespace dcr {
 
 namespace {
 
-constexpr int kBlockM = 128;      // query rows per CTA (TMEM lanes)
-constexpr int kBlockN = 256;      // gallery rows per tile (TMEM columns per accumulator buffer)
+constexpr int kBlockM = 128;      // query rows per CTA
+constexpr int kBlockN = 128;      // gallery rows per tile (accumulator columns: 128 registers per thread with one warpgroup)
 constexpr int kBlockK = 64;       // bf16 elements per 128-byte swizzled smem row
 constexpr int kMaxKB = 8;         // d_pad <= 512: the query tile stays resident in shared memory; larger: streamed
 constexpr int kMaxDim = 8192;     // largest descriptor dimension accepted
@@ -40,19 +40,13 @@ constexpr int kWarmTiles = 4;     // tiles replayed at the start of every segmen
 constexpr uint32_t kFull = 0xffffffffu;
 constexpr int kATileBytes = kBlockM * kBlockK * 2;  // 16 KB
 constexpr int kMaxSlotsPerQuery = 512;  // (chunk, unit) segments that may cover one q-tile
-// Timing experiments (results are garbage), compile-time only so that the production issue loops carry no trace of them:
-// 1 = the epilogue loads TMEM but does not scan, 2 = does not even load, 3 = additionally no gallery loads at all.
-#ifndef DCR_SIM_TIMING_MODE
-#define DCR_SIM_TIMING_MODE 0
-#endif
-constexpr int kTimingMode = DCR_SIM_TIMING_MODE;
 
 struct SimParams {
   int nq, ng;
   int num_kb;          // d_pad / 64
   int stream_a;        // 1 (d_pad > 512): query k-blocks travel with the gallery k-blocks instead of staying resident
-  int n_qtiles;        // ceil(nq / (128*CG))
-  int n_gtiles;        // ceil(ng / 256)
+  int n_qtiles;        // ceil(nq / 128)
+  int n_gtiles;        // ceil(ng / 128)
   int gchunk;          // gallery tiles per L2-sized chunk (all units sweep chunk c before chunk c+1)
   int n_chunks;
   int kp;              // candidates kept per (query, segment): 8, 16 or 32
@@ -169,7 +163,7 @@ __global__ void __launch_bounds__(256) to_bf16_rows_kernel(const float* __restri
 // column sums of x[n, d] accumulated in double; mean = sum / n afterwards (rows r*row_stride, r < n: any fixed vector works
 // as the centre, so a strided sample of the gallery is enough).  A thread owns one 16-byte column group and a slice of the
 // block's rows (independent loads, four in flight), the slices meet in shared memory and the block does ONE atomicAdd per
-// column: the first version had 592 blocks each add all d columns -- 300k same-address double atomics, 22 us for a 16 MB sample.
+// column instead of every block adding all d columns (hundreds of thousands of same-address double atomics).
 constexpr int kColSumThreads = 512;
 __global__ void __launch_bounds__(kColSumThreads)
     col_sum_kernel(const float* __restrict__ x, int n, int row_stride, int d, double* __restrict__ sums,
@@ -289,16 +283,6 @@ DCR_DEVICE float thr_from_key(unsigned int k) {
 
 DCR_DEVICE float max8(const float* v) {
   return fmaxf(fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])), fmaxf(fmaxf(v[4], v[5]), fmaxf(v[6], v[7])));
-}
-
-DCR_DEVICE void tmem_ld_wait_dep(uint32_t (&r)[32]) {
-  // the registers are tied to the wait so that no consumer of r[] can be scheduled above it
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]),
-                 "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]),
-                 "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]),
-                 "+r"(r[29]), "+r"(r[30]), "+r"(r[31])::"memory");
 }
 
 // Keep the kp best of lane L's n (kp < n <= 64) list entries, stored at list[j * 128] (j = 0..n-1); returns the
@@ -496,26 +480,26 @@ struct SegWalker {
 };
 
 // ------------------------------------------------------------------------------------------------------------
-// stage 2: the fused kernel.  kCG = 1: one CTA per work unit (UMMA 128x256x16).  kCG = 2: a CTA pair per work
-// unit (UMMA 256x256x16, cta_group::2): each CTA keeps its own 128 queries resident and loads half of every
-// gallery tile, so L2->SMEM traffic per FLOP halves.
+// stage 2: the fused kernel.  One CTA per work unit; kSets consumer warpgroups (warps 0 .. 4 kSets - 1) each issue the
+// wgmma for their column range of every 128 x 128 tile (fp32 accumulators in registers) and filter it; the last warp is
+// the TMA producer.
 //
 // Work decomposition: the (q-tile, g-tile) grid is linearised q-major into T = n_qtiles * n_gtiles tiles and cut
-// into gridDim/kCG equal contiguous ranges.  A unit's range is walked as "segments" (maximal runs inside one
+// into gridDim equal contiguous ranges.  A unit's range is walked as "segments" (maximal runs inside one
 // q-tile); per segment the query tile is loaded once (A stays resident) and the thresholds are seeded by
 // replaying the first kWarmTiles tiles.  Segment (unit u, q-tile i) owns candidate slot u + i.
 // kBias: compiled with / without the per-column offset path of query centring.  Both variants are launched; the one
 // that does not match the device-side decision (p.bias_flag) exits at once -- no host synchronisation needed.
-template <int kCG, bool kBias, int kSets>
-__global__ void __launch_bounds__(64 + 128 * kSets, 1)
+template <bool kBias, int kSets>
+__global__ void __launch_bounds__(32 + 128 * kSets, 1)
     sim_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_g,
                     const SimParams p) {
   if (((p.col_bias != nullptr) && (p.bias_flag != nullptr) && (*p.bias_flag != 0)) != kBias) return;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // carve-up (all tile bases 1024-byte aligned for the 128B swizzle)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr int kBRows = kBlockN / kCG;
-  constexpr int kBTileBytes = kBRows * kBlockK * 2;
+  constexpr int kBTileBytes = kBlockN * kBlockK * 2;
+  constexpr int kSetCols = kBlockN / kSets;
   // resident mode: [num_kb x 16 KB query tile][stages x gallery tile]; streamed mode (d_pad > 512, the query tile no
   // longer fits): [stages x (gallery tile | 16 KB query k-block)] -- twice the L2->SMEM traffic per FLOP
   const bool stream_a = p.stream_a != 0;
@@ -528,162 +512,99 @@ __global__ void __launch_bounds__(64 + 128 * kSets, 1)
   uint64_t* b_empty = bars + 8;         // [stages]
   uint64_t* a_full = bars + 16;
   uint64_t* a_empty = bars + 17;
-  uint64_t* t_full = bars + 18;         // [2]
-  uint64_t* t_empty = bars + 20;        // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 22);
   float* carry = reinterpret_cast<float*>(bars + 32);   // [kSets][4][128] thresholds carried to the next chunk, by q-tile & 3
+  uint8_t* acc_xpose = reinterpret_cast<uint8_t*>(carry + kSets * 4 * kBlockM);   // [4 kSets warps] accumulator transposes
 
   const uint32_t warp = threadIdx.x >> 5;
   const uint32_t lane = threadIdx.x & 31;
-  const uint32_t cta_rank = (kCG == 2) ? cluster_ctarank() : 0;
-  const bool leader = (cta_rank == 0);
+  constexpr uint32_t kProducerWarp = 4 * kSets;
 
-  if (warp == 0 && elect_one()) {
+  if (warp == kProducerWarp && elect_one()) {
     tma_prefetch_desc(&tmap_q);
     tma_prefetch_desc(&tmap_g);
   }
-  if (warp == 1 && elect_one()) {
+  if (warp == 0 && elect_one()) {
     for (int s = 0; s < p.stages; ++s) {
-      mbar_init(&b_full[s], kCG);
-      mbar_init(&b_empty[s], 1);
+      mbar_init(&b_full[s], 1);
+      mbar_init(&b_empty[s], 4 * kSets);   // one arrive per consumer warp
     }
-    mbar_init(a_full, kCG);
-    mbar_init(a_empty, 1);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&t_full[b], 1);
-      mbar_init(&t_empty[b], 4 * kSets * kCG);
-    }
+    mbar_init(a_full, 1);
+    mbar_init(a_empty, 4 * kSets);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc<kCG>(tmem_slot, 512);
-    tmem_relinquish<kCG>();
-  }
-  tc_fence_before();
-  __syncthreads();   // CTA-local ordering of the set-up writes (mbarrier init, TMEM slot) for this CTA's own readers ...
-  if constexpr (kCG == 2) cluster_sync();   // ... and the peer CTA's barriers are initialised before any remote arrive
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   if (p.clk && blockIdx.x == 0 && threadIdx.x == 0) {
     p.clk[0] = clock64();
     p.clk[1] = global_timer_ns();
   }
 
   // this unit's tile range
-  const long long n_units = gridDim.x / kCG;
-  const long long unit = blockIdx.x / kCG;
-  const int rows_per_qtile = kBlockM * kCG;
+  const long long n_units = gridDim.x;
+  const long long unit = blockIdx.x;
+  const int rows_per_qtile = kBlockM;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===================================== TMA producer =====================================
-    // The whole warp walks the loop (warp-uniform values stay in uniform registers) and one elected lane issues: under
-    // `if (lane == 0)` every UTMALDG / UTCHMMA gets an ELECT + R2UR + BRA.U.ANY wrapper, and the single-thread
-    // instruction stream is the critical path of the pipeline (tools/microbench/umma_rate.cu).
-    {
-      uint32_t seg = 0;
-      PipeState st(p.stages);
-      SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
-      while (w.next()) {
-        const int qi = w.qi, g_begin = w.g_begin, ntiles = w.ntiles;
-        const int warm = (p.thr_init || w.carried) ? 0 : min(kWarmTiles, ntiles);
-        const int q_row = qi * rows_per_qtile + static_cast<int>(cta_rank) * kBlockM;
-        if (!stream_a) {   // resident query tile
-          mbar_wait(a_empty, (seg & 1) ^ 1);
+    // The whole warp walks the loop (warp-uniform values stay in uniform registers) and one elected lane issues.
+    uint32_t seg = 0;
+    PipeState st(p.stages);
+    SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
+    while (w.next()) {
+      const int qi = w.qi, g_begin = w.g_begin, ntiles = w.ntiles;
+      const int warm = (p.thr_init || w.carried) ? 0 : min(kWarmTiles, ntiles);
+      const int q_row = qi * rows_per_qtile;
+      if (!stream_a) {   // resident query tile
+        mbar_wait(a_empty, (seg & 1) ^ 1);
+        if (elect_one()) {
+          mbar_arrive_expect_tx(a_full, p.num_kb * kATileBytes);
+          for (int kb = 0; kb < p.num_kb; ++kb)
+            tma_load_2d(smem_a + kb * kATileBytes, &tmap_q, a_full, kb * kBlockK, q_row, kEvictNormal);
+        }
+        __syncwarp();
+      }
+      for (int j = 0; j < warm + ntiles; ++j) {
+        const int gi = g_begin + (j < warm ? j : j - warm);
+        const int g_row = gi * kBlockN;
+        for (int kb = 0; kb < p.num_kb; ++kb, st.next()) {
+          const uint32_t s = st.s, ph = st.ph;
+          mbar_wait(&b_empty[s], ph ^ 1);
           if (elect_one()) {
-            if (leader) mbar_arrive_expect_tx(a_full, p.num_kb * kATileBytes * kCG);
-            else mbar_arrive_cluster(a_full, 0);
-            for (int kb = 0; kb < p.num_kb; ++kb)
-              tma_load_2d<kCG>(smem_a + kb * kATileBytes, &tmap_q, a_full, kb * kBlockK, q_row, kEvictNormal);
+            mbar_arrive_expect_tx(&b_full[s], stage_bytes);
+            tma_load_2d(smem_b + s * stage_bytes, &tmap_g, &b_full[s], kb * kBlockK, g_row, kEvictNormal);
+            if (stream_a)
+              tma_load_2d(smem_b + s * stage_bytes + kBTileBytes, &tmap_q, &b_full[s], kb * kBlockK, q_row, kEvictNormal);
           }
           __syncwarp();
         }
-        for (int j = 0; j < warm + ntiles; ++j) {
-          const int gi = g_begin + (j < warm ? j : j - warm);
-          const int g_row = gi * kBlockN + static_cast<int>(cta_rank) * kBRows;
-          if constexpr (kTimingMode == 3) continue;   // timing experiment: no gallery loads at all
-          for (int kb = 0; kb < p.num_kb; ++kb, st.next()) {
-            const uint32_t s = st.s, ph = st.ph;
-            mbar_wait(&b_empty[s], ph ^ 1);
-            if (elect_one()) {
-              if (leader) mbar_arrive_expect_tx(&b_full[s], stage_bytes * kCG);
-              else mbar_arrive_cluster(&b_full[s], 0);
-              tma_load_2d<kCG>(smem_b + s * stage_bytes, &tmap_g, &b_full[s], kb * kBlockK, g_row, kEvictNormal);
-              if (stream_a)
-                tma_load_2d<kCG>(smem_b + s * stage_bytes + kBTileBytes, &tmap_q, &b_full[s], kb * kBlockK, q_row, kEvictNormal);
-            }
-            __syncwarp();
-          }
-        }
-        ++seg;
       }
-    }
-  } else if (warp == 1) {
-    // ===================================== MMA issuer (leader CTA) =====================================
-    if (leader) {
-      constexpr uint32_t idesc = umma_idesc_bf16(kBlockM * kCG, kBlockN);
-      uint32_t seg = 0, tc = 0;
-      PipeState st(p.stages);
-      const uint64_t da0 = umma_desc_sw128(smem_u32(stream_a ? smem_b + kBTileBytes : smem_a));
-      const uint64_t db0 = umma_desc_sw128(smem_u32(smem_b));
-      const uint32_t stage_step = static_cast<uint32_t>(stage_bytes) >> 4;   // descriptor start-address units (16 B)
-      SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
-      while (w.next()) {
-        const int ntiles = w.ntiles;
-        const int warm = (p.thr_init || w.carried) ? 0 : min(kWarmTiles, ntiles);
-        if (!stream_a) {
-          mbar_wait(a_full, seg & 1);
-          tc_fence_after();
-        }
-        for (int j = 0; j < warm + ntiles; ++j, ++tc) {
-          const uint32_t buf = tc & 1;
-          mbar_wait(&t_empty[buf], ((tc >> 1) & 1) ^ 1);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + buf * kBlockN;
-          for (int kb = 0; kb < p.num_kb; ++kb, st.next()) {
-            const uint32_t s = st.s;
-            if constexpr (kTimingMode != 3) mbar_wait(&b_full[s], st.ph);
-            tc_fence_after();
-            const uint64_t da = da0 + static_cast<uint64_t>(stream_a ? s * stage_step : static_cast<uint32_t>(kb) * (kATileBytes >> 4));
-            const uint64_t db = db0 + static_cast<uint64_t>(s * stage_step);
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < kBlockK / 16; ++k)
-                umma_f16<kCG>(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);  // +32 B per K=16 step
-              if constexpr (kTimingMode != 3) umma_commit<kCG>(&b_empty[s]);   // frees this B stage (both CTAs) once the MMAs above retire
-              if (kb == p.num_kb - 1) {
-                umma_commit<kCG>(&t_full[buf]);
-                if (!stream_a && j == warm + ntiles - 1) umma_commit<kCG>(a_empty);
-              }
-            }
-            __syncwarp();
-          }
-        }
-        ++seg;
-      }
+      ++seg;
     }
   } else {
-    // ===================================== epilogue warps =====================================
-    // kSets = 2: two warps per TMEM lane quadrant, each owning one column half ("set") of every accumulator tile and
-    // its own candidate lists / slot -- the filter is issue- and latency-bound with a single warp per sub-partition.
-    const uint32_t quad = warp & 3;             // TMEM lane quadrant this warp may read
-    const uint32_t set = (warp - 2) >> 2;       // column range [set * kSetCols, (set + 1) * kSetCols) of every tile
+    // ===================================== consumer warpgroups =====================================
+    // kSets = 2: two warps per 32-row block, each owning one column half ("set") of every tile and its own candidate
+    // lists / slot -- the filter is issue- and latency-bound with a single warp per sub-partition.
+    const uint32_t quad = warp & 3;             // rows quad*32 .. +31 of the tile
+    const uint32_t set = warp >> 2;             // column range [set * kSetCols, (set + 1) * kSetCols) of every tile
     const uint32_t row = quad * 32 + lane;      // query row inside this CTA's tile
-    constexpr int kSetCols = kBlockN / kSets;
     uint2* set_list = cand + set * p.cap * 128;
     const uint32_t my_list = smem_u32(set_list + row);
     uint2* warp_list = set_list + quad * 32;
-    const uint32_t tmem_row = tmem_base + ((quad * 32u) << 16);
+    const uint32_t xacc = smem_u32(acc_xpose) + warp * kAccXposeWarpBytes;
     float* my_carry = carry + set * 4 * kBlockM;
     const int kp = p.kp, cap = p.cap;
     const float* colbias = kBias ? p.col_bias : nullptr;
-    uint32_t tc = 0, dbg = 0;
+    const uint32_t a_base = smem_u32(stream_a ? smem_b + kBTileBytes : smem_a);
+    const uint32_t b_base = smem_u32(smem_b) + set * kSetCols * 128;
+    const uint32_t a_step = stream_a ? 0u : static_cast<uint32_t>(kATileBytes);   // per k-block (resident query tile)
+    PipeState st(p.stages);
+    uint32_t seg = 0;
     SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
     while (w.next()) {
       const int qi = w.qi, g_begin = w.g_begin, ntiles = w.ntiles;
       const int warm = (p.thr_init || w.carried) ? 0 : min(kWarmTiles, ntiles);
       float thr = -INFINITY;
       if (p.thr_init) {
-        const int qrow_g = qi * rows_per_qtile + static_cast<int>(cta_rank) * kBlockM + static_cast<int>(row);
+        const int qrow_g = qi * rows_per_qtile + static_cast<int>(row);
         thr = qrow_g < p.nq ? p.thr_init[qrow_g] : INFINITY;   // padding rows collect nothing
       }
       // a threshold this row reached on an earlier gallery chunk is a valid (and usually tight) start here
@@ -691,24 +612,44 @@ __global__ void __launch_bounds__(64 + 128 * kSets, 1)
       int cnt = 0;
       // Threshold sharing: a threshold ANY unit reached for this query row (kp recorded scores above it exist somewhere
       // in the gallery) is a valid drop bound for every other unit sweeping the same query tile.  Read once per tile
-      // (the load is issued before the accumulator-ready wait), published when it has risen.
-      const int qrow_s = qi * rows_per_qtile + static_cast<int>(cta_rank) * kBlockM + static_cast<int>(row);
+      // (the load is issued before the main loop), published when it has risen.
+      const int qrow_s = qi * rows_per_qtile + static_cast<int>(row);
       unsigned int* gslot = (p.gthr && qrow_s < p.nq) ? p.gthr + qrow_s : nullptr;
       float published = gslot ? thr_from_key(*reinterpret_cast<volatile unsigned int*>(gslot)) : INFINITY;
       if (gslot) thr = fmaxf(thr, published);
+      if (!stream_a) mbar_wait(a_full, seg & 1);
 
       // one accumulator tile: warm-up tiles only track column-slot maxima, the others feed the candidate lists.  Two
       // separate loops so that the 32 slot registers are dead while the lists are live.
-      auto tile = [&](auto warm_tag, int gi, float (&slot)[32]) {
+      auto tile = [&](auto warm_tag, int gi, bool last, float (&slot)[32]) {
         constexpr bool kWarm = decltype(warm_tag)::value;
         const int gcol0 = gi * kBlockN + static_cast<int>(set) * kSetCols;
         const bool tail = gcol0 + kSetCols > p.ng;
-        const uint32_t buf = tc & 1;
         const float* sb = kBias ? colbias + gcol0 : nullptr;   // per-column offsets: warp-uniform (broadcast) loads
         unsigned int shared_key = 0;
         if (!kWarm && gslot) shared_key = *reinterpret_cast<volatile unsigned int*>(gslot);
-        mbar_wait(&t_full[buf], (tc >> 1) & 1);
-        tc_fence_after();
+        // main loop: the stage of k-block kb is released once wgmma_wait<1> in k-block kb+1 has seen its MMAs complete
+        WgAcc<kSetCols> acc;
+        uint32_t prev_s = 0;
+        for (int kb = 0; kb < p.num_kb; ++kb, st.next()) {
+          const uint32_t s = st.s;
+          mbar_wait(&b_full[s], st.ph);
+          const uint32_t a_addr = a_base + (stream_a ? s * static_cast<uint32_t>(stage_bytes) : static_cast<uint32_t>(kb) * a_step);
+          const uint32_t b_addr = b_base + s * static_cast<uint32_t>(stage_bytes);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kBlockK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), (kb | k) != 0);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (kb > 0 && lane == 0) mbar_arrive(&b_empty[prev_s]);
+          prev_s = s;
+        }
+        wgmma_wait<0>();
+        acc.fence_regs();
+        if (lane == 0) {
+          mbar_arrive(&b_empty[prev_s]);
+          if (!stream_a && last) mbar_arrive(a_empty);
+        }
         if (!kWarm && gslot) {
           if (thr > published) {   // risen since the last publication (compaction): let the other units know
             atomicMax(gslot, thr_key(thr));
@@ -720,43 +661,13 @@ __global__ void __launch_bounds__(64 + 128 * kSets, 1)
             published = other;
           }
         }
-        const uint32_t taddr = tmem_row + buf * kBlockN + set * kSetCols;
-        uint32_t ra[32], rb[32];
-        auto release = [&]() {   // this warp's columns of the accumulator buffer are in registers
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if constexpr (kCG == 2) mbar_arrive_cluster(&t_empty[buf], 0);
-            else mbar_arrive(&t_empty[buf]);
-          }
-        };
-        if constexpr (kTimingMode >= 2) {   // timing experiment: do not even read the accumulator (results are meaningless)
-          release();
-          return;
-        }
-        // TMEM read pipeline: chunk i+1 is in flight while chunk i is scanned
-        tmem_ld_32x32(taddr, ra);
-#pragma unroll 1
-        for (int ch = 0; ch < kSetCols / 32; ch += 2) {
-          tmem_ld_wait_dep(ra);
-          tmem_ld_32x32(taddr + (ch + 1) * 32, rb);
-          if (tail) mask_tail(ra, gcol0 + ch * 32, p.ng);
-          if constexpr (kTimingMode == 0) {
-            if constexpr (kWarm) warm_chunk<false>(ra, sb ? sb + ch * 32 : nullptr, gcol0 + ch * 32, p.ng, slot);
-            else scan_chunk<false>(ra, sb ? sb + ch * 32 : nullptr, gcol0 + ch * 32, p.ng, thr, cnt, my_list, warp_list, kp, cap, lane);
-          } else {
-            dbg ^= ra[0] ^ ra[31];
-          }
-          tmem_ld_wait_dep(rb);
-          if (ch + 2 < kSetCols / 32) tmem_ld_32x32(taddr + (ch + 2) * 32, ra);
-          else release();
-          if (tail) mask_tail(rb, gcol0 + (ch + 1) * 32, p.ng);
-          if constexpr (kTimingMode == 0) {
-            if constexpr (kWarm) warm_chunk<false>(rb, sb ? sb + (ch + 1) * 32 : nullptr, gcol0 + (ch + 1) * 32, p.ng, slot);
-            else scan_chunk<false>(rb, sb ? sb + (ch + 1) * 32 : nullptr, gcol0 + (ch + 1) * 32, p.ng, thr, cnt, my_list, warp_list, kp, cap, lane);
-          } else {
-            dbg ^= rb[0] ^ rb[31];
-          }
+#pragma unroll
+        for (int ch = 0; ch < kSetCols / 32; ++ch) {
+          uint32_t r[32];
+          acc.rows32(ch, r, xacc, lane);
+          if (tail) mask_tail(r, gcol0 + ch * 32, p.ng);
+          if constexpr (kWarm) warm_chunk<false>(r, sb ? sb + ch * 32 : nullptr, gcol0 + ch * 32, p.ng, slot);
+          else scan_chunk<false>(r, sb ? sb + ch * 32 : nullptr, gcol0 + ch * 32, p.ng, thr, cnt, my_list, warp_list, kp, cap, lane);
         }
       };
       if (warm > 0) {
@@ -764,14 +675,15 @@ __global__ void __launch_bounds__(64 + 128 * kSets, 1)
 #pragma unroll
         for (int c = 0; c < 32; ++c) slot[c] = -INFINITY;
 #pragma unroll 1
-        for (int j = 0; j < warm; ++j, ++tc) tile(std::true_type{}, g_begin + j, slot);
+        for (int j = 0; j < warm; ++j) tile(std::true_type{}, g_begin + j, false, slot);
         thr = seed_threshold(slot, kp);
       }
       {
         float unused[32];
 #pragma unroll 1
-        for (int j = 0; j < ntiles; ++j, ++tc) tile(std::false_type{}, g_begin + j, unused);
+        for (int j = 0; j < ntiles; ++j) tile(std::false_type{}, g_begin + j, j == ntiles - 1, unused);
       }
+      ++seg;
       // ---- flush this segment's lists: final compaction to kp, then coalesced copy to the slot ----
       __syncwarp();
       {
@@ -781,21 +693,19 @@ __global__ void __launch_bounds__(64 + 128 * kSets, 1)
       __syncwarp();
       my_carry[(qi & 3) * kBlockM + row] = thr;
       if (gslot && thr > published) atomicMax(gslot, thr_key(thr));
-      const size_t slot_row0 = (static_cast<size_t>(w.slot) * kSets + set) * rows_per_qtile + cta_rank * kBlockM + quad * 32;
+      const size_t slot_row0 = (static_cast<size_t>(w.slot) * kSets + set) * rows_per_qtile + quad * 32;
       for (int L = 0; L < 32; ++L) {
         const int n = __shfl_sync(kFull, cnt, L);
         if (static_cast<int>(lane) < n) p.cand[(slot_row0 + L) * kKPMax + lane] = warp_list[L + lane * 128];
       }
       p.cand_cnt[slot_row0 + lane] = cnt;
-      p.cand_thr[slot_row0 + lane] = (kTimingMode != 0 && dbg == 0x12345678u) ? 0.f : thr;   // keeps `dbg` live in the timing modes
+      p.cand_thr[slot_row0 + lane] = thr;
       __syncwarp();
     }
   }
 
   // teardown
-  tc_fence_before();
-  if constexpr (kCG == 2) cluster_sync(); else __syncthreads();
-  if (warp == 2) tmem_dealloc<kCG>(tmem_base, 512);
+  __syncthreads();
   if (p.clk && blockIdx.x == 0 && threadIdx.x == 0) {
     p.clk[2] = clock64();
     p.clk[3] = global_timer_ns();
@@ -923,7 +833,6 @@ __global__ void __launch_bounds__(128)
   __shared__ int s_n, s_overflow, s_kept, s_nslots, s_off[kMaxSlotsPerQuery], s_cnt[kMaxSlotsPerQuery], s_slot[kMaxSlotsPerQuery];
   __shared__ float s_thr, s_eps, s_qx, s_gn, s_ak, s_nun, s_mun;
   __shared__ double s_qmu, s_kth;
-  __shared__ BlockBest s_bb;
 
   // blockIdx.x indexes the (possibly compacted) query matrix the fused kernel saw; qrow is the caller's row
   const int crow = blockIdx.x;
@@ -1091,8 +1000,8 @@ __global__ void __launch_bounds__(128)
 // stage 3, one WARP per query (four queries per block, no block-wide barrier): the same steps and the same arithmetic
 // as rescore_select_kernel -- identical candidate sets, eps, exact scores, order and certificate -- for passes whose
 // q-tiles are covered by at most 32 candidate slots (a lane per slot; kKPMax = 32 entries per slot: a lane per entry).
-// The block form spent a third of its warp time on barriers behind one thread's slot walk and fetched one gallery row
-// per warp at a time: 171 us for 10k queries x ~14 surviving rows (1.7 TB/s of gathers).
+// The block form spends a third of its warp time on barriers behind one thread's slot walk and fetches one gallery row
+// per warp at a time.
 constexpr int kRescoreWarps = 4;
 
 // two rows, each with exactly the association of exact_dot_warp_qd; both rows' loads are issued before the first fma
@@ -1536,7 +1445,7 @@ struct PassPlan {
 };
 
 struct SimPlan {
-  int cg, d_pad, num_kb, ng_pad, n_gtiles, rows_per_qtile;
+  int d_pad, num_kb, ng_pad, n_gtiles, rows_per_qtile;
   int stream_a;  // d_pad > 512: query tile streamed with the gallery k-blocks
   int max_sets;  // upper bound for PassPlan::n_sets (1 or 2)
   int gchunk, n_chunks;   // preferred gallery chunking (a pass may use fewer chunks)
@@ -1555,18 +1464,17 @@ int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, i
   pp->kp = kp;
   // ---- shared memory: resident A + stages*B + n_sets * cap KB of lists + barriers + carried thresholds ----
   const size_t a_bytes = sp.stream_a ? 0 : static_cast<size_t>(sp.num_kb) * kATileBytes;
-  const size_t b_tile = static_cast<size_t>(kBlockN / sp.cg) * kBlockK * 2 + (sp.stream_a ? kATileBytes : 0);
+  const size_t b_tile = static_cast<size_t>(kBlockN) * kBlockK * 2 + (sp.stream_a ? kATileBytes : 0);
   const size_t fixed = 1024 /*align slack*/ + 256 /*barriers*/ + 4096 /*carried thresholds*/;
-  auto fits = [&](int st, int cp, int sets) {
-    return max_smem >= a_bytes + st * b_tile + static_cast<size_t>(cp) * 1024 * sets + fixed;
-  };
+  auto per_set = [&](int cp) { return static_cast<size_t>(cp) * 1024 + 4 * kAccXposeWarpBytes; };   // lists + transposes
+  auto fits = [&](int st, int cp, int sets) { return max_smem >= a_bytes + st * b_tile + per_set(cp) * sets + fixed; };
   // two epilogue warp sets whenever their lists (at least kp + 8 entries per row and set) fit next to 3 B stages
   int sets = (sp.max_sets >= 2 && fits(3, kp + 8, 2)) ? 2 : 1;
   int cap = kp + (sets == 2 ? 8 : 16);
+  if (!fits(2, cap, sets)) cap = kp + 8;   // d = 512 with k > 10: the resident query tile leaves room for 8 spare entries
   const int cap_max = std::max(cap, std::min(64, env_int("DCR_SIM_CAP", 64)));
   int stages = 2;
-  DCR_REQUIRE(fits(stages, cap, sets), "sim_topk: not enough shared memory (%zu B) for d=%d k=%d cta_group=%d", max_smem,
-              d, k, sp.cg);
+  DCR_REQUIRE(fits(stages, cap, sets), "sim_topk: not enough shared memory (%zu B) for d=%d k=%d", max_smem, d, k);
   // priorities: 3 B stages, then list capacity up to 64 (fewer compactions), then more stages (up to 8)
   if (fits(3, cap, sets)) stages = 3;
   const int want_stages = env_int("DCR_SIM_STAGES", 0);
@@ -1576,7 +1484,7 @@ int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, i
   pp->cap = cap;
   pp->stages = stages;
   pp->n_sets = sets;
-  pp->smem_bytes = fixed + a_bytes + stages * b_tile + static_cast<size_t>(cap) * 1024 * sets;
+  pp->smem_bytes = fixed + a_bytes + stages * b_tile + per_set(cap) * sets;
 
   // ---- gallery chunking and work units ----
   pp->gchunk = sp.gchunk;
@@ -1585,7 +1493,7 @@ int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, i
   long long span_total = 0;
   for (;;) {
     const long long T = static_cast<long long>(pp->n_qtiles) * pp->gchunk;   // tiles of one (full) gallery chunk
-    units = num_sms / sp.cg;
+    units = num_sms;
     if (T < units) units = static_cast<int>(std::max<long long>(1, T));
     // per chunk a q-tile is covered by at most ceil(tiles_in_chunk / (T_c / units)) + 1 units
     span_total = 0;
@@ -1614,22 +1522,19 @@ int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, i
 
 int env_int(const char* name, int dflt) { return tuning_int(name, dflt); }   // honoured only under DCR_B200_TUNING=1
 
-int make_plan(int nq, int ng, int d, int k, int cg, int num_sms, size_t max_smem, SimPlan* pl) {
+int make_plan(int nq, int ng, int d, int k, int num_sms, size_t max_smem, SimPlan* pl) {
   DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "sim_topk: empty problem (nq=%d ng=%d d=%d)", nq, ng, d);
   DCR_REQUIRE(d <= kMaxDim, "sim_topk: descriptor dim %d > %d not supported", d, kMaxDim);
   DCR_REQUIRE(k >= 1 && k <= 16, "sim_topk: k=%d outside [1,16]", k);
   DCR_REQUIRE(k <= ng, "sim_topk: k=%d > gallery size %d", k, ng);
-  DCR_REQUIRE(cg == 1 || cg == 2, "sim_topk: cta group must be 1 or 2");
-  pl->cg = cg;
   pl->d_pad = static_cast<int>(align_up(d, kBlockK));
   pl->num_kb = pl->d_pad / kBlockK;
   pl->stream_a = pl->num_kb > kMaxKB ? 1 : 0;
-  pl->rows_per_qtile = kBlockM * cg;
-  // Two epilogue warp sets (two warps per TMEM lane quadrant, each with its own lists for one column half) pay off when
-  // few candidates are kept: measured on B200 (10k x 100k x 512) k = 1: 0.79 ms vs 0.82 ms and no second-chance pass
-  // (each segment keeps 2 x 4 candidates); k = 10: slower (the lists of two sets only fit with a small capacity).
-  // DCR_SIM_SETS=1|2 overrides.
-  pl->max_sets = (cg == 2) ? std::max(1, std::min(2, env_int("DCR_SIM_SETS", k <= 2 ? 2 : 1))) : 1;
+  pl->rows_per_qtile = kBlockM;
+  // Two consumer warpgroups (two warps per 32-row block, each with its own lists for one column half) when few
+  // candidates are kept (k <= 2: each segment keeps 2 x 4 candidates); with larger k the lists of two sets only fit with
+  // a small capacity.  DCR_SIM_SETS=1|2 overrides.
+  pl->max_sets = std::max(1, std::min(2, env_int("DCR_SIM_SETS", k <= 2 ? 2 : 1)));
   pl->n_gtiles = (ng + kBlockN - 1) / kBlockN;
   pl->ng_pad = pl->n_gtiles * kBlockN;
   // gallery chunks of ~DCR_SIM_CHUNK_MB of bf16 rows: the units sweep one chunk at a time so that it stays L2 resident
@@ -1643,8 +1548,7 @@ int make_plan(int nq, int ng, int d, int k, int cg, int num_sms, size_t max_smem
   pl->n_chunks = n_chunks;
   // first pass keeps few candidates per (query, segment) -- enough unless many gallery rows sit within the error
   // bound of the k-th score; such queries get a second chance with 32 candidates before the brute-force path
-  // k in 6..10 keeps 12 (measured on B200, 10k x 100k x 512, k = 10: 1.20 ms with 16, 1.14 ms with 12, 1.10 ms with 10;
-  // two spare candidates per segment keep the second-chance pass rare)
+  // k in 6..10 keeps 12 (two spare candidates per segment keep the second-chance pass rare)
   int kp0 = (k <= 2) ? 4 : (k <= 5 ? 8 : (k <= 10 ? 12 : 32));
   kp0 = env_int("DCR_SIM_KP0", kp0);
   DCR_REQUIRE(kp0 >= 1 && kp0 <= kKPMax, "sim_topk: DCR_SIM_KP0 must be in [1, 32]");
@@ -1688,10 +1592,6 @@ int make_plan(int nq, int ng, int d, int k, int cg, int num_sms, size_t max_smem
   return 0;
 }
 
-int default_cg() {
-  const int cg = tuning_int("DCR_SIM_CTA_GROUP", 2);
-  return (cg == 1 || cg == 2) ? cg : 2;
-}
 
 struct PassBuffers {
   uint2* cand;
@@ -1705,7 +1605,7 @@ int launch_fused(const SimPlan& pl, const PassPlan& pp, const __nv_bfloat16* qb,
                  unsigned long long* clk, unsigned int* gthr, cudaStream_t stream) {
   CUtensorMap tq, tg;
   if (int rc = make_tmap_2d_bf16(&tq, qb, pp.nq_pad, pl.d_pad, pl.d_pad, kBlockM, kBlockK)) return rc;
-  if (int rc = make_tmap_2d_bf16(&tg, gb, pl.ng_pad, pl.d_pad, pl.d_pad, kBlockN / pl.cg, kBlockK)) return rc;
+  if (int rc = make_tmap_2d_bf16(&tg, gb, pl.ng_pad, pl.d_pad, pl.d_pad, kBlockN, kBlockK)) return rc;
   SimParams p;
   p.nq = pp.nq;
   p.ng = ng;
@@ -1727,35 +1627,21 @@ int launch_fused(const SimPlan& pl, const PassPlan& pp, const __nv_bfloat16* qb,
   p.clk = clk;
   p.gthr = gthr;
   if (gthr) DCR_CUDA_CHECK(cudaMemsetAsync(gthr, 0, static_cast<size_t>(pp.nq_pad) * 4, stream));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(pp.n_units * pl.cg);
-  cfg.blockDim = dim3(64 + 128 * pp.n_sets);
-  cfg.dynamicSmemBytes = pp.smem_bytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = pl.cg;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
   auto launch = [&](auto kern) -> int {
     DCR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pp.smem_bytes)));
-    DCR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tq, tg, p));
+    kern<<<pp.n_units, 32 + 128 * pp.n_sets, pp.smem_bytes, stream>>>(tq, tg, p);
     count_launch();
+    DCR_CUDA_CHECK(cudaGetLastError());
     return 0;
   };
   // the variant without the offset path always runs unless the device flag says otherwise; the offset variant is only
   // launched when query centring is possible at all (it returns immediately when the flag is 0)
-  if (pl.cg == 2 && pp.n_sets == 2) {
-    if (int rc = launch(sim_topk_kernel<2, false, 2>)) return rc;
-    if (col_bias) return launch(sim_topk_kernel<2, true, 2>);
-  } else if (pl.cg == 2) {
-    if (int rc = launch(sim_topk_kernel<2, false, 1>)) return rc;
-    if (col_bias) return launch(sim_topk_kernel<2, true, 1>);
+  if (pp.n_sets == 2) {
+    if (int rc = launch(sim_topk_kernel<false, 2>)) return rc;
+    if (col_bias) return launch(sim_topk_kernel<true, 2>);
   } else {
-    if (int rc = launch(sim_topk_kernel<1, false, 1>)) return rc;
-    if (col_bias) return launch(sim_topk_kernel<1, true, 1>);
+    if (int rc = launch(sim_topk_kernel<false, 1>)) return rc;
+    if (col_bias) return launch(sim_topk_kernel<true, 1>);
   }
   return 0;
 }
@@ -1780,7 +1666,7 @@ int split_rescore(const float* q, const float* g, int nq, int d, int n_chunks, i
 size_t sim_topk_workspace_size(int nq, int ng, int d, int k) {
   const DeviceInfo* di = device_info();
   SimPlan pl;
-  if (make_plan(nq, ng, d, k, default_cg(), di ? di->num_sms : 148, di ? di->max_smem_optin : 232448, &pl) != 0)
+  if (make_plan(nq, ng, d, k, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &pl) != 0)
     return 0;
   return pl.total;
 }
@@ -1790,10 +1676,10 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
              cudaStream_t stream, SimStats* stats) {
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  DCR_REQUIRE(di->cc_major == 10, "sim_topk: this build targets sm_100a; device reports sm_%d%d", di->cc_major, di->cc_minor);
-  const int cg = default_cg();
+  DCR_REQUIRE(di->cc_major == 9 && di->cc_minor == 0, "sim_topk: this build targets sm_90a; device reports sm_%d%d", di->cc_major,
+              di->cc_minor);
   SimPlan pl;
-  if (int rc = make_plan(nq, ng, d, k, cg, di->num_sms, di->max_smem_optin, &pl)) return rc;
+  if (int rc = make_plan(nq, ng, d, k, di->num_sms, di->max_smem_optin, &pl)) return rc;
   DCR_REQUIRE(ws != nullptr && ws_bytes >= pl.total, "sim_topk: workspace too small (%zu < %zu)", ws_bytes, pl.total);
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "sim_topk: workspace must be 256-byte aligned");
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0 && d % 4 == 0,
@@ -1954,8 +1840,8 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
                                                                static_cast<double>(h_clk[3] - h_clk[1]))
                                           : 0.f;
     stats->n_sets = pl.p0.n_sets;
-    stats->cta_group = cg;
-    stats->grid = pl.p0.n_units * cg;
+    stats->cta_group = 1;   // one CTA per work unit (the field stays for callers that read it)
+    stats->grid = pl.p0.n_units;
     stats->smem_bytes = static_cast<int>(pl.p0.smem_bytes);
     stats->stages = pl.p0.stages;
     stats->kp = pl.p0.kp;

@@ -1,7 +1,7 @@
-// ResNet stem (7x7 / stride 2 / pad 3 convolution + BatchNorm + ReLU) as a tcgen05 implicit GEMM whose A operand is an
+// ResNet stem (7x7 / stride 2 / pad 3 convolution + BatchNorm + ReLU) as a wgmma implicit GEMM whose A operand is an
 // OVERLAPPING-WINDOW (Toeplitz) view of the input in shared memory -- every input pixel travels L2 -> shared memory ~1.7
 // times instead of 16 times (conv_gemm.cu's space-to-depth path re-reads each stored pixel once per window position and
-// filter row: 357 us of a 4.07 ms SSCD forward at batch 256, ingest bound; profiles/r01_layers_sscd.txt).
+// filter row, which makes that path ingest bound).
 //
 // Reference call site: `model(samples)` (utils_ret.py:751) -> torchvision ResNet conv1 / bn1 / relu of the SSCD trunk.
 //
@@ -13,14 +13,14 @@
 // position m = y * PW + x the A operand of K-chunk (a, e, b) is the SAME linear array shifted by (a * PW + b) units: in a
 // K-major SWIZZLE_NONE shared-memory descriptor rows are 16 bytes apart (stride-dimension offset 128 B per 8 rows) and
 // the second 16-byte K chunk of an instruction sits leading-dimension-offset = 16 bytes further -- i.e. row m+1 and
-// K-chunk b+1 address the same bytes.  tools/microbench/toeplitz_probe.cu verifies the hardware accepts this.
+// K-chunk b+1 address the same bytes.
 // Positions with x >= OW (PW - OW per row) are junk and dropped by the epilogue.
 //
-// Roles (352 threads, persistent over tiles of 512 positions = 4 MMA row blocks):
-//   warp 0   producer: two cp.async.bulk copies per tile (the even / odd plane windows, 512 + 3*PW + 3 units each)
-//   warps 1, 10   tcgen05.mma issuers (alternate row blocks): 16 x (128 x 64 x 16) per row block, weights (64 x 256, 32 KB,
-//            128B swizzle) resident
-//   warps 2-9 epilogue: TMEM -> BN affine + ReLU -> bf16 -> staging -> coalesced NHWC stores of the valid positions
+// Roles (288 threads, persistent over tiles of 512 positions = 4 MMA row blocks):
+//   warps 0-7 two consumer warpgroups, warpgroup h owns output channels [32h, 32h+32): per row block 16 x two
+//            m64 x 32 x 16 wgmma (weights 64 x 256, 32 KB, 128B swizzle, resident) -> BN affine + ReLU -> bf16 -> staging
+//            -> coalesced NHWC stores of the valid positions
+//   warp 8   producer: two cp.async.bulk copies per tile (the even / odd plane windows, 512 + 3*PW + 3 units each)
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -37,7 +37,7 @@ namespace {
 constexpr int kSN = 64;                   // output channels
 constexpr int kSTile = 512;               // positions per tile
 constexpr int kSBlocks = kSTile / 128;    // MMA row blocks per tile
-constexpr int kSThreads = 352;             // warp 0 producer, warps 1 and 10 MMA issuers, warps 2-9 epilogue
+constexpr int kSThreads = 288;             // warps 0-7 MMA + epilogue, warp 8 producer
 constexpr int kWBytes = kSN * 256 * 2;    // resident weights: 4 k-blocks of [64 rows x 128 B]
 
 struct StemParams {
@@ -58,12 +58,12 @@ struct StemParams {
 };
 
 DCR_DEVICE uint64_t desc_nosw(uint32_t addr) {
-  // K-major, SWIZZLE_NONE: 8-row x 16-byte core matrices; LBO (next K chunk) = 16 B, SBO (next 8 rows) = 128 B
+  // K-major, no swizzle: 8-row x 16-byte core matrices; LBO (next K chunk) = 16 B, SBO (next used 8-row group) = 256 B:
+  // each m64 half of a WgAcc takes every other 8-row group (the odd groups start 128 B later)
   uint64_t d = 0;
   d |= static_cast<uint64_t>((addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(16 >> 4) << 16;
-  d |= static_cast<uint64_t>(128 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
+  d |= static_cast<uint64_t>(256 >> 4) << 32;
   return d;
 }
 
@@ -98,41 +98,30 @@ __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_co
   uint8_t* s_win = s_w + kWBytes;                               // win_stages x [even | odd]
   uint8_t* s_out = s_win + p.win_stages * stage_bytes;          // 2 x [128 positions x 128 B] | kPool: ring of 8 conv rows
   const int ring_row_bytes = p.OW * 128;
-  float* sb = reinterpret_cast<float*>(s_out + (kPool ? ((8 * ring_row_bytes + 1023) & ~1023) : 2 * 16384));   // scale[64] | bias[64]
+  uint8_t* acc_xpose = s_out + (kPool ? ((8 * ring_row_bytes + 1023) & ~1023) : 2 * 16384);   // [8 warps]
+  float* sb = reinterpret_cast<float*>(acc_xpose + 8 * kAccXposeWarpBytes);   // scale[64] | bias[64]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sb + 128);
   uint64_t* w_full = bars;
   uint64_t* win_full = bars + 1;      // [4]
   uint64_t* win_empty = bars + 5;     // [4]
-  uint64_t* t_full = bars + 9;        // [2][4]
-  uint64_t* t_empty = bars + 17;      // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 19);
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) tma_prefetch_desc(&tmap_w);
-  if (warp == 1 && lane == 0) {
+  if (warp == 8 && lane == 0) tma_prefetch_desc(&tmap_w);
+  if (warp == 0 && lane == 0) {
     mbar_init(w_full, 1);
     for (int s = 0; s < 4; ++s) {
       mbar_init(&win_full[s], 1);
-      mbar_init(&win_empty[s], 2);   // both MMA issuers commit once per tile
+      mbar_init(&win_empty[s], 8);   // one arrive per consumer warp and tile
     }
-    for (int s = 0; s < 8; ++s) mbar_init(&t_full[s], 1);
-    for (int s = 0; s < 2; ++s) mbar_init(&t_empty[s], 8);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc<1>(tmem_slot, 512);
-    tmem_relinquish<1>();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================================== producer =====================================
     if (elect_one()) {
       mbar_arrive_expect_tx(w_full, kWBytes);
-      for (int kb = 0; kb < 4; ++kb) tma_load_2d<1>(s_w + kb * 8192, &tmap_w, w_full, kb * 64, 0, kEvictLast);
+      for (int kb = 0; kb < 4; ++kb) tma_load_2d(s_w + kb * 8192, &tmap_w, w_full, kb * 64, 0, kEvictLast);
     }
     __syncwarp();
     PipeState ws(p.win_stages);
@@ -151,59 +140,18 @@ __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_co
         __syncwarp();
       }
     }
-  } else if (warp == 1 || warp == 10) {
-    // ===================================== MMA issuers =====================================
-    // Two issuing warps on separate accumulators: one thread issues a 128x64x16 tcgen05.mma every ~90 cycles at best (the
-    // tensor core needs 32), so the row blocks of a tile alternate between two issuers (tools/microbench/umma_rate.cu).
-    const int issuer = (warp == 1) ? 0 : 1;
-    constexpr uint32_t idesc = umma_idesc_bf16(128, kSN);
-    mbar_wait(w_full, 0);
-    tc_fence_after();
-    const uint64_t dw0 = umma_desc_sw128(smem_u32(s_w));
-    const uint32_t win0 = smem_u32(s_win);
-    PipeState ws(p.win_stages);
-    uint32_t tc = 0;
-    const uint32_t PW = static_cast<uint32_t>(p.PW);
-    int my_tiles = 0;
-    for (int unit = blockIdx.x; unit < p.num_units; unit += gridDim.x) my_tiles += p.tiles_per_unit;
-    for (int it = 0; it < my_tiles; ++it, ++tc, ws.next()) {
-      const uint32_t buf = tc & 1;
-      mbar_wait(&win_full[ws.s], ws.ph);
-      mbar_wait(&t_empty[buf], ((tc >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t wbase = win0 + ws.s * stage_bytes;
-#pragma unroll 1
-      for (int mb = issuer; mb < kSBlocks; mb += 2) {
-        const uint32_t tmem_d = tmem_base + (buf * kSBlocks + mb) * kSN;
-        if (elect_one()) {
-#pragma unroll
-          for (int a = 0; a < 4; ++a) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-#pragma unroll
-              for (int bp = 0; bp < 2; ++bp) {
-                // A: positions mb*128.., shifted by filter row pair a and column pair 2*bp (units of 16 B)
-                const uint32_t a_addr = wbase + e * win_bytes + (mb * 128 + a * PW + 2 * bp) * 16;
-                const int kc = (a * 2 + e) * 2 + bp;                 // K = 16 chunk of the weights
-                const uint64_t db = dw0 + static_cast<uint64_t>((kc >> 2) * (8192 >> 4) + (kc & 3) * 2);
-                umma_f16<1>(tmem_d, desc_nosw(a_addr), db, idesc, kc != 0);
-              }
-            }
-          }
-          umma_commit<1>(&t_full[buf * kSBlocks + mb]);
-          if (mb + 2 >= kSBlocks) umma_commit<1>(&win_empty[ws.s]);   // this issuer's last row block of the tile
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp < 10) {
-    // ===================================== epilogue warps =====================================
-    const uint32_t ewarp = warp - 2;
+  } else {
+    // ===================================== consumer warpgroups =====================================
+    const uint32_t ewarp = warp;
     const uint32_t quad = warp & 3;
-    const uint32_t half = ewarp >> 2;                 // 32-column half of the 64 channels
+    const uint32_t half = ewarp >> 2;                 // 32-column half of the 64 channels (= warpgroup)
     const uint32_t row = quad * 32 + lane;            // position inside the row block
     const uint32_t etid = ewarp * 32 + lane;
-    const uint32_t tmem_row = tmem_base + ((quad * 32u) << 16);
+    const uint32_t xacc = smem_u32(acc_xpose) + warp * kAccXposeWarpBytes;
+    const uint32_t win0 = smem_u32(s_win);
+    const uint32_t PW = static_cast<uint32_t>(p.PW);
+    const uint64_t dw0 = wgmma_desc_sw128(smem_u32(s_w) + half * 32 * 128);
+    PipeState ws(p.win_stages);
     const uint32_t sb_addr = smem_u32(sb), so_addr = smem_u32(s_out);
     for (int c = etid; c < kSN; c += 256) {
       st_shared_f32(sb_addr + c * 4, p.scale ? p.scale[c] : 1.f);
@@ -219,6 +167,7 @@ __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_co
       bi[c] = b4.x; bi[c + 1] = b4.y; bi[c + 2] = b4.z; bi[c + 3] = b4.w;
     }
     const int positions = p.OH * p.PW;
+    mbar_wait(w_full, 0);
     uint32_t tc = 0, blk = 0;
     for (int unit = blockIdx.x; unit < p.num_units; unit += gridDim.x) {
       const int b = unit / p.units_per_img;
@@ -230,21 +179,34 @@ __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_co
       int next_yp = part * p.prow_per_part;
       const int yp_end = min(p.OHp, next_yp + p.prow_per_part);
       if constexpr (kPool) asm volatile("bar.sync 2, 256;" ::: "memory");   // nobody still pools the previous unit's rows
-      for (int t = 0; t < p.tiles_per_unit; ++t, ++tc) {
+      for (int t = 0; t < p.tiles_per_unit; ++t, ++tc, ws.next()) {
         const int m0 = mu + t * kSTile;
-        const uint32_t buf = tc & 1;
+        mbar_wait(&win_full[ws.s], ws.ph);
+        const uint32_t wbase = win0 + ws.s * stage_bytes;
 #pragma unroll 1
         for (int mb = 0; mb < kSBlocks; ++mb, ++blk) {
-          mbar_wait(&t_full[buf * kSBlocks + mb], (tc >> 1) & 1);
-          tc_fence_after();
-          uint32_t r[32];
-          tmem_ld_32x32(tmem_row + (buf * kSBlocks + mb) * kSN + half * 32, r);
-          tmem_ld_wait_regs(r);
-          if (mb == kSBlocks - 1) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&t_empty[buf]);
+          WgAcc<32> acc;
+          wgmma_fence();
+#pragma unroll
+          for (int a = 0; a < 4; ++a) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+#pragma unroll
+              for (int bp = 0; bp < 2; ++bp) {
+                // A: positions mb*128.., shifted by filter row pair a and column pair 2*bp (units of 16 B)
+                const uint32_t a_addr = wbase + e * win_bytes + (mb * 128 + a * PW + 2 * bp) * 16;
+                const int kc = (a * 2 + e) * 2 + bp;                 // K = 16 chunk of the weights
+                const uint64_t db = dw0 + static_cast<uint64_t>((kc >> 2) * (8192 >> 4) + (kc & 3) * 2);
+                acc.mma2(desc_nosw(a_addr), desc_nosw(a_addr + 128), db, kc != 0);
+              }
+            }
           }
+          wgmma_commit();
+          wgmma_wait<0>();
+          acc.fence_regs();
+          if (mb == kSBlocks - 1 && lane == 0) mbar_arrive(&win_empty[ws.s]);
+          uint32_t r[32];
+          acc.rows32(0, r, xacc, lane);
           uint4 v[4];
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
@@ -336,9 +298,6 @@ __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_co
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<1>(tmem_base, 512);
 }
 
 // ---- input kernel: uint8 HWC (or fp32 NCHW) image -> the two column-parity planes ----------------------------------------
@@ -460,7 +419,8 @@ int stem_conv(const __nv_bfloat16* planes, int B, int OH, int OW, const __nv_bfl
               __nv_bfloat16* out, cudaStream_t stream, int pool) {
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  DCR_REQUIRE(di->cc_major == 10, "stem_conv: this build targets sm_100a; device reports sm_%d%d", di->cc_major, di->cc_minor);
+  DCR_REQUIRE(di->cc_major == 9 && di->cc_minor == 0, "stem_conv: this build targets sm_90a; device reports sm_%d%d", di->cc_major,
+              di->cc_minor);
   if (B == 0) return 0;
   StemParams p;
   memset(&p, 0, sizeof(p));
@@ -494,8 +454,10 @@ int stem_conv(const __nv_bfloat16* planes, int B, int OH, int OW, const __nv_bfl
   if (int rc = make_tmap_2d_bf16(&tw, weight, kSN, 256, 256, kSN, 64)) return rc;
   const size_t stage = (static_cast<size_t>(2) * p.win_units * 16 + 1023) & ~size_t(1023);
   const size_t out_bytes = pool ? ((static_cast<size_t>(8) * OW * 128 + 1023) & ~size_t(1023)) : 2 * 16384;
-  const size_t fixed = 1024 + kWBytes + out_bytes + 512 + 256;
-  DCR_REQUIRE(fixed + 2 * stage <= di->max_smem_optin, "stem_conv: image too wide for the window buffers (OW = %d)", OW);
+  const size_t fixed = 1024 + kWBytes + out_bytes + 8 * kAccXposeWarpBytes + 512 + 256;
+  // with the pooling ring of a 224-pixel image only one window stage fits: the next tile's window is loaded once the
+  // current tile's MMAs have completed
+  DCR_REQUIRE(fixed + stage <= di->max_smem_optin, "stem_conv: image too wide for the window buffers (OW = %d)", OW);
   p.win_stages = static_cast<int>(std::min<size_t>(4, (di->max_smem_optin - fixed) / stage));
   const size_t smem = fixed + p.win_stages * stage;
   static bool attr_set[64][2] = {};

@@ -1,4 +1,4 @@
-"""FID on the B200 path: the host mirror of metrics/fid.py.
+"""FID on the H100 path: the host mirror of metrics/fid.py.
 
     get_activations / calculate_activation_statistics   metrics/fid.py:76-139, 199-221
         -> ActivationStatistics: Inception pool3 features computed by the dcr_net executor are folded, batch by batch,

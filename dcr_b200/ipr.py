@@ -1,4 +1,4 @@
-"""Improved Precision & Recall on the B200 path: the host mirror of metrics/ipr.py (imported by diff_retrieval.py:587).
+"""Improved Precision & Recall on the H100 path: the host mirror of metrics/ipr.py (imported by diff_retrieval.py:587).
 
     IPR(batch_size, k, num_samples, model)      metrics/ipr.py:33-181   same methods and return types
     compute_manifold -> Manifold(features, radii)           :80-122
@@ -6,7 +6,7 @@
     realism                                                 :71-77, 253-263
 
 What changes underneath:
-  * the VGG-16 fc2 features (:124-147) come from the dcr_net executor (nets.build_vgg16_fc2: tcgen05 implicit-GEMM convs);
+  * the VGG-16 fc2 features (:124-147) come from the dcr_net executor (nets.build_vgg16_fc2: wgmma implicit-GEMM convs);
   * the N x N (and N x M) float64 distance matrices of compute_pairwise_distances (:184-217) are never built.  Both uses of
     them are nearest-neighbour questions, answered by the fused similarity + top-k kernel on augmented vectors:
         -d(x,y)^2 / 2 + ||x||^2 / 2 = x.y - ||y||^2 / 2            = [x, 1] . [y, -||y||^2 / 2]              (k-th NN radius)

@@ -9,7 +9,7 @@ Host-side mirror of the reference's model zoo for the hot path:
         VisionTransformer(patch 16, dim 384, depth 12, heads 6)            dino_vits.py:171-289
 
 Each builder takes a state_dict (real weights when the user has them, seeded random weights in the tests), folds
-BatchNorm into a per-channel affine, lays the weights out for the tcgen05 GEMM kernel and records the op list.
+BatchNorm into a per-channel affine, lays the weights out for the wgmma GEMM kernel and records the op list.
 `forward` takes a uint8 NHWC image batch on the GPU and returns fp32 descriptors -- the resize/crop/ToTensor/
 Normalize of diff_retrieval.py:325-330 is fused into the first op.
 """
@@ -31,8 +31,8 @@ OP_IM2COL_U8, OP_CONV, OP_MAXPOOL, OP_AVGPOOL, OP_GEM, OP_GAP, OP_LAYERNORM, OP_
 # exact: three planes, products accumulated in float64 on the CUDA cores (correctly rounded fp32 layer outputs).
 # "s2d": 7x7/2 stem as a 4x4 window convolution over a space-to-depth tensor (conv_gemm.cu, every mode);
 # "toeplitz": fused stem kernel with overlapping-window operand descriptors (stem_fused.cu, fast mode);
-# "toeplitz_pool": the same with the 3x3/2 max pool taken in its epilogue (default of the fast mode: measured on B200 at
-# batch 256, input kernel + conv + pool: 471 us (s2d) -> 300 us (toeplitz) -> 230 us (toeplitz_pool))
+# "toeplitz_pool": the same with the 3x3/2 max pool taken in its epilogue (default of the fast mode: the stem activation
+# never reaches HBM)
 DEFAULT_STEM = "toeplitz_pool"
 PRECISION_PLANES = {"fast": 1, "bf16": 1, "parity": 3, "fp32": 3, "bf16x3": 2, "exact": 3}
 
@@ -43,7 +43,7 @@ class DcrNet:
     def __init__(self, max_batch: int, precision: str = "fast", device: Optional[torch.device] = None):
         self.lib = _lib.load()
         if not torch.cuda.is_available():
-            raise _lib.DcrError("dcr_b200 networks need a CUDA (sm_100a) device; there is no CPU path")
+            raise _lib.DcrError("dcr_b200 networks need a CUDA (sm_90a) device; there is no CPU path")
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self.max_batch = int(max_batch)
         self.planes = PRECISION_PLANES[precision]
@@ -277,7 +277,7 @@ def _dense_from_grouped(w: torch.Tensor, c_in: int) -> torch.Tensor:
     [N, c_in, kh, kw].  The tensor cores then run the grouped 3x3 convs of a ResNeXt trunk as ordinary dense
     implicit GEMMs (zeros included): `groups` times the arithmetic of the grouped form, but at the widths involved
     (128..1024 channels) that is still tensor-bound work at full tile efficiency, where per-group GEMMs with 4..32
-    output channels would use a few percent of a UMMA tile."""
+    output channels would use a few percent of a wgmma tile."""
     n, cpg, kh, kw = w.shape
     if cpg == c_in:
         return w

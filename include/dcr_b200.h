@@ -1,8 +1,8 @@
 /*
- * dcr_b200.h -- C ABI of libdcr_b200.so: the B200 (sm_100a) replacement for DCR's embed -> match -> top-k (+FID)
+ * dcr_b200.h -- C ABI of libdcr_b200.so: the H100 (sm_90a) replacement for DCR's embed -> match -> top-k (+FID)
  * hot path.  Plain pointers and sizes only; no torch / CUDA types in any signature.
  *
- * The reference (somepago/DCR, /root/reference) is pure Python and has no FFI layer; each entry point below names
+ * The reference (somepago/DCR) is pure Python and has no FFI layer; each entry point below names
  * the reference call site it replaces (file:line).  A Python maintainer binds these with ctypes (INTEGRATION.md).
  *
  * Conventions
@@ -13,7 +13,7 @@
  *     result back (dcr_sim_topk: the count of queries that needed the exact fallback) synchronise that stream
  *     before returning.
  *   - workspaces are caller-owned device buffers, 256-byte aligned, sized by the matching *_workspace_size().
- *   - the library never falls back to the CPU: on a machine without an sm_100 device every compute call fails with
+ *   - the library never falls back to the CPU: on a machine without an sm_90 device every compute call fails with
  *     a message.
  */
 #ifndef DCR_B200_H_
@@ -118,7 +118,7 @@ int dcr_split_rescore(const float* q, const float* g, int nq, int d, int n_chunk
                       int n_cand, int k, float* out_scores, int64_t* out_idx, void* stream);
 
 /* ---- dense contraction of the descriptor networks ------------------------------------------------------------- */
-/* y = act(scale[n] * conv2d(x, w)[.., n] + bias[n] (+ residual)) as a tcgen05 implicit GEMM.
+/* y = act(scale[n] * conv2d(x, w)[.., n] + bias[n] (+ residual)) as a wgmma implicit GEMM.
  *   x        NHWC bf16, `x_planes` planes of B*H*W*C elements each (plane p at x + p*x_plane_stride elements);
  *            C % 8 == 0.  A Linear layer is the case H = W = kh = kw = 1, B = rows.
  *   w        prepared weights: bf16 [w_planes][N][kh*kw*ceil64(C)], tap-major, channels zero-padded to 64
@@ -179,7 +179,7 @@ int dcr_conv2d_bf16(const void* x, int x_planes, int64_t x_plane_stride, int B, 
 typedef struct dcr_net dcr_net;
 int dcr_net_create(int max_batch, int planes, dcr_net** out);
 /* on != 0: every CONV op accumulates its products in float64 on the CUDA cores (correctly rounded fp32 layer outputs,
- * the mode the parity tests use against the fp32 oracle); needs planes == 3.  Default 0: tcgen05 tensor cores. */
+ * the mode the parity tests use against the fp32 oracle); needs planes == 3.  Default 0: wgmma tensor cores. */
 int dcr_net_set_exact(dcr_net* net, int on);
 void dcr_net_destroy(dcr_net* net);
 /* A second executor of a fully described network: its own activation buffers, the same uploaded parameters (reference

@@ -1,4 +1,4 @@
-"""GPU numerics: the tcgen05 implicit-GEMM convolution vs torch.nn.functional.conv2d (fp32, TF32 off)."""
+"""GPU numerics: the wgmma implicit-GEMM convolution vs torch.nn.functional.conv2d (fp32, TF32 off)."""
 import numpy as np
 import pytest
 import torch
@@ -132,57 +132,16 @@ def test_conv3x3_halo_path(shape, act, monkeypatch):
     assert (got != gen_got).float().mean().item() < 0.02
 
 
-PAIR_SHAPES = [   # (M rows as B x H x W, C = K, N, residual, act): plain GEMMs for the cta_group::2 form
-    ((4, 14, 14), 1024, 256, False, 1),     # layer3 reduce: 7 m-tiles (odd: rank 1 of the last pair works a tile past M)
-    ((2, 7, 7), 512, 2048, True, 1),        # layer4 expansion with residual: 128-wide pair tiles, ragged last m-tile
-    ((600, 1, 1), 1536, 384, True, 0),      # ViT fc2 + residual: N = 3 x 128
-    ((600, 1, 1), 384, 1152, False, 0),     # ViT qkv: N = 4.5 x 256 (the last pair tile's second W half is past N)
-    ((600, 1, 1), 384, 1536, False, 2),     # ViT fc1 + GELU
-    ((300, 1, 1), 64, 128, False, 0),       # one k-block
-    ((2, 5, 5), 320, 136, True, 1),         # K not a multiple of 64, N not a multiple of 64
-]
-
-
-@pytest.mark.parametrize("shape", PAIR_SHAPES)
-def test_cta_pair_gemm_matches_single_cta(shape, monkeypatch):
-    """gemm_bf16_kernel<..., kCG = 2> (two CTAs per 256-row tile, UMMA 256 x BN x 16, half a W tile per CTA) against the
-    single-CTA kernel: same products, same k order into one fp32 accumulator, same epilogue -> the same bf16 tensor bit
-    for bit; and both against the float64 reference."""
-    (b, h, w_), c, n, with_res, act = shape
-    gen = torch.Generator(device="cuda").manual_seed(c + n + b)
-    x = torch.randn(b, h, w_, c, device="cuda", generator=gen)
-    w = torch.randn(n, c, 1, 1, device="cuda", generator=gen) / c ** 0.5
-    scale = 0.5 + torch.rand(n, device="cuda", generator=gen)
-    bias = torch.randn(n, device="cuda", generator=gen) * 0.1
-    res = torch.randn(b, h, w_, n, device="cuda", generator=gen) if with_res else None
-    xp, wp = ops.split_planes(x, 1), ops.prepare_conv_weight(w, 1)
-    rp = ops.split_planes(res, 1) if with_res else None
-    monkeypatch.setenv("DCR_B200_TUNING", "1")
-    monkeypatch.setenv("DCR_GEMM_CG2", "0")
-    one, _ = ops.conv2d(xp, wp, n, 1, 1, 1, 0, 0, scale=scale, bias=bias, residual=rp, act=act)
-    torch.cuda.synchronize()
-    monkeypatch.setenv("DCR_GEMM_CG2", "1")
-    two, _ = ops.conv2d(xp, wp, n, 1, 1, 1, 0, 0, scale=scale, bias=bias, residual=rp, act=act)
-    again, _ = ops.conv2d(xp, wp, n, 1, 1, 1, 0, 0, scale=scale, bias=bias, residual=rp, act=act)
-    torch.cuda.synchronize()
-    assert torch.equal(one, two), f"pair form differs: {(ops.merge_planes(one) - ops.merge_planes(two)).abs().max().item()}"
-    assert torch.equal(two, again)
-    ref = _ref(ops.merge_planes(xp), ops.merge_planes(wp).reshape(n, 1, 1, -1)[..., :c].permute(0, 3, 1, 2), scale, bias,
-               ops.merge_planes(rp) if with_res else None, act, 1, (0, 0))
-    mx = max(1.0, ref.abs().max().item())
-    assert (ops.merge_planes(two) - ref).abs().max().item() < (2 ** -8 + 3e-4) * mx
-
-
 @pytest.mark.parametrize("shape", [
     ((600, 1, 1), 1536, 384, 1, 1, 0, True, 0),     # plain GEMM, three column blocks, residual
     ((3, 28, 28), 128, 512, 3, 2, 1, False, 1),    # strided 3x3 through TMA im2col, four column blocks
-    ((4, 14, 14), 1024, 512, 1, 1, 0, False, 1),   # two 256-wide column blocks (CTA-pair form when forced)
+    ((4, 14, 14), 1024, 512, 1, 1, 0, False, 1),   # two 256-wide column blocks
 ])
-@pytest.mark.parametrize("pair", ["0", "1"])
-def test_tile_order_does_not_change_results(shape, pair, monkeypatch):
+@pytest.mark.parametrize("direct", ["0", "1"])
+def test_tile_order_does_not_change_results(shape, direct, monkeypatch):
     """n-fastest tile order (chosen when A is larger than L2: consecutive tiles share an m-tile's rows) against the default
-    m-fastest order, in the single-CTA and the CTA-pair kernel: every tile computes the same thing, only who computes it
-    and when changes."""
+    m-fastest order, with the TMA-store epilogue and with the direct epilogue: every tile computes the same thing, only who
+    computes it and when changes."""
     (b, h, w_), c, n, k, stride, pad, with_res, act = shape
     gen = torch.Generator(device="cuda").manual_seed(c + n + k)
     x = torch.randn(b, h, w_, c, device="cuda", generator=gen)
@@ -193,7 +152,8 @@ def test_tile_order_does_not_change_results(shape, pair, monkeypatch):
     xp, wp = ops.split_planes(x, 1), ops.prepare_conv_weight(w, 1)
     rp = ops.split_planes(res, 1) if with_res else None
     monkeypatch.setenv("DCR_B200_TUNING", "1")
-    monkeypatch.setenv("DCR_GEMM_CG2", pair)
+    if direct == "1":
+        monkeypatch.setenv("DCR_GEMM_DIRECT_EPILOGUE", "1")
     outs = []
     for order in ("0", "1"):
         monkeypatch.setenv("DCR_GEMM_TILE_ORDER", order)

@@ -1,5 +1,5 @@
 """Whole-network throughput of the SSCD ResNet-50 (fast mode) as a function of the batch size: tile / wave quantisation of the
-persistent kernels (148 SMs) makes some batch sizes better operating points than others."""
+persistent kernels (one CTA per SM) makes some batch sizes better operating points than others."""
 import os
 import sys
 
