@@ -13,8 +13,10 @@
 //                            accumulator registers, warp-cooperative compaction in shared memory)
 //   3. rescore_select_kernel exact re-score (fp64 accumulate, fixed order) of the <= slots*kp candidates per query,
 //                            final order (score desc, gallery index asc), plus a per-query certificate that no
-//                            non-candidate can reach the k-th exact score.  Queries failing the certificate are
-//                            recomputed by brute force in fp64 (exact_scan_kernel / exact_select_kernel).
+//                            non-candidate can reach the k-th exact score.  One kernel body, two widths: a warp per
+//                            query when a q-tile has few candidate slots, the whole 128-thread block otherwise; both
+//                            compute the same values.  Queries failing the certificate are recomputed by brute force in
+//                            fp64 (exact_scan_kernel / exact_select_kernel).
 // Result: indices identical to ranking all G exact dot products with ties broken by lowest index.
 #include <cuda_bf16.h>
 
@@ -432,17 +434,27 @@ DCR_DEVICE float seed_threshold(float (&slot)[32], int kp) {
   return thr;
 }
 
-// Work decomposition shared by the three warp roles (and mirrored by rescore_select_kernel): for every gallery chunk
-// c (chunks are L2-sized so that the units, which all sweep chunk c at about the same time, share its tiles in L2)
-// the (q-tile, g-tile-in-chunk) grid is linearised q-major and cut into n_units equal contiguous ranges; a unit's range
-// is walked as segments = maximal runs inside one q-tile.  Thresholds carry over from chunk to chunk: `carried` says
-// that this unit finished a segment of the same q-tile before (its final per-row thresholds are valid lower bounds, so
-// no warm-up replay is needed).
+// Work decomposition shared by the three warp roles and rescore_select_kernel: for every gallery chunk c (chunks are
+// L2-sized so that the units, which all sweep chunk c at about the same time, share its tiles in L2) the
+// (q-tile, g-tile-in-chunk) grid is linearised q-major into T tiles and cut into n_units equal contiguous ranges, unit u
+// owning [u*T/U, (u+1)*T/U); a unit's range is walked as segments = maximal runs inside one q-tile.
+
+// owner unit of linear tile t
+DCR_DEVICE long long owner_unit(long long t, long long T, long long U) { return ((t + 1) * U + T - 1) / T - 1; }
+
+// Candidate slot of the segment (chunk, unit, q-tile qi) and epilogue set: the q-tiles of a unit's range never lie below
+// those of the previous unit, so unit + qi is distinct within a chunk and below n_units + n_qtiles.
+DCR_DEVICE int slot_index(int chunk, int unit, int qi, int set, int n_units, int n_qtiles, int n_sets) {
+  return (chunk * (n_units + n_qtiles) + unit + qi) * n_sets + set;
+}
+
+// Thresholds carry over from chunk to chunk: `carried` says that this unit finished a segment of the same q-tile before
+// (its final per-row thresholds are valid lower bounds, so no warm-up replay is needed).
 struct SegWalker {
   int n_qtiles, n_gtiles, gchunk, n_chunks;
   long long unit, n_units;
   // current segment
-  int chunk, qi, g_begin, ntiles, slot;
+  int chunk, qi, g_begin, ntiles;
   bool carried;
   // state
   long long t, t_end;
@@ -470,7 +482,6 @@ struct SegWalker {
     g_begin = g_lo + static_cast<int>(t % ncg);
     const long long seg_end = min(t_end, static_cast<long long>(qi + 1) * ncg);
     ntiles = static_cast<int>(seg_end - t);
-    slot = chunk * (static_cast<int>(n_units) + n_qtiles) + static_cast<int>(unit) + qi;
     const int s4 = qi & 3;
     const int tg = s4 == 0 ? tag[0] : (s4 == 1 ? tag[1] : (s4 == 2 ? tag[2] : tag[3]));
     carried = (tg == qi);
@@ -693,7 +704,9 @@ __global__ void __launch_bounds__(32 + 128 * kSets, 1)
       __syncwarp();
       my_carry[(qi & 3) * kBlockM + row] = thr;
       if (gslot && thr > published) atomicMax(gslot, thr_key(thr));
-      const size_t slot_row0 = (static_cast<size_t>(w.slot) * kSets + set) * rows_per_qtile + quad * 32;
+      const int slot = slot_index(w.chunk, static_cast<int>(unit), qi, static_cast<int>(set), static_cast<int>(n_units),
+                                  p.n_qtiles, kSets);
+      const size_t slot_row0 = static_cast<size_t>(slot) * rows_per_qtile + quad * 32;
       for (int L = 0; L < 32; ++L) {
         const int n = __shfl_sync(kFull, cnt, L);
         if (static_cast<int>(lane) < n) p.cand[(slot_row0 + L) * kKPMax + lane] = warp_list[L + lane * 128];
@@ -757,15 +770,7 @@ DCR_DEVICE double exact_dot_warp_qd(const double* __restrict__ a_smem, const flo
   return acc;
 }
 
-// owner unit of linear tile t  (units own [u*T/U, (u+1)*T/U) )
-DCR_DEVICE long long owner_unit(long long t, long long T, long long U) { return ((t + 1) * U + T - 1) / T - 1; }
-
-// block-wide arg-best over (score desc, index asc); entries with taken[i] != 0 are skipped
-struct Best {
-  double s;
-  long long i;
-  int pos;
-};
+// order (score desc, index asc)
 DCR_DEVICE bool better(double s, long long i, double bs, long long bi) { return (s > bs) || (s == bs && i < bi); }
 
 // block-wide arg-best over (key desc, index asc) of 128 threads; every thread passes its local best (pos < 0 = none)
@@ -804,205 +809,6 @@ DCR_DEVICE void block_argbest(double& bs, long long& bi, int& bp, BlockBest* sb,
     }
   __syncthreads();
 }
-
-// stage 3: one block (128 threads) per query.
-//   1. gather the (gallery row, approximate score) candidates of every segment slot of this query's q-tile
-//   2. prune: with A_k the k-th largest approximate score, a candidate below A_k - 2*eps cannot be in the exact
-//      top-k (its exact score is < A_k - eps <= the exact scores of the k best-approximate candidates)
-//   3. exact fp64 scores of the survivors, selection by (score desc, index asc)
-//   4. certificate against the rows the fused kernel dropped; failures are appended to `flagged` together with
-//      a threshold for the second-chance pass (thr_next).
-__global__ void __launch_bounds__(128)
-    rescore_select_kernel(const float* __restrict__ q, const float* __restrict__ g, int nq, int ng, int d, int k,
-                          int n_qtiles, int n_gtiles, int gchunk, int n_chunks, int n_units, int rows_per_qtile,
-                          int n_sets, int d_pad, const uint2* __restrict__ cand, const int* __restrict__ cand_cnt,
-                          const float* __restrict__ cand_thr, const int* __restrict__ qmap,
-                          const float* __restrict__ mu, const float* __restrict__ nu, const int* __restrict__ nu_flag,
-                          const float* __restrict__ q_norm_hat,
-                          const float* __restrict__ q_norm_res, const float* __restrict__ q_norm_x,
-                          const unsigned int* __restrict__ g_max,
-                          long long g_index_base, long long g_index_stride, float* __restrict__ out_scores,
-                          long long* __restrict__ out_idx, int* __restrict__ flagged, int* __restrict__ n_flagged,
-                          float* __restrict__ thr_next, int max_cand) {
-  extern __shared__ __align__(16) uint8_t sm[];
-  double* qs = reinterpret_cast<double*>(sm);                          // [d] the query row, widened once
-  double* sc = qs + ((d + 1) & ~1);                                    // [max_cand] scratch keys / exact scores
-  int* ci = reinterpret_cast<int*>(sc + max_cand);                      // [max_cand] gallery rows of all candidates
-  float* ap = reinterpret_cast<float*>(ci + max_cand);                  // [max_cand] approximate scores
-  int* kc = reinterpret_cast<int*>(ap + max_cand);                      // [max_cand] gallery rows of the survivors
-  __shared__ int s_n, s_overflow, s_kept, s_nslots, s_off[kMaxSlotsPerQuery], s_cnt[kMaxSlotsPerQuery], s_slot[kMaxSlotsPerQuery];
-  __shared__ float s_thr, s_eps, s_qx, s_gn, s_ak, s_nun, s_mun;
-  __shared__ double s_qmu, s_kth;
-
-  // blockIdx.x indexes the (possibly compacted) query matrix the fused kernel saw; qrow is the caller's row
-  const int crow = blockIdx.x;
-  const int qrow = qmap ? qmap[crow] : crow;
-  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int c = threadIdx.x; c < d; c += blockDim.x) qs[c] = q[static_cast<size_t>(qrow) * d + c];
-
-  const int qi = crow / rows_per_qtile, r = crow % rows_per_qtile;
-  if (threadIdx.x == 0) {
-    int n = 0, overflow = 0, ns = 0;
-    float thr = -INFINITY;
-    for (int c = 0; c < n_chunks; ++c) {      // mirror of SegWalker: which (chunk, unit) segments cover this q-tile
-      const int g_lo = c * gchunk;
-      const int ncg = min(gchunk, n_gtiles - g_lo);
-      const long long T = static_cast<long long>(n_qtiles) * ncg;
-      const long long u_lo = owner_unit(static_cast<long long>(qi) * ncg, T, n_units);
-      const long long u_hi = owner_unit(static_cast<long long>(qi + 1) * ncg - 1, T, n_units);
-      for (long long us = u_lo * n_sets; us < (u_hi + 1) * n_sets; ++us) {   // n_sets candidate slots per segment
-        const int slot = (c * (n_units + n_qtiles) + static_cast<int>(us / n_sets) + qi) * n_sets + static_cast<int>(us % n_sets);
-        const size_t sr = static_cast<size_t>(slot) * rows_per_qtile + r;
-        int cc = cand_cnt[sr];
-        thr = fmaxf(thr, cand_thr[sr]);
-        if (n + cc > max_cand || ns >= kMaxSlotsPerQuery) {   // cannot happen with make_plan's bounds
-          cc = 0;
-          overflow = 1;
-        }
-        if (ns < kMaxSlotsPerQuery) {
-          s_off[ns] = n;
-          s_cnt[ns] = cc;
-          s_slot[ns] = slot;
-          ++ns;
-        }
-        n += cc;
-      }
-    }
-    s_nslots = ns;
-    s_n = n;
-    s_thr = thr;
-    s_overflow = overflow;
-    s_kept = 0;
-    // eps bounds |tensor-core score of (bf16 q, bf16 (g-mu)) - q.(g-mu)| for this query from the measured norms
-    // (DESIGN.md section 4): bf16 rounding of both operands, fp32 accumulation, fp32 rounding of g - mu.
-    const float g_norm = __uint_as_float(g_max[0]), g_res = __uint_as_float(g_max[1]);
-    const float qh = q_norm_hat[qrow], qr = q_norm_res[qrow], qx = q_norm_x[qrow];
-    s_eps = 1.001f * (qh * g_res + qr * g_norm) + d_pad * 2.4e-7f * qh * (g_norm + g_res) + 1e-30f;
-    s_qx = qx;
-    s_gn = g_norm;
-  }
-  __syncthreads();
-  if (warp == 1) {   // ||nu||: fp32 roundings of q - nu, g - mu, the offset nu.(g - mu) and its addition
-    float acc = 0.f;
-    if (nu && nu_flag && *nu_flag)
-      for (int c = lane; c < d; c += 32) acc += nu[c] * nu[c];
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(kFull, acc, off);
-    if (lane == 0) {
-      s_nun = sqrtf(acc) * 1.001f;
-      s_eps += 3e-7f * (s_qx + s_nun) * s_gn;
-    }
-  }
-  if (warp == 0) {   // q . mu in fp64: the constant the centred approximate scores are offset by
-    double acc = 0.0;
-    float mu2 = 0.f;
-    if (mu)
-      for (int c = lane; c < d; c += 32) {
-        acc = fma(qs[c], static_cast<double>(mu[c]), acc);
-        mu2 = fmaf(mu[c], mu[c], mu2);
-      }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      acc += __shfl_xor_sync(kFull, acc, off);
-      mu2 += __shfl_xor_sync(kFull, mu2, off);
-    }
-    if (lane == 0) {
-      s_qmu = acc;
-      s_mun = sqrtf(mu2) * 1.001f;
-    }
-  }
-  const int nslots = s_nslots;
-  for (int t = threadIdx.x; t < nslots * kKPMax; t += blockDim.x) {
-    const int s = t / kKPMax, j = t % kKPMax;
-    if (j < s_cnt[s]) {
-      const size_t sr = static_cast<size_t>(s_slot[s]) * rows_per_qtile + r;
-      const uint2 e = cand[sr * kKPMax + j];
-      ci[s_off[s] + j] = static_cast<int>(e.y);
-      ap[s_off[s] + j] = __uint_as_float(e.x);
-    }
-  }
-  __syncthreads();
-  const int n = s_n;
-  const int kk = min(k, n);
-
-  // ---- prune by approximate score ----
-  // A_k = k-th largest approximate score, found by rank counting (n is a few dozen: one pass, one barrier, instead of k
-  // block-wide arg-max rounds)
-  if (threadIdx.x == 0) s_ak = -INFINITY;
-  __syncthreads();
-  for (int c = threadIdx.x; c < n; c += blockDim.x) {
-    const float v = ap[c];
-    int rank = 0;
-    for (int j = 0; j < n; ++j) {
-      const float o = ap[j];
-      rank += (o > v) || (o == v && j < c);
-    }
-    if (rank == kk - 1) s_ak = v;
-  }
-  __syncthreads();
-  const float a_k = s_ak;
-  const float cut = a_k - 2.f * s_eps - 1e-6f * fabsf(a_k);
-  for (int c = threadIdx.x; c < n; c += blockDim.x)
-    if (n <= k || ap[c] >= cut) kc[atomicAdd(&s_kept, 1)] = ci[c];
-  __syncthreads();
-  const int m = s_kept;
-
-  // ---- exact scores of the survivors, then selection by (score desc, index asc): again by rank counting ----
-  for (int c = warp; c < m; c += 4) {
-    const double v = exact_dot_warp_qd(qs, g + static_cast<size_t>(kc[c]) * d, d, lane);
-    if (lane == 0) sc[c] = v;
-  }
-  if (threadIdx.x == 0) s_kth = -INFINITY;
-  __syncthreads();
-  const int km = min(k, m);
-  for (int c = threadIdx.x; c < m; c += blockDim.x) {
-    const double v = sc[c];
-    const int iv = kc[c];
-    int rank = 0;
-    for (int j = 0; j < m; ++j) {
-      const double o = sc[j];
-      const int io = kc[j];
-      rank += (o > v) || (o == v && (io < iv || (io == iv && j < c)));   // candidate rows are distinct; j < c only for safety
-    }
-    if (rank < km) {
-      out_scores[static_cast<size_t>(qrow) * k + rank] = static_cast<float>(v);
-      out_idx[static_cast<size_t>(qrow) * k + rank] = g_index_base + g_index_stride * iv;
-      if (rank == km - 1) s_kth = v;
-    }
-  }
-  __syncthreads();
-  const double kth = (km > 0) ? s_kth : -INFINITY;
-  if (threadIdx.x == 0) {
-    // certificate: every gallery row g that is not a candidate has approximate centred score <= s_thr, hence exact
-    // score q.g <= s_thr + eps + q.mu
-    const bool closed = s_thr > -INFINITY;   // some segment dropped rows
-    // fp64 rounding of kth and q.mu themselves (each a d-term dot of vectors no longer than (|q'| + |nu|), (|g'| + |mu|)):
-    // irrelevant next to eps except when the centred gallery is (nearly) zero -- all rows identical -- and eps with it
-    const double slack = 4.6e-16 * (d + 8) * static_cast<double>(s_qx + s_nun) * static_cast<double>(s_gn + s_mun);
-    const bool ok = (n >= k) && (m >= k) && !s_overflow &&
-                    (!closed || kth > static_cast<double>(s_thr) + static_cast<double>(s_eps) + s_qmu + slack);
-    if (!ok) {
-      const int pos = atomicAdd(n_flagged, 1);
-      flagged[pos] = qrow;
-      if (thr_next) {
-        // every row of the true top-k has exact score >= kth, hence centred approximate score >= kth - q.mu - eps
-        float t = -INFINITY;
-        if (m >= k && kth > -INFINITY) {
-          const double lo = kth - s_qmu - static_cast<double>(s_eps);
-          t = static_cast<float>(lo) - 2e-6f * fabsf(static_cast<float>(lo)) - 1e-7f;
-        }
-        thr_next[pos] = t;
-      }
-    }
-  }
-}
-
-// stage 3, one WARP per query (four queries per block, no block-wide barrier): the same steps and the same arithmetic
-// as rescore_select_kernel -- identical candidate sets, eps, exact scores, order and certificate -- for passes whose
-// q-tiles are covered by at most 32 candidate slots (a lane per slot; kKPMax = 32 entries per slot: a lane per entry).
-// The block form spends a third of its warp time on barriers behind one thread's slot walk and fetches one gallery row
-// per warp at a time.
-constexpr int kRescoreWarps = 4;
 
 // two rows, each with exactly the association of exact_dot_warp_qd; both rows' loads are issued before the first fma
 DCR_DEVICE void exact_dot_warp_qd2(const double* __restrict__ a_smem, const float* __restrict__ b0,
@@ -1066,123 +872,221 @@ DCR_DEVICE void exact_dot_warp_qd2(const double* __restrict__ a_smem, const floa
   out1 = acc1;
 }
 
-__global__ void __launch_bounds__(32 * kRescoreWarps)
-    rescore_select_warp_kernel(const float* __restrict__ q, const float* __restrict__ g, int nq_pass, int d, int k,
-                               int n_qtiles, int n_gtiles, int gchunk, int n_chunks, int n_units, int rows_per_qtile,
-                               int n_sets, int d_pad, const uint2* __restrict__ cand, const int* __restrict__ cand_cnt,
-                               const float* __restrict__ cand_thr, const int* __restrict__ qmap,
-                               const float* __restrict__ mu, const float* __restrict__ nu, const int* __restrict__ nu_flag,
-                               const float* __restrict__ q_norm_hat, const float* __restrict__ q_norm_res,
-                               const float* __restrict__ q_norm_x, const unsigned int* __restrict__ g_max,
-                               long long g_index_base, long long g_index_stride, float* __restrict__ out_scores,
-                               long long* __restrict__ out_idx, int* __restrict__ flagged, int* __restrict__ n_flagged,
-                               float* __restrict__ thr_next, int max_cand) {
-  extern __shared__ __align__(16) uint8_t sm[];
-  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int crow = blockIdx.x * kRescoreWarps + static_cast<int>(warp);
-  if (crow >= nq_pass) return;   // whole warps leave; nothing below synchronises the block
-  const int d2 = (d + 1) & ~1, mc = (max_cand + 3) & ~3;
-  uint8_t* base = sm + static_cast<size_t>(warp) * (static_cast<size_t>(d2) * 8 + static_cast<size_t>(mc) * 20);
-  double* qs = reinterpret_cast<double*>(base);     // [d2] the query row, widened once
-  double* sc = qs + d2;                              // [mc] exact scores of the survivors
-  int* ci = reinterpret_cast<int*>(sc + mc);         // [mc] gallery rows of all candidates
-  float* ap = reinterpret_cast<float*>(ci + mc);     // [mc] approximate scores
-  int* kc = reinterpret_cast<int*>(ap + mc);         // [mc] gallery rows of the survivors
-  const int qrow = qmap ? qmap[crow] : crow;
-  // the query row: requested first, consumed after the slot walk below has issued its own loads (one memory round trip for
-  // both instead of one after the other)
-  const bool q_fast = (d & 127) == 0 && d <= 512;
-  float4 qv[4];
-  if (q_fast) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-      if (i * 128 < d) qv[i] = *reinterpret_cast<const float4*>(q + static_cast<size_t>(qrow) * d + lane * 4 + i * 128);
-  }
+// ------------------------------------------------------------------------------------------------------------
+// stage 3: exact re-score, selection and certificate.  A group of kThreads threads serves one query: a warp (kThreads =
+// 32, four queries per block, no block-wide barrier) or the whole 128-thread block.  Both widths run this one body, so
+// they gather the same candidates and compute the same eps, exact scores, order and certificate.
+//   1. gather the (gallery row, approximate score) candidates of every segment slot of this query's q-tile
+//   2. prune: with A_k the k-th largest approximate score, a candidate below A_k - 2*eps cannot be in the exact
+//      top-k (its exact score is < A_k - eps <= the exact scores of the k best-approximate candidates)
+//   3. exact fp64 scores of the survivors, selection by (score desc, index asc)
+//   4. certificate against the rows the fused kernel dropped; failures are appended to `flagged` together with
+//      a threshold for the second-chance pass (thr_next).
+constexpr int kRescoreThreads = 128;   // block size of both widths
 
-  // ---- which (chunk, unit, set) slots cover this q-tile (mirror of SegWalker): lane c owns chunk c, then lane s slot s ----
-  const int qi = crow / rows_per_qtile, r = crow % rows_per_qtile;
-  int my_lo = 0, my_cnt = 0;
-  if (static_cast<int>(lane) < n_chunks) {
-    const int g_lo = lane * gchunk;
-    const int ncg = min(gchunk, n_gtiles - g_lo);
-    const long long T = static_cast<long long>(n_qtiles) * ncg;
-    const long long u_lo = owner_unit(static_cast<long long>(qi) * ncg, T, n_units);
-    const long long u_hi = owner_unit(static_cast<long long>(qi + 1) * ncg - 1, T, n_units);
-    my_lo = static_cast<int>(u_lo);
-    my_cnt = static_cast<int>(u_hi - u_lo + 1) * n_sets;
+struct RescoreParams {
+  const float* q;                   // the caller's query rows [*][d]
+  const float* g;                   // [ng][d]
+  int nq;                           // queries of this pass: rows of the (possibly compacted) matrix the fused kernel saw
+  int d, d_pad, k;
+  int n_qtiles, n_gtiles, gchunk, n_chunks, n_units, n_sets;   // the fused pass's work decomposition
+  int max_cand;                     // candidates one query may gather (sizes its shared memory)
+  const uint2* cand;                // the fused pass's slots: SimParams::cand, cand_cnt, cand_thr
+  const int* cand_cnt;
+  const float* cand_thr;
+  const int* qmap;                  // pass row -> caller's row; null = identity
+  const float* mu;                  // gallery centre; null = no centring
+  const float* nu;                  // query centre, used when *nu_flag != 0; null = none
+  const int* nu_flag;
+  const float* q_norm_hat;          // per caller row, from stage 1
+  const float* q_norm_res;
+  const float* q_norm_x;
+  const unsigned int* g_max;        // [2] from stage 1
+  long long g_index_base, g_index_stride;
+  float* out_scores;                // [*][k] by caller row
+  long long* out_idx;
+  int* flagged;                     // caller rows whose certificate failed, counted by *n_flagged
+  int* n_flagged;
+  float* thr_next;                  // per flagged entry: start threshold of the second-chance pass; null = last pass
+};
+
+// One query's shared memory: the query row widened to fp64, then four arrays of max_cand entries.  Every part is a
+// multiple of 16 bytes, so the four queries of a 32-wide block lie back to back.
+struct RescoreSmem {
+  size_t sc, ci, ap, kc, bytes;   // byte offsets of: exact scores (fp64), candidate rows, approximate scores, survivor rows
+  __host__ __device__ RescoreSmem(int d, int max_cand) {
+    const size_t d2 = (static_cast<size_t>(d) + 1) & ~size_t(1), mc = (static_cast<size_t>(max_cand) + 3) & ~size_t(3);
+    sc = d2 * 8;
+    ci = sc + mc * 8;
+    ap = ci + mc * 4;
+    kc = ap + mc * 4;
+    bytes = kc + mc * 4;
   }
-  int ns = 0, my_slot = -1;
-  for (int c = 0; c < n_chunks; ++c) {
-    const int lo = __shfl_sync(kFull, my_lo, c), cnt = __shfl_sync(kFull, my_cnt, c);
-    const int rel = static_cast<int>(lane) - ns;
-    if (rel >= 0 && rel < cnt) my_slot = (c * (n_units + n_qtiles) + lo + rel / n_sets + qi) * n_sets + rel % n_sets;
-    ns += cnt;
-  }
-  int cc = 0;
-  float thr = -INFINITY;
-  if (my_slot >= 0) {
-    const size_t sr = static_cast<size_t>(my_slot) * rows_per_qtile + r;
-    cc = cand_cnt[sr];
-    thr = cand_thr[sr];
-  }
-  if (q_fast) {
+};
+
+// Collectives of a group.  Every thread of the group calls them; the 128-wide forms go through a 4-entry shared array.
+template <int kThreads>
+DCR_DEVICE void group_sync() {
+  if constexpr (kThreads == 32) __syncwarp();
+  else __syncthreads();
+}
+
+// float or double; fmax ignores NaN
+template <int kThreads, typename T>
+DCR_DEVICE T group_max(T v) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      if (i * 128 < d) {
-        double* dst = qs + lane * 4 + i * 128;
-        *reinterpret_cast<double2*>(dst) = make_double2(static_cast<double>(qv[i].x), static_cast<double>(qv[i].y));
-        *reinterpret_cast<double2*>(dst + 2) = make_double2(static_cast<double>(qv[i].z), static_cast<double>(qv[i].w));
-      }
-    }
-  } else {
-    for (int c = lane; c < d; c += 32) qs[c] = static_cast<double>(q[static_cast<size_t>(qrow) * d + c]);
+  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(kFull, v, o));
+  if constexpr (kThreads > 32) {
+    __shared__ T part[4];
+    __syncthreads();   // the previous call's readers are done
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+    __syncthreads();
+    v = fmax(fmax(part[0], part[1]), fmax(part[2], part[3]));
   }
-  int off = cc;   // inclusive prefix sum of the slot counts
+  return v;
+}
+
+// exclusive prefix sum over the group in thread order; total = the group's sum
+template <int kThreads>
+DCR_DEVICE int group_scan(int v, int& total) {
+  const int lane = threadIdx.x & 31;
+  int incl = v;
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(kFull, off, o);
-    if (static_cast<int>(lane) >= o) off += t;
+    const int t = __shfl_up_sync(kFull, incl, o);
+    if (lane >= o) incl += t;
   }
-  const int n_total = __shfl_sync(kFull, off, 31);
-  off -= cc;
+  total = __shfl_sync(kFull, incl, 31);
+  if constexpr (kThreads == 32) {
+    return incl - v;
+  } else {
+    __shared__ int part[4];
+    const int w = threadIdx.x >> 5;
+    __syncthreads();
+    if (lane == 0) part[w] = total;
+    __syncthreads();
+    for (int i = 0; i < w; ++i) incl += part[i];
+    total = part[0] + part[1] + part[2] + part[3];
+    return incl - v;
+  }
+}
+
+template <int kThreads>
+__global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const RescoreParams p) {
+  constexpr int kWarps = kThreads / 32;
+  extern __shared__ __align__(16) uint8_t sm[];
+  const int tid = static_cast<int>(threadIdx.x) % kThreads;
+  const uint32_t lane = threadIdx.x & 31;
+  const int warp = tid >> 5;   // warp of the group
+  const int grp = static_cast<int>(threadIdx.x) / kThreads;
+  // crow indexes the (possibly compacted) query matrix the fused kernel saw; qrow is the caller's row
+  const int crow = blockIdx.x * (kRescoreThreads / kThreads) + grp;
+  if (crow >= p.nq) return;   // whole groups leave; nothing below synchronises across groups
+  const RescoreSmem L(p.d, p.max_cand);
+  uint8_t* base = sm + grp * L.bytes;
+  double* qs = reinterpret_cast<double*>(base);          // [d] the query row, widened once
+  double* sc = reinterpret_cast<double*>(base + L.sc);   // exact scores of the survivors
+  int* ci = reinterpret_cast<int*>(base + L.ci);         // gallery rows of all candidates
+  float* ap = reinterpret_cast<float*>(base + L.ap);     // approximate scores
+  int* kc = reinterpret_cast<int*>(base + L.kc);         // gallery rows of the survivors
+  const int d = p.d, k = p.k;
+  const int qrow = p.qmap ? p.qmap[crow] : crow;
+  // the query row: requested first, consumed after the slot walk below has issued its own loads (one memory round trip for
+  // both instead of one after the other).  Thread t owns the 16-byte granules t, t + kThreads, ... of the first 512 dims.
+  constexpr int kQv = 512 / (4 * kThreads);
+  float4 qv[kQv];
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) thr = fmaxf(thr, __shfl_xor_sync(kFull, thr, o));
-  const bool overflow = ns > 32 || n_total > max_cand;   // cannot happen: the host picks this kernel for <= 32 slots
-  const int n = overflow ? 0 : n_total;
-  const int nsl = min(ns, 32);
-#pragma unroll 4
-  for (int s = 0; s < nsl; ++s) {
-    const int c_s = overflow ? 0 : __shfl_sync(kFull, cc, s), off_s = __shfl_sync(kFull, off, s);
-    const int slot_s = __shfl_sync(kFull, my_slot, s);
-    if (static_cast<int>(lane) < c_s) {
-      const uint2 e = cand[(static_cast<size_t>(slot_s) * rows_per_qtile + r) * kKPMax + lane];
-      ci[off_s + lane] = static_cast<int>(e.y);
-      ap[off_s + lane] = __uint_as_float(e.x);
-    }
+  for (int i = 0; i < kQv; ++i) {
+    const int c = (i * kThreads + tid) * 4;
+    if (c < d) qv[i] = *reinterpret_cast<const float4*>(p.q + static_cast<size_t>(qrow) * d + c);   // d % 4 == 0
   }
 
+  // ---- the (chunk, unit, set) slots that cover this q-tile, in rounds: lane c owns chunk c0 + c (every warp of the group
+  // holds the same 32 chunks), then thread t owns slot s0 + t; prefix sums of the slot counts place the entries ----
+  const int qi = crow / kBlockM, r = crow % kBlockM;
+  int n = 0;
+  bool overflow = false;
+  float thr = -INFINITY;
+  for (int c0 = 0; c0 < p.n_chunks; c0 += 32) {
+    const int chunk = c0 + static_cast<int>(lane);
+    int u_lo = 0, n_cs = 0;   // this lane's chunk: first unit whose range covers q-tile qi, and the chunk's slot count
+    if (chunk < p.n_chunks) {
+      const int ncg = min(p.gchunk, p.n_gtiles - chunk * p.gchunk);
+      const long long T = static_cast<long long>(p.n_qtiles) * ncg;
+      u_lo = static_cast<int>(owner_unit(static_cast<long long>(qi) * ncg, T, p.n_units));
+      n_cs = (static_cast<int>(owner_unit(static_cast<long long>(qi + 1) * ncg - 1, T, p.n_units)) - u_lo + 1) * p.n_sets;
+    }
+    int n_slots;
+    const int first = group_scan<32>(n_cs, n_slots);
+    const int nc = min(32, p.n_chunks - c0);
+    for (int s0 = 0; s0 < n_slots; s0 += kThreads) {
+      const int s = s0 + tid;
+      int slot = -1;
+      for (int c = 0; c < nc; ++c) {
+        const int rel = s - __shfl_sync(kFull, first, c), cnt = __shfl_sync(kFull, n_cs, c), lo = __shfl_sync(kFull, u_lo, c);
+        if (rel >= 0 && rel < cnt) slot = slot_index(c0 + c, lo + rel / p.n_sets, qi, rel % p.n_sets, p.n_units, p.n_qtiles, p.n_sets);
+      }
+      int cc = 0;
+      if (slot >= 0) {
+        const size_t sr = static_cast<size_t>(slot) * kBlockM + r;
+        cc = p.cand_cnt[sr];
+        thr = fmaxf(thr, p.cand_thr[sr]);
+      }
+      int n_round;
+      const int off = n + group_scan<kThreads>(cc, n_round);
+      overflow |= n + n_round > p.max_cand;   // cannot happen: plan_pass sizes max_cand for kp entries in every slot
+      if (!overflow) {
+        // each warp copies its own threads' slots, a lane per entry (kKPMax = 32 entries per slot)
+        const int nsl = min(32, n_slots - s0 - warp * 32);
+#pragma unroll 4
+        for (int j = 0; j < nsl; ++j) {
+          const int c_j = __shfl_sync(kFull, cc, j), off_j = __shfl_sync(kFull, off, j), slot_j = __shfl_sync(kFull, slot, j);
+          if (static_cast<int>(lane) < c_j) {
+            const uint2 e = p.cand[(static_cast<size_t>(slot_j) * kBlockM + r) * kKPMax + lane];
+            ci[off_j + lane] = static_cast<int>(e.y);
+            ap[off_j + lane] = __uint_as_float(e.x);
+          }
+        }
+      }
+      n += n_round;
+    }
+  }
+  if (overflow) n = 0;   // k >= 1: the certificate fails and the query is flagged
+  thr = group_max<kThreads>(thr);
+#pragma unroll
+  for (int i = 0; i < kQv; ++i) {
+    const int c = (i * kThreads + tid) * 4;
+    if (c < d) {
+      *reinterpret_cast<double2*>(qs + c) = make_double2(static_cast<double>(qv[i].x), static_cast<double>(qv[i].y));
+      *reinterpret_cast<double2*>(qs + c + 2) = make_double2(static_cast<double>(qv[i].z), static_cast<double>(qv[i].w));
+    }
+  }
+  for (int c = 512 + tid; c < d; c += kThreads) qs[c] = static_cast<double>(p.q[static_cast<size_t>(qrow) * d + c]);
+  group_sync<kThreads>();
+
   // eps bounds |tensor-core score of (bf16 q, bf16 (g-mu)) - q.(g-mu)| for this query from the measured norms
-  // (DESIGN.md section 4); same expression, same order of operations as the block form
-  const float g_norm = __uint_as_float(g_max[0]), g_res = __uint_as_float(g_max[1]);
-  const float qh = q_norm_hat[qrow], qr = q_norm_res[qrow], qx = q_norm_x[qrow];
-  float eps = 1.001f * (qh * g_res + qr * g_norm) + d_pad * 2.4e-7f * qh * (g_norm + g_res) + 1e-30f;
+  // (DESIGN.md section 4): bf16 rounding of both operands, fp32 accumulation, fp32 rounding of g - mu.  Every warp of
+  // the group computes eps, ||nu||, ||mu|| and q.mu itself.
+  const float g_norm = __uint_as_float(p.g_max[0]), g_res = __uint_as_float(p.g_max[1]);
+  const float qh = p.q_norm_hat[qrow], qr = p.q_norm_res[qrow], qx = p.q_norm_x[qrow];
+  float eps = 1.001f * (qh * g_res + qr * g_norm) + p.d_pad * 2.4e-7f * qh * (g_norm + g_res) + 1e-30f;
   float nun = 0.f, mun = 0.f;   // |nu|, |mu| (upper bounds)
   {
+    // ||nu||: fp32 roundings of q - nu, g - mu, the offset nu.(g - mu) and its addition
     float acc = 0.f;
-    if (nu && nu_flag && *nu_flag)
-      for (int c = lane; c < d; c += 32) acc += nu[c] * nu[c];
+    if (p.nu && p.nu_flag && *p.nu_flag)
+      for (int c = lane; c < d; c += 32) acc += p.nu[c] * p.nu[c];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
     nun = sqrtf(acc) * 1.001f;
     eps += 3e-7f * (qx + nun) * g_norm;
   }
-  __syncwarp();
   double qmu = 0.0;   // q . mu in fp64: the constant the centred approximate scores are offset by
-  if (mu) {
+  if (p.mu) {
     float mu2 = 0.f;
     for (int c = lane; c < d; c += 32) {
-      qmu = fma(qs[c], static_cast<double>(mu[c]), qmu);
-      mu2 = fmaf(mu[c], mu[c], mu2);
+      qmu = fma(qs[c], static_cast<double>(p.mu[c]), qmu);
+      mu2 = fmaf(p.mu[c], p.mu[c], mu2);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -1191,11 +1095,18 @@ __global__ void __launch_bounds__(32 * kRescoreWarps)
     }
     mun = sqrtf(mu2) * 1.001f;
   }
+  // certificate: every gallery row that is not a candidate has approximate centred score <= thr, hence exact score
+  // q.g <= thr + eps + q.mu.  `slack` covers the fp64 rounding of kth and q.mu themselves (each a d-term dot of vectors
+  // no longer than (|q'| + |nu|), (|g'| + |mu|)): irrelevant next to eps except when the centred gallery is (nearly)
+  // zero -- all rows identical -- and eps with it
+  const bool closed = thr > -INFINITY;   // some segment dropped rows
+  const double slack = 4.6e-16 * (d + 8) * static_cast<double>(qx + nun) * static_cast<double>(g_norm + mun);
+  const double bound = static_cast<double>(thr) + static_cast<double>(eps) + qmu + slack;
 
-  // ---- prune by approximate score: A_k by rank counting ----
+  // ---- prune by approximate score: A_k by rank counting (n is a few dozen: one pass instead of k arg-max rounds) ----
   const int kk = min(k, n);
   float a_k = -INFINITY;
-  for (int c = lane; c < n; c += 32) {
+  for (int c = tid; c < n; c += kThreads) {
     const float v = ap[c];
     int rank = 0;
     for (int j = 0; j < n; ++j) {
@@ -1204,76 +1115,70 @@ __global__ void __launch_bounds__(32 * kRescoreWarps)
     }
     if (rank == kk - 1) a_k = v;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) a_k = fmaxf(a_k, __shfl_xor_sync(kFull, a_k, o));
+  a_k = group_max<kThreads>(a_k);
   const float cut = a_k - 2.f * eps - 1e-6f * fabsf(a_k);
   int m = 0;
-  for (int c0 = 0; c0 < n; c0 += 32) {
-    const int c = c0 + lane;
+  for (int c0 = 0; c0 < n; c0 += kThreads) {
+    const int c = c0 + tid;
     const bool keep = c < n && (n <= k || ap[c] >= cut);
-    const uint32_t mask = __ballot_sync(kFull, keep);
-    if (keep) kc[m + __popc(mask & ((1u << lane) - 1u))] = ci[c];
-    m += __popc(mask);
+    int kept;
+    const int pos = m + group_scan<kThreads>(keep ? 1 : 0, kept);
+    if (keep) kc[pos] = ci[c];
+    m += kept;
   }
-  __syncwarp();
+  group_sync<kThreads>();
   // every surviving row's cache lines are requested at once (L2 prefetch): the dot products below then wait for L2, not for
   // one DRAM round trip per pair of rows
   {
     const int lines = (d * 4 + 127) / 128;
-    for (int t = lane; t < m * lines; t += 32) {
-      const float* ptr = g + static_cast<size_t>(kc[t / lines]) * d + (t % lines) * 32;
+    for (int t = tid; t < m * lines; t += kThreads) {
+      const float* ptr = p.g + static_cast<size_t>(kc[t / lines]) * d + (t % lines) * 32;
       asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
     }
   }
 
-  // ---- exact scores of the survivors (two rows in flight), then selection by (score desc, index asc) ----
-  for (int c = 0; c < m; c += 2) {
+  // ---- exact scores of the survivors (two rows in flight per warp), then selection by (score desc, index asc) ----
+  for (int c = 2 * warp; c < m; c += 2 * kWarps) {
     double v0, v1 = 0.0;
-    if (c + 1 < m) exact_dot_warp_qd2(qs, g + static_cast<size_t>(kc[c]) * d, g + static_cast<size_t>(kc[c + 1]) * d, d, lane, v0, v1);
-    else v0 = exact_dot_warp_qd(qs, g + static_cast<size_t>(kc[c]) * d, d, lane);
+    if (c + 1 < m) exact_dot_warp_qd2(qs, p.g + static_cast<size_t>(kc[c]) * d, p.g + static_cast<size_t>(kc[c + 1]) * d, d, lane, v0, v1);
+    else v0 = exact_dot_warp_qd(qs, p.g + static_cast<size_t>(kc[c]) * d, d, lane);
     if (lane == 0) {
       sc[c] = v0;
       if (c + 1 < m) sc[c + 1] = v1;
     }
   }
-  __syncwarp();
+  group_sync<kThreads>();
   const int km = min(k, m);
   double kth = -INFINITY;
-  for (int c = lane; c < m; c += 32) {
+  for (int c = tid; c < m; c += kThreads) {
     const double v = sc[c];
     const int iv = kc[c];
     int rank = 0;
     for (int j = 0; j < m; ++j) {
       const double o = sc[j];
       const int io = kc[j];
-      rank += (o > v) || (o == v && (io < iv || (io == iv && j < c)));
+      rank += (o > v) || (o == v && (io < iv || (io == iv && j < c)));   // candidate rows are distinct; j < c only for safety
     }
     if (rank < km) {
-      out_scores[static_cast<size_t>(qrow) * k + rank] = static_cast<float>(v);
-      out_idx[static_cast<size_t>(qrow) * k + rank] = g_index_base + g_index_stride * iv;
+      p.out_scores[static_cast<size_t>(qrow) * k + rank] = static_cast<float>(v);
+      p.out_idx[static_cast<size_t>(qrow) * k + rank] = p.g_index_base + p.g_index_stride * iv;
       if (rank == km - 1) kth = v;
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) kth = fmax(kth, __shfl_xor_sync(kFull, kth, o));   // one lane holds it (NaN -> -inf: flagged)
-  if (lane == 0) {
-    // certificate: every gallery row that is not a candidate has approximate centred score <= thr, hence exact score
-    // q.g <= thr + eps + q.mu
-    const bool closed = thr > -INFINITY;
-    // fp64 rounding of kth and q.mu themselves: see the block form
-    const double slack = 4.6e-16 * (d + 8) * static_cast<double>(qx + nun) * static_cast<double>(g_norm + mun);
-    const bool ok = (n >= k) && (m >= k) && !overflow &&
-                    (!closed || kth > static_cast<double>(thr) + static_cast<double>(eps) + qmu + slack);
+  kth = group_max<kThreads>(kth);   // one thread holds it (NaN -> -inf: flagged)
+  if (tid == 0) {
+    const bool ok = (n >= k) && (m >= k) && (!closed || kth > bound);
     if (!ok) {
-      const int pos = atomicAdd(n_flagged, 1);
-      flagged[pos] = qrow;
-      if (thr_next) {
+      const int pos = atomicAdd(p.n_flagged, 1);
+      p.flagged[pos] = qrow;
+      if (p.thr_next) {
+        // every row of the true top-k has exact score >= kth, hence centred approximate score >= kth - q.mu - eps
         float t = -INFINITY;
         if (m >= k && kth > -INFINITY) {
           const double lo = kth - qmu - static_cast<double>(eps);
           t = static_cast<float>(lo) - 2e-6f * fabsf(static_cast<float>(lo)) - 1e-7f;
         }
-        thr_next[pos] = t;
+        p.thr_next[pos] = t;
       }
     }
   }
@@ -1760,29 +1665,25 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
   DCR_CUDA_CHECK(cudaEventRecord(ev1, stream));
 
   auto rescore = [&](const PassPlan& pp, const int* qmap, int* flagged, int* n_flagged, float* thr_next) -> int {
+    RescoreParams rp;
+    rp.q = q, rp.g = g, rp.nq = pp.nq, rp.d = d, rp.d_pad = pl.d_pad, rp.k = k;
+    rp.n_qtiles = pp.n_qtiles, rp.n_gtiles = pl.n_gtiles, rp.gchunk = pp.gchunk, rp.n_chunks = pp.n_chunks;
+    rp.n_units = pp.n_units, rp.n_sets = pp.n_sets, rp.max_cand = pp.max_cand;
+    rp.cand = pb.cand, rp.cand_cnt = pb.ccnt, rp.cand_thr = pb.cthr, rp.qmap = qmap;
+    rp.mu = centre ? mu : nullptr, rp.nu = centre ? nu : nullptr, rp.nu_flag = qflag;
+    rp.q_norm_hat = qnh, rp.q_norm_res = qnr, rp.q_norm_x = qnx, rp.g_max = gmax;
+    rp.g_index_base = g_index_base, rp.g_index_stride = g_index_stride, rp.out_scores = out_scores, rp.out_idx = out_idx;
+    rp.flagged = flagged, rp.n_flagged = n_flagged, rp.thr_next = thr_next;
     // one warp per query when a q-tile's candidate slots fit a lane each and four queries' rows fit a block's shared memory
-    const size_t per_warp = ((static_cast<size_t>(d) + 1) & ~size_t(1)) * 8 + ((static_cast<size_t>(pp.max_cand) + 3) & ~size_t(3)) * 20;
-    const bool warp_form = pp.kp > 0 && pp.max_cand / pp.kp <= 32 && pp.n_chunks <= 32 && kRescoreWarps * per_warp <= 56 * 1024 &&
+    // (the block-wide form spends its time on barriers for such small candidate sets)
+    const size_t per_query = RescoreSmem(d, pp.max_cand).bytes;
+    const bool warp_form = pp.kp > 0 && pp.max_cand / pp.kp <= 32 && pp.n_chunks <= 32 && 4 * per_query <= 56 * 1024 &&
                            !tuning_flag("DCR_SIM_RESCORE_BLOCK");
-    if (warp_form) {
-      const size_t smem = kRescoreWarps * per_warp;
-      DCR_CUDA_CHECK(cudaFuncSetAttribute(rescore_select_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-      rescore_select_warp_kernel<<<(pp.nq + kRescoreWarps - 1) / kRescoreWarps, 32 * kRescoreWarps, smem, stream>>>(
-          q, g, pp.nq, d, k, pp.n_qtiles, pl.n_gtiles, pp.gchunk, pp.n_chunks, pp.n_units, pl.rows_per_qtile, pp.n_sets, pl.d_pad,
-          pb.cand, pb.ccnt, pb.cthr, qmap, centre ? mu : nullptr, centre ? nu : nullptr, qflag, qnh, qnr, qnx, gmax, g_index_base,
-          g_index_stride, out_scores, out_idx, flagged, n_flagged, thr_next, pp.max_cand);
-      count_launch();
-      DCR_CUDA_CHECK(cudaGetLastError());
-      return 0;
-    }
-    const size_t rs_smem = ((static_cast<size_t>(d) + 1) & ~size_t(1)) * 8 + static_cast<size_t>(pp.max_cand) * 20 + 16;
-    DCR_CUDA_CHECK(cudaFuncSetAttribute(rescore_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(rs_smem)));
-    rescore_select_kernel<<<pp.nq, 128, rs_smem, stream>>>(
-        q, g, nq, ng, d, k, pp.n_qtiles, pl.n_gtiles, pp.gchunk, pp.n_chunks, pp.n_units, pl.rows_per_qtile, pp.n_sets, pl.d_pad,
-        pb.cand, pb.ccnt,
-        pb.cthr, qmap, centre ? mu : nullptr, centre ? nu : nullptr, qflag, qnh, qnr, qnx, gmax, g_index_base, g_index_stride, out_scores, out_idx,
-        flagged, n_flagged, thr_next, pp.max_cand);
+    const int per_block = warp_form ? kRescoreThreads / 32 : 1;
+    const size_t smem = per_block * per_query;
+    auto kern = warp_form ? rescore_select_kernel<32> : rescore_select_kernel<kRescoreThreads>;
+    DCR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    kern<<<(pp.nq + per_block - 1) / per_block, kRescoreThreads, smem, stream>>>(rp);
     count_launch();
     DCR_CUDA_CHECK(cudaGetLastError());
     return 0;
