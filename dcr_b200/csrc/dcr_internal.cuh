@@ -83,15 +83,19 @@ bool expand_only_eligible(const ConvGemmDesc& a, size_t max_smem);
 int expand_only(const ConvGemmDesc& a, cudaStream_t stream);
 
 
+// ---- input kernels (image_in.cu): the transformed image batch -> the first layer's operand --------------------------
+struct ImageSource;   // image_in.cuh
+// im2col rows [B * OH * OW, k_pad] of a kh x kw first convolution / patch embedding over the RH x RW network input
+int im2col_u8(const ImageSource& src, int B, int kh, int kw, int stride, int pad, int k_pad, __nv_bfloat16* out,
+              long long out_plane_stride, int planes, cudaStream_t stream);
+// 2x2 space-to-depth tensor [B, (RH+6)/2, (RW+6)/2, 16] of the 7x7/2/pad-3 ResNet stem
+int stem_s2d_u8(const ImageSource& src, int B, __nv_bfloat16* out, long long out_plane_stride, int planes,
+                cudaStream_t stream);
+// the column-parity planes stem_conv reads (one plane per tensor: fast mode)
+int stem_rows(const ImageSource& src, int B, __nv_bfloat16* out, cudaStream_t stream);
+
+
 // ---- HBM-bound kernels (pool_norm.cu, attention.cu) ---------------------------------------------------------------
-int im2col_u8(const uint8_t* img, int B, int IH, int IW, int crop_y, int crop_x, int H, int W, int kh, int kw,
-              int stride, int pad, int k_pad, const float* mean3, const float* std3, float post_scale,
-              float post_shift, __nv_bfloat16* out, long long out_plane_stride, int planes, cudaStream_t stream,
-              const float* img_f32 = nullptr,    // img_f32: fp32 NCHW [B,3,IH,IW] already transformed (img unused)
-              int RH = 0, int RW = 0, float rscale = 0.f);   // optional bilinear resize of the crop (multi_scale)
-int stem_s2d_u8(const uint8_t* img, int B, int IH, int IW, int crop_y, int crop_x, int H, int W, const float* mean3,
-                const float* std3, float post_scale, float post_shift, __nv_bfloat16* out, long long out_plane_stride,
-                int planes, cudaStream_t stream, int RH = 0, int RW = 0, float rscale = 0.f, const float* img_f32 = nullptr);
 int pool2d(bool is_max, const __nv_bfloat16* in, long long in_plane_stride, __nv_bfloat16* out,
            long long out_plane_stride, int planes, int B, int H, int W, int C, int k, int stride, int pad, int ld_out,
            int out_col_off, cudaStream_t stream);
@@ -112,9 +116,6 @@ int embed_tokens(const int* ids, int B, int T, int C, const float* table, int vo
 // ---- fused ResNet stem (stem_fused.cu): overlapping-window (Toeplitz) A operand, fast mode ------------------------------
 int stem_fused_pitch(int out_w);                              // units (16-byte pixels) per stored pair-row
 long long stem_fused_plane_units(int out_h, int out_w);       // units per column-parity plane and image (incl. slack)
-int stem_rows(const uint8_t* img, const float* img_f32, int B, int IH, int IW, int crop_y, int crop_x, int H, int W, int RH, int RW,
-              float rscale, const float* mean3, const float* std3, float post_scale, float post_shift, __nv_bfloat16* out,
-              cudaStream_t stream);
 int stem_conv(const __nv_bfloat16* planes, int B, int OH, int OW, const __nv_bfloat16* weight, const float* scale, const float* bias,
               __nv_bfloat16* out, cudaStream_t stream, int pool = 0);   // pool: fuse the 3x3/2/pad-1 max pool, out = [OHp*OWp, 64]
 

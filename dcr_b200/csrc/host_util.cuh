@@ -48,6 +48,12 @@ bool tuning_flag(const char* name);   // true when tuning is enabled and the var
 // cached per current device; returns nullptr and sets the error on failure
 const DeviceInfo* device_info();
 
+// blocks for a grid-stride loop over work_items: one item per thread, at most 16 blocks per SM
+inline int grid_for(long long work_items, int block, int num_sms) {
+  const long long blocks = (work_items + block - 1) / block;
+  return static_cast<int>(blocks < 16ll * num_sms ? blocks : 16ll * num_sms);
+}
+
 // 2-D row-major bf16 tensor [rows, cols] (cols contiguous), box = [box_rows, box_cols], 128-byte swizzle.
 // box_cols * 2 bytes must be 128.
 int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride_elems,

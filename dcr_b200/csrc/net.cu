@@ -12,6 +12,7 @@
 
 #include "dcr_internal.cuh"
 #include "host_util.cuh"
+#include "image_in.cuh"
 
 namespace dcr {
 
@@ -54,6 +55,35 @@ struct Net {
 namespace {
 const int kTermA[6] = {0, 0, 1, 1, 0, 2};
 const int kTermW[6] = {0, 1, 0, 1, 2, 0};
+
+// The input prefix of IM2COL_U8, STEM_S2D and STEM_ROWS: ints [out_t, IH, IW, crop_y, crop_x, H, W], floats [mean[3],
+// std[3], post_scale, post_shift]; the resizing form adds RH, RW at ints [rs, rs + 1] and rscale at floats [8] (unset
+// arguments are zero: no resizing).
+int input_source(const NetOp& op, int rs, const uint8_t* images, const float* images_f32, ImageSource* s) {
+  const int* a = op.i;
+  const bool f32 = images_f32 != nullptr;
+  s->img = images;
+  s->img_f32 = images_f32;
+  // fp32 input: the tensor is the transformed crop itself ([B,3,H,W]: no crop offset)
+  s->IH = f32 ? a[5] : a[1];
+  s->IW = f32 ? a[6] : a[2];
+  s->crop_y = f32 ? 0 : a[3];
+  s->crop_x = f32 ? 0 : a[4];
+  s->H = a[5];
+  s->W = a[6];
+  s->rscale = op.f[8];
+  s->RH = s->rscale == 0.f ? s->H : a[rs];
+  s->RW = s->rscale == 0.f ? s->W : a[rs + 1];
+  for (int c = 0; c < 3; ++c) {
+    s->mean[c] = op.f[c];
+    s->std[c] = op.f[3 + c];
+  }
+  s->post_scale = op.f[6];
+  s->post_shift = op.f[7];
+  DCR_REQUIRE(s->crop_y >= 0 && s->crop_x >= 0 && s->crop_y + s->H <= s->IH && s->crop_x + s->W <= s->IW,
+              "net_forward: %d x %d crop at (%d, %d) outside the %d x %d image", s->H, s->W, s->crop_y, s->crop_x, s->IH, s->IW);
+  return 0;
+}
 }
 
 int net_create(int max_batch, int planes, Net** out) {
@@ -281,24 +311,22 @@ int net_forward(Net* n, const uint8_t* images, int B, float* out, cudaStream_t s
     switch (op.kind) {
       case NET_OP_IM2COL_U8: {
         NetTensor& t = n->tensors[a[0]];
-        // fp32 input: the tensor is the transformed crop itself ([B,3,H,W]: no crop offset, no mean/std)
-        rc = im2col_u8(images, B, f32 ? a[5] : a[1], f32 ? a[6] : a[2], f32 ? 0 : a[3], f32 ? 0 : a[4], a[5], a[6], a[7], a[8],
-                       a[9], a[10], a[11], &op.f[0], &op.f[3], op.f[6], op.f[7], t.ptr, t.plane_stride, P, stream, images_f32,
-                       a[12], a[13], op.f[8]);   // optional 14-int / 9-float form: resized size + float(1 / scale_factor)
+        ImageSource src;
+        rc = input_source(op, 12, images, images_f32, &src);
+        if (rc == 0) rc = im2col_u8(src, B, a[7], a[8], a[9], a[10], a[11], t.ptr, t.plane_stride, P, stream);
         break;
       }
       case NET_OP_STEM_S2D: {
         NetTensor& t = n->tensors[a[0]];
-        // optional 9-int / 9-float form: a[7], a[8] = size after bilinear resizing of the crop, f[8] = float(1 / scale_factor)
-        rc = stem_s2d_u8(images, B, f32 ? a[5] : a[1], f32 ? a[6] : a[2], f32 ? 0 : a[3], f32 ? 0 : a[4], a[5], a[6], &op.f[0],
-                         &op.f[3], op.f[6], op.f[7], t.ptr, t.plane_stride, P, stream, a[7], a[8], op.f[8],
-                         images_f32);   // unset arguments are zero = no resizing
+        ImageSource src;
+        rc = input_source(op, 7, images, images_f32, &src);
+        if (rc == 0) rc = stem_s2d_u8(src, B, t.ptr, t.plane_stride, P, stream);
         break;
       }
       case NET_OP_STEM_ROWS: {
-        NetTensor& t = n->tensors[a[0]];
-        rc = stem_rows(images, images_f32, B, f32 ? a[5] : a[1], f32 ? a[6] : a[2], f32 ? 0 : a[3], f32 ? 0 : a[4], a[5], a[6], a[7],
-                       a[8], op.f[8], &op.f[0], &op.f[3], op.f[6], op.f[7], t.ptr, stream);
+        ImageSource src;
+        rc = input_source(op, 7, images, images_f32, &src);
+        if (rc == 0) rc = stem_rows(src, B, n->tensors[a[0]].ptr, stream);
         break;
       }
       case NET_OP_STEM_CONV: {

@@ -4,9 +4,6 @@
 // is a 16-byte vector.
 //
 // Reference ops replaced:
-//   diff_retrieval.py:325-330  Resize(256)/CenterCrop(224)/ToTensor/Normalize            -> im2col_u8_kernel
-//   embedding_search/utils.py:35-50 (ImageNet mean/std variant)                           -> im2col_u8_kernel
-//   metrics/fid.py:104-110 + metrics/inception.py:152-153 (normalise twice)               -> im2col_u8_kernel (post affine)
 //   torchvision resnet maxpool(3,2,1); inception max_pool2d(3,2)                          -> maxpool_kernel
 //   metrics/inception.py:241,269,302 avg_pool2d(3,1,1,count_include_pad=False)            -> avgpool3_kernel
 //   SSCD GeM pooling (p=3, eps=1e-6) [upstream, unverified]                               -> gem_kernel
@@ -19,213 +16,12 @@
 
 #include "dcr_internal.cuh"
 #include "host_util.cuh"
+#include "planes.cuh"
 
 namespace dcr {
 namespace {
 
 constexpr uint32_t kFull = 0xffffffffu;
-
-__device__ __forceinline__ void load8(const __nv_bfloat16* base, long long plane_stride, int planes, size_t idx,
-                                      float (&v)[8]) {
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = 0.f;
-  for (int p = 0; p < planes; ++p) {
-    const uint4 u = *reinterpret_cast<const uint4*>(base + p * plane_stride + idx);
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      v[2 * j] += __uint_as_float(w[j] << 16);
-      v[2 * j + 1] += __uint_as_float(w[j] & 0xffff0000u);
-    }
-  }
-}
-
-__device__ __forceinline__ void store8(__nv_bfloat16* base, long long plane_stride, int planes, size_t idx,
-                                       float (&v)[8]) {
-  for (int p = 0; p < planes; ++p) {
-    uint32_t w[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const __nv_bfloat16 a = __float2bfloat16_rn(v[2 * j]), b = __float2bfloat16_rn(v[2 * j + 1]);
-      w[j] = static_cast<uint32_t>(__bfloat16_as_ushort(a)) | (static_cast<uint32_t>(__bfloat16_as_ushort(b)) << 16);
-      v[2 * j] -= __bfloat162float(a);
-      v[2 * j + 1] -= __bfloat162float(b);
-    }
-    *reinterpret_cast<uint4*>(base + p * plane_stride + idx) = make_uint4(w[0], w[1], w[2], w[3]);
-  }
-}
-
-// ---- uint8 HWC image -> normalised im2col matrix for the (3-channel) first convolution ------------------------
-// out[m, k], m = (b, p, q) over the OHxOW output grid, k = (r*kw + s)*3 + c  (zero for k >= kh*kw*3 and for taps
-// that fall into the zero padding).  value = post_scale * ((u8/255 - mean[c]) / std[c]) + post_shift.
-struct Im2colU8Params {
-  const uint8_t* img;
-  const float* img_f32;   // kF32 kernels: fp32 NCHW [B,3,IH,IW], already transformed (ToTensor/Normalize done by the caller)
-  int B, IH, IW, crop_y, crop_x, H, W;   // H, W: size after the centre crop
-  int RH, RW;                            // network input size: == H, W, or the bilinearly resized crop (rscale != 0)
-  float rscale;                          // float(1 / scale_factor) of utils_ret.py:676-698 `multi_scale`, 0 = no resizing
-  int kh, kw, stride, pad, OH, OW, k_pad;
-  float mean[3], std[3], post_scale, post_shift;
-  __nv_bfloat16* out;
-  long long out_plane_stride;
-  int planes;
-};
-
-// K layout: k = r * RP + s * 3 + c with RP = ceil8(3 * KW) (each filter row padded to a multiple of 8 elements so
-// that a thread owns whole 16-byte groups and every (s, c) index is a compile-time constant).  One thread per
-// (output pixel, filter row): 3*KW contiguous image bytes -> RP normalised bf16 values.
-// kF32: the input is the tensor the reference hands to `model(samples)` (utils_ret.py:751): fp32 NCHW, already
-// normalised; only the optional post affine (FID's second 2x-1, inception.py:152-153) is applied.
-template <int KW, bool kF32, bool kResize>
-__global__ void __launch_bounds__(256) im2col_u8_kernel(const Im2colU8Params p) {
-  constexpr int RP = (3 * KW + 7) / 8 * 8;
-  // per-channel lookup table u8 -> normalised value, computed once per block with the reference's exact arithmetic
-  // (ToTensor: u8/255, Normalize: (x-mean)/std, both fp32 with IEEE division), then the optional post affine
-  __shared__ float lut[3][256];
-  for (int i = threadIdx.x; i < 768; i += blockDim.x) {
-    const int c = i >> 8, u = i & 255;
-    const float val = (static_cast<float>(u) / 255.f - p.mean[c]) / p.std[c];
-    lut[c][u] = p.post_scale * val + p.post_shift;
-  }
-  __syncthreads();
-  const int rows_k = (p.k_pad + RP - 1) / RP;   // kh filter rows + zero rows up to k_pad (the last one may be partial)
-  const long long total = static_cast<long long>(p.B) * p.OH * p.OW * rows_k;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int r = static_cast<int>(i % rows_k);
-    const long long m = i / rows_k;
-    const int q = static_cast<int>(m % p.OW);
-    const int pp = static_cast<int>((m / p.OW) % p.OH);
-    const int b = static_cast<int>(m / (static_cast<long long>(p.OW) * p.OH));
-    const int y = pp * p.stride - p.pad + r;           // in crop coordinates
-    const int x0 = q * p.stride - p.pad;
-    const bool row_ok = r < p.kh && y >= 0 && y < p.RH;
-    const size_t plane = static_cast<size_t>(p.IH) * p.IW;
-    const uint8_t* img = p.img + static_cast<size_t>(b) * p.IH * p.IW * 3;
-    const float* imgf = p.img_f32 + static_cast<size_t>(b) * 3 * plane;
-    // transformed value of channel c at crop coordinates (yy, xx)
-    auto px = [&](int yy, int xx, int c) -> float {
-      if constexpr (kF32) return fmaf(p.post_scale, imgf[c * plane + static_cast<size_t>(yy + p.crop_y) * p.IW + (xx + p.crop_x)], p.post_shift);
-      else return lut[c][img[(static_cast<size_t>(yy + p.crop_y) * p.IW + (xx + p.crop_x)) * 3 + c]];
-    };
-    // bilinear source rows of the resized image (torch F.interpolate, align_corners=False, scale_factor given)
-    int y0 = 0, y1 = 0;
-    float ly = 0.f, hy = 1.f;
-    if constexpr (kResize) {
-      const float sy = fmaxf(p.rscale * (static_cast<float>(y) + 0.5f) - 0.5f, 0.f);
-      y0 = min(static_cast<int>(sy), p.H - 1);
-      y1 = y0 + (y0 < p.H - 1 ? 1 : 0);
-      ly = sy - static_cast<float>(y0);
-      hy = 1.f - ly;
-    }
-    __nv_bfloat16* dst = p.out + static_cast<size_t>(m) * p.k_pad + r * RP;
-#pragma unroll
-    for (int g = 0; g < RP / 8; ++g) {
-      if (r * RP + g * 8 >= p.k_pad) break;   // partial last zero row (k_pad is a multiple of 8, not always of RP)
-      float v[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const int j = g * 8 + e;          // compile-time after unrolling
-        const int s = j / 3, c = j % 3;
-        float val = 0.f;
-        if (j < 3 * KW && row_ok && x0 + s >= 0 && x0 + s < p.RW) {
-          if constexpr (kResize) {
-            const float sx = fmaxf(p.rscale * (static_cast<float>(x0 + s) + 0.5f) - 0.5f, 0.f);
-            const int xa = min(static_cast<int>(sx), p.W - 1);
-            const int xb = xa + (xa < p.W - 1 ? 1 : 0);
-            const float lx = sx - static_cast<float>(xa), hx = 1.f - lx;
-            val = hy * (hx * px(y0, xa, c) + lx * px(y0, xb, c)) + ly * (hx * px(y1, xa, c) + lx * px(y1, xb, c));
-          } else {
-            val = px(y, x0 + s, c);
-          }
-        }
-        v[e] = val;
-      }
-      store8(dst, p.out_plane_stride, p.planes, g * 8, v);
-    }
-  }
-}
-
-// ---- space-to-depth stem input (7x7 / stride 2 / pad 3 first convolution of the ResNet trunk) ----------------------
-// Z[b, u, v, (i*2+j)*3 + c] = xn[2u + i - 3, 2v + j - 3, c]  (zero outside the image), channels 12..15 = 0, with
-// xn the normalised crop.  A 7x7/2 convolution of xn equals a 4x4/1 convolution of Z (weights regrouped on the host),
-// which the GEMM kernel reads through an overlapping-window tensor map -- no im2col matrix in HBM.
-// Optional bilinear down-scaling of the normalised crop first (utils_ret.py:676-698 `multi_scale`:
-// F.interpolate(x, scale_factor=s, mode='bilinear', align_corners=False)): xn is then the [RH, RW] resized image,
-// sampled with torch's arithmetic (source index = rscale * (dst + 0.5) - 0.5 clamped at 0, rscale = float(1 / s)).
-struct StemS2dParams {
-  const uint8_t* img;
-  const float* img_f32;   // kF32 kernels: fp32 NCHW [B,3,IH,IW], already transformed
-  int B, IH, IW, crop_y, crop_x, H, W, U, V;
-  int RH, RW;        // size of xn (== H, W without resizing)
-  float rscale;      // 0 = no resizing
-  float mean[3], std[3], post_scale, post_shift;
-  __nv_bfloat16* out;
-  long long out_plane_stride;
-  int planes;
-};
-
-template <bool kResize, bool kF32>
-__global__ void __launch_bounds__(256) stem_s2d_u8_kernel(const StemS2dParams p) {
-  __shared__ float lut[3][256];
-  for (int i = threadIdx.x; i < 768; i += blockDim.x) {
-    const int c = i >> 8, u = i & 255;
-    const float val = (static_cast<float>(u) / 255.f - p.mean[c]) / p.std[c];   // ToTensor + Normalize, IEEE fp32
-    lut[c][u] = p.post_scale * val + p.post_shift;
-  }
-  __syncthreads();
-  const long long total = static_cast<long long>(p.B) * p.U * p.V;
-  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
-       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int v = static_cast<int>(idx % p.V);
-    const int u = static_cast<int>((idx / p.V) % p.U);
-    const int b = static_cast<int>(idx / (static_cast<long long>(p.V) * p.U));
-    const uint8_t* img = p.img + static_cast<size_t>(b) * p.IH * p.IW * 3;
-    const size_t plane = static_cast<size_t>(p.IH) * p.IW;
-    const float* imgf = p.img_f32 + static_cast<size_t>(b) * 3 * plane;
-    // normalised value of channel c at crop coordinates (yy, xx)
-    auto px = [&](int yy, int xx, int c) -> float {
-      if constexpr (kF32) return fmaf(p.post_scale, imgf[c * plane + static_cast<size_t>(yy + p.crop_y) * p.IW + (xx + p.crop_x)], p.post_shift);
-      else return lut[c][img[(static_cast<size_t>(yy + p.crop_y) * p.IW + (xx + p.crop_x)) * 3 + c]];
-    };
-    float z[16];
-#pragma unroll
-    for (int e = 0; e < 16; ++e) z[e] = 0.f;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int y = 2 * u + i - 3;
-      if (y < 0 || y >= p.RH) continue;
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int x = 2 * v + j - 3;
-        if (x < 0 || x >= p.RW) continue;
-        if constexpr (!kResize) {
-#pragma unroll
-          for (int c = 0; c < 3; ++c) z[(i * 2 + j) * 3 + c] = px(y, x, c);
-        } else {
-          const float sy = fmaxf(p.rscale * (static_cast<float>(y) + 0.5f) - 0.5f, 0.f);
-          const float sx = fmaxf(p.rscale * (static_cast<float>(x) + 0.5f) - 0.5f, 0.f);
-          const int y0 = static_cast<int>(sy), x0 = static_cast<int>(sx);
-          const int y1 = y0 + (y0 < p.H - 1 ? 1 : 0), x1 = x0 + (x0 < p.W - 1 ? 1 : 0);
-          const float ly = sy - static_cast<float>(y0), lx = sx - static_cast<float>(x0);
-          const float hy = 1.f - ly, hx = 1.f - lx;
-#pragma unroll
-          for (int c = 0; c < 3; ++c)
-            z[(i * 2 + j) * 3 + c] = hy * (hx * px(y0, x0, c) + lx * px(y0, x1, c)) +
-                                     ly * (hx * px(y1, x0, c) + lx * px(y1, x1, c));
-        }
-      }
-    }
-    float lo[8], hi[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      lo[e] = z[e];
-      hi[e] = z[8 + e];
-    }
-    store8(p.out, p.out_plane_stride, p.planes, static_cast<size_t>(idx) * 16, lo);
-    store8(p.out, p.out_plane_stride, p.planes, static_cast<size_t>(idx) * 16 + 8, hi);
-  }
-}
 
 // ---- pooling -------------------------------------------------------------------------------------------------
 struct PoolParams {
@@ -654,58 +450,7 @@ __global__ void embed_tokens_kernel(const EmbedParams p) {
   }
 }
 
-int grid_for(long long work_items, int block, int num_sms) {
-  long long blocks = (work_items + block - 1) / block;
-  return static_cast<int>(std::min<long long>(blocks, static_cast<long long>(num_sms) * 16));
-}
-
 }  // namespace
-
-int im2col_u8(const uint8_t* img, int B, int IH, int IW, int crop_y, int crop_x, int H, int W, int kh, int kw,
-              int stride, int pad, int k_pad, const float* mean3, const float* std3, float post_scale,
-              float post_shift, __nv_bfloat16* out, long long out_plane_stride, int planes, cudaStream_t stream,
-              const float* img_f32, int RH, int RW, float rscale) {
-  const DeviceInfo* di = device_info();
-  if (!di) return -2;
-  const int rp = (3 * kw + 7) / 8 * 8;
-  DCR_REQUIRE(k_pad % 8 == 0 && k_pad >= kh * rp, "im2col_u8: k_pad %d must be a multiple of 8 and >= %d", k_pad, kh * rp);
-  DCR_REQUIRE(kw == 3 || kw == 7 || kw == 8 || kw == 14 || kw == 16, "im2col_u8: filter width %d not instantiated (3, 7, 8, 14, 16)", kw);
-  DCR_REQUIRE(crop_y >= 0 && crop_x >= 0 && crop_y + H <= IH && crop_x + W <= IW, "im2col_u8: crop outside image");
-  Im2colU8Params p;
-  p.img = img; p.img_f32 = img_f32; p.B = B; p.IH = IH; p.IW = IW; p.crop_y = crop_y; p.crop_x = crop_x; p.H = H; p.W = W;
-  p.kh = kh; p.kw = kw; p.stride = stride; p.pad = pad;
-  if (rscale == 0.f) { RH = H; RW = W; }
-  DCR_REQUIRE(RH >= kh && RW >= kw, "im2col_u8: network input %d x %d smaller than the filter", RH, RW);
-  p.RH = RH; p.RW = RW; p.rscale = rscale;
-  p.OH = (RH + 2 * pad - kh) / stride + 1;
-  p.OW = (RW + 2 * pad - kw) / stride + 1;
-  p.k_pad = k_pad;
-  for (int c = 0; c < 3; ++c) { p.mean[c] = mean3[c]; p.std[c] = std3[c]; }
-  p.post_scale = post_scale; p.post_shift = post_shift;
-  p.out = out; p.out_plane_stride = out_plane_stride; p.planes = planes;
-  if (B == 0) return 0;
-  const long long total = static_cast<long long>(B) * p.OH * p.OW * ((k_pad + rp - 1) / rp);
-  const int grid = grid_for(total, 256, di->num_sms);
-#define DCR_IM2COL(KWv)                                                                             \
-  do {                                                                                              \
-    if (img_f32) {                                                                                  \
-      if (rscale == 0.f) im2col_u8_kernel<KWv, true, false><<<grid, 256, 0, stream>>>(p);           \
-      else im2col_u8_kernel<KWv, true, true><<<grid, 256, 0, stream>>>(p);                          \
-    } else {                                                                                        \
-      if (rscale == 0.f) im2col_u8_kernel<KWv, false, false><<<grid, 256, 0, stream>>>(p);          \
-      else im2col_u8_kernel<KWv, false, true><<<grid, 256, 0, stream>>>(p);                         \
-    }                                                                                               \
-  } while (0)
-  if (kw == 7) DCR_IM2COL(7);
-  else if (kw == 3) DCR_IM2COL(3);
-  else if (kw == 8) DCR_IM2COL(8);
-  else if (kw == 14) DCR_IM2COL(14);
-  else DCR_IM2COL(16);
-#undef DCR_IM2COL
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
 
 int embed_tokens(const int* ids, int B, int T, int C, const float* table, int vocab, const float* pos, __nv_bfloat16* out,
                  long long out_plane_stride, int planes, cudaStream_t stream) {
@@ -717,36 +462,6 @@ int embed_tokens(const int* ids, int B, int T, int C, const float* table, int vo
   p.ids = ids; p.table = table; p.pos = pos; p.out = out; p.out_plane_stride = out_plane_stride;
   p.planes = planes; p.B = B; p.T = T; p.C = C; p.vocab = vocab;
   embed_tokens_kernel<<<grid_for(static_cast<long long>(B) * T * (C / 8), 256, di->num_sms), 256, 0, stream>>>(p);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
-
-int stem_s2d_u8(const uint8_t* img, int B, int IH, int IW, int crop_y, int crop_x, int H, int W, const float* mean3,
-                const float* std3, float post_scale, float post_shift, __nv_bfloat16* out, long long out_plane_stride,
-                int planes, cudaStream_t stream, int RH, int RW, float rscale, const float* img_f32) {
-  const DeviceInfo* di = device_info();
-  if (!di) return -2;
-  DCR_REQUIRE(crop_y >= 0 && crop_x >= 0 && crop_y + H <= IH && crop_x + W <= IW, "stem_s2d_u8: crop outside image");
-  if (rscale == 0.f) { RH = H; RW = W; }
-  DCR_REQUIRE(RH >= 2 && RW >= 2 && RH % 2 == 0 && RW % 2 == 0, "stem_s2d_u8: network input size must be even (%d x %d)", RH, RW);
-  StemS2dParams p;
-  p.img = img; p.img_f32 = img_f32; p.B = B; p.IH = IH; p.IW = IW; p.crop_y = crop_y; p.crop_x = crop_x; p.H = H; p.W = W;
-  p.RH = RH; p.RW = RW; p.rscale = rscale;
-  p.U = (RH + 6) / 2; p.V = (RW + 6) / 2;
-  for (int c = 0; c < 3; ++c) { p.mean[c] = mean3[c]; p.std[c] = std3[c]; }
-  p.post_scale = post_scale; p.post_shift = post_shift;
-  p.out = out; p.out_plane_stride = out_plane_stride; p.planes = planes;
-  if (B == 0) return 0;
-  const long long total = static_cast<long long>(B) * p.U * p.V;
-  const int grid = grid_for(total, 256, di->num_sms);
-  if (img_f32) {
-    if (rscale == 0.f) stem_s2d_u8_kernel<false, true><<<grid, 256, 0, stream>>>(p);
-    else stem_s2d_u8_kernel<true, true><<<grid, 256, 0, stream>>>(p);
-  } else {
-    if (rscale == 0.f) stem_s2d_u8_kernel<false, false><<<grid, 256, 0, stream>>>(p);
-    else stem_s2d_u8_kernel<true, false><<<grid, 256, 0, stream>>>(p);
-  }
   count_launch();
   DCR_CUDA_CHECK(cudaGetLastError());
   return 0;

@@ -5,7 +5,7 @@
 //
 // Reference call site: `model(samples)` (utils_ret.py:751) -> torchvision ResNet conv1 / bn1 / relu of the SSCD trunk.
 //
-// Input layout (stem_rows_u8_kernel, fused with Resize/CenterCrop/ToTensor/Normalize of diff_retrieval.py:325-330):
+// Input layout (stem_rows_kernel in image_in.cu, fused with Resize/CenterCrop/ToTensor/Normalize of diff_retrieval.py:325-330):
 // with ip the zero-padded (3 pixels) normalised crop, the image is stored as two "column-parity planes" of 16-byte units
 //     plane_e[P * PW + u] = { ip[2P + i][2u + e][c] : i in {0,1}, c in {0,1,2} } + 2 zero channels      (8 bf16)
 // so that   out[y][x] = sum_{a<4, e<2, b<4, ch<8} W[a][e][b][ch] * plane_e[(y + a) * PW + (x + b)][ch]
@@ -300,119 +300,14 @@ __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_co
 
 }
 
-// ---- input kernel: uint8 HWC (or fp32 NCHW) image -> the two column-parity planes ----------------------------------------
-struct StemRowsParams {
-  const uint8_t* img;
-  const float* img_f32;
-  int B, IH, IW, crop_y, crop_x, H, W, RH, RW;
-  float rscale;
-  float mean[3], std[3], post_scale, post_shift;
-  __nv_bfloat16* out;
-  long long img_stride, plane_stride;
-  int PW, rows;     // units per pair-row, pair-rows written (OH + 3)
-};
-
-template <bool kResize, bool kF32>
-__global__ void __launch_bounds__(256) stem_rows_kernel(const StemRowsParams p) {
-  __shared__ float lut[3][256];
-  for (int i = threadIdx.x; i < 768; i += blockDim.x) {
-    const int c = i >> 8, u = i & 255;
-    const float val = (static_cast<float>(u) / 255.f - p.mean[c]) / p.std[c];   // ToTensor + Normalize, IEEE fp32
-    lut[c][u] = p.post_scale * val + p.post_shift;
-  }
-  __syncthreads();
-  const long long per_img = 2ll * p.rows * p.PW;
-  const long long total = per_img * p.B;
-  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
-       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int b = static_cast<int>(idx / per_img);
-    long long rem = idx - b * per_img;
-    const int e = static_cast<int>(rem / (static_cast<long long>(p.rows) * p.PW));
-    rem -= static_cast<long long>(e) * p.rows * p.PW;
-    const int P = static_cast<int>(rem / p.PW), u = static_cast<int>(rem % p.PW);
-    const uint8_t* img = p.img + static_cast<size_t>(b) * p.IH * p.IW * 3;
-    const size_t plane = static_cast<size_t>(p.IH) * p.IW;
-    const float* imgf = p.img_f32 + static_cast<size_t>(b) * 3 * plane;
-    auto px = [&](int yy, int xx, int c) -> float {
-      if constexpr (kF32) return fmaf(p.post_scale, imgf[c * plane + static_cast<size_t>(yy + p.crop_y) * p.IW + (xx + p.crop_x)], p.post_shift);
-      else return lut[c][img[(static_cast<size_t>(yy + p.crop_y) * p.IW + (xx + p.crop_x)) * 3 + c]];
-    };
-    float z[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) z[k] = 0.f;
-    const int x = 2 * u + e - 3;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int y = 2 * P + i - 3;
-      if (y < 0 || y >= p.RH || x < 0 || x >= p.RW) continue;
-      if constexpr (!kResize) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) z[i * 3 + c] = px(y, x, c);
-      } else {
-        const float sy = fmaxf(p.rscale * (static_cast<float>(y) + 0.5f) - 0.5f, 0.f);
-        const float sx = fmaxf(p.rscale * (static_cast<float>(x) + 0.5f) - 0.5f, 0.f);
-        const int y0 = static_cast<int>(sy), x0 = static_cast<int>(sx);
-        const int y1 = y0 + (y0 < p.H - 1 ? 1 : 0), x1 = x0 + (x0 < p.W - 1 ? 1 : 0);
-        const float ly = sy - static_cast<float>(y0), lx = sx - static_cast<float>(x0);
-        const float hy = 1.f - ly, hx = 1.f - lx;
-#pragma unroll
-        for (int c = 0; c < 3; ++c)
-          z[i * 3 + c] = hy * (hx * px(y0, x0, c) + lx * px(y0, x1, c)) + ly * (hx * px(y1, x0, c) + lx * px(y1, x1, c));
-      }
-    }
-    uint4 v;
-    v.x = pack2s(z[0], z[1]);
-    v.y = pack2s(z[2], z[3]);
-    v.z = pack2s(z[4], z[5]);
-    v.w = pack2s(z[6], z[7]);
-    __nv_bfloat16* dst = p.out + static_cast<size_t>(b) * p.img_stride + static_cast<size_t>(e) * p.plane_stride +
-                         (static_cast<size_t>(P) * p.PW + u) * 8;
-    *reinterpret_cast<uint4*>(dst) = v;
-  }
-}
-
 }  // namespace
 
-// geometry shared by the host graph builder (through dcr_stem_plane_units) and the two launchers
+// geometry shared by the host graph builder (through dcr_stem_plane_units), stem_rows (image_in.cu) and stem_conv
 int stem_fused_pitch(int out_w) { return out_w + 4; }
 long long stem_fused_plane_units(int out_h, int out_w) {
   const int PW = stem_fused_pitch(out_w);
   const long long tiles = (static_cast<long long>(out_h) * PW + kSTile - 1) / kSTile;
   return tiles * kSTile + 3ll * PW + 16 + 2 * kSTile;   // read slack: tiles of the pooled schedule may start past a tile boundary
-}
-
-int stem_rows(const uint8_t* img, const float* img_f32, int B, int IH, int IW, int crop_y, int crop_x, int H, int W, int RH, int RW,
-              float rscale, const float* mean3, const float* std3, float post_scale, float post_shift, __nv_bfloat16* out,
-              cudaStream_t stream) {
-  const DeviceInfo* di = device_info();
-  if (!di) return -2;
-  DCR_REQUIRE(crop_y >= 0 && crop_x >= 0 && crop_y + H <= IH && crop_x + W <= IW, "stem_rows: crop outside image");
-  if (rscale == 0.f) { RH = H; RW = W; }
-  DCR_REQUIRE(RH >= 2 && RW >= 2 && RH % 2 == 0 && RW % 2 == 0, "stem_rows: network input size must be even (%d x %d)", RH, RW);
-  if (B == 0) return 0;
-  StemRowsParams p;
-  p.img = img; p.img_f32 = img_f32; p.B = B; p.IH = IH; p.IW = IW; p.crop_y = crop_y; p.crop_x = crop_x; p.H = H; p.W = W;
-  p.RH = RH; p.RW = RW; p.rscale = rscale;
-  for (int c = 0; c < 3; ++c) { p.mean[c] = mean3[c]; p.std[c] = std3[c]; }
-  p.post_scale = post_scale; p.post_shift = post_shift;
-  const int OH = RH / 2, OW = RW / 2;
-  p.PW = stem_fused_pitch(OW);
-  p.rows = OH + 3;
-  p.plane_stride = stem_fused_plane_units(OH, OW) * 8;
-  p.img_stride = 2 * p.plane_stride;
-  p.out = out;
-  const long long total = 2ll * p.rows * p.PW * B;
-  const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, static_cast<long long>(di->num_sms) * 16));
-  if (img_f32) {
-    if (rscale == 0.f) stem_rows_kernel<false, true><<<grid, 256, 0, stream>>>(p);
-    else stem_rows_kernel<true, true><<<grid, 256, 0, stream>>>(p);
-  } else {
-    if (rscale == 0.f) stem_rows_kernel<false, false><<<grid, 256, 0, stream>>>(p);
-    else stem_rows_kernel<true, false><<<grid, 256, 0, stream>>>(p);
-  }
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
 }
 
 int stem_conv(const __nv_bfloat16* planes, int B, int OH, int OW, const __nv_bfloat16* weight, const float* scale, const float* bias,

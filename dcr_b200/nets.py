@@ -272,6 +272,29 @@ def _first_conv_weight(w: torch.Tensor, k_pad: int) -> torch.Tensor:
     return out
 
 
+def _scaled_size(size: int, scale_factor: Optional[float]) -> int:
+    """Output size of F.interpolate(scale_factor=s) (multi_scale, utils_ret.py:676-698); None or 1 = no resizing."""
+    if scale_factor is None or scale_factor == 1:
+        return size
+    import math
+    return int(math.floor(float(size) * float(scale_factor)))
+
+
+def _input_op(net: DcrNet, kind: int, out_t: int, in_size: int, crop: int, mean: Sequence[float], std: Sequence[float],
+              op_ints: Sequence[int] = (), post: Sequence[float] = (1.0, 0.0), scale_factor: Optional[float] = None) -> None:
+    """An op that reads the image batch (IM2COL_U8, STEM_S2D, STEM_ROWS): the centre `crop` of the in_size x in_size
+    image, ToTensor, Normalize(mean, std), the affine `post`, then the bilinear resize by `scale_factor`.
+    ints [out_t, IH, IW, crop_y, crop_x, H, W] + op_ints (+ [RH, RW]), floats mean + std + post (+ [float(1 / s)])."""
+    off = (in_size - crop) // 2
+    iargs = [out_t, in_size, in_size, off, off, crop, crop, *op_ints]
+    fargs = [*mean, *std, *post]
+    if scale_factor is not None and scale_factor != 1:
+        size = _scaled_size(crop, scale_factor)
+        iargs += [size, size]
+        fargs.append(float(np.float32(1.0 / float(scale_factor))))
+    net.op(kind, iargs, fargs)
+
+
 def _dense_from_grouped(w: torch.Tensor, c_in: int) -> torch.Tensor:
     """Grouped convolution weight [N, c_in/groups, kh, kw] -> the equivalent dense block-diagonal weight
     [N, c_in, kh, kw].  The tensor cores then run the grouped 3x3 convs of a ResNeXt trunk as ordinary dense
@@ -317,19 +340,13 @@ def build_sscd_resnet50(state_dict: Dict[str, torch.Tensor], max_batch: int = 64
     net = DcrNet(max_batch, precision)
     net.in_shape = (in_size, in_size)
     net.net_input = (crop, crop)
-    off = (in_size - crop) // 2
     eps = 1e-5
     src_crop = crop
-    stem_i, stem_f = [], []
-    if scale_factor is not None and scale_factor != 1:
-        # multi_scale (utils_ret.py:676-698): the transformed crop is bilinearly resized by `scale_factor` before the
-        # network; fused into the stem's input kernel.  Output size and coordinate scale as F.interpolate computes them.
-        import math
-        crop = int(math.floor(float(src_crop) * float(scale_factor)))
-        if crop % 2:
-            raise _lib.DcrError(f"scale_factor {scale_factor} gives an odd network input size {crop}")
-        stem_i = [crop, crop]
-        stem_f = [float(np.float32(1.0 / float(scale_factor)))]
+    # multi_scale (utils_ret.py:676-698): the transformed crop is bilinearly resized by `scale_factor` before the
+    # network; fused into the stem's input kernel
+    crop = _scaled_size(src_crop, scale_factor)
+    if scale_factor not in (None, 1) and crop % 2:
+        raise _lib.DcrError(f"scale_factor {scale_factor} gives an odd network input size {crop}")
     # stem: 7x7/2/pad-3 conv == 4x4/1 conv over the zero-padded 2x2 space-to-depth input (12 -> 16 channels); the
     # preprocessing (crop, ToTensor, Normalize) is fused into the space-to-depth kernel, and the GEMM kernel reads 4
     # horizontally adjacent 16-channel pixels as one 64-channel pixel through an overlapping-window tensor map
@@ -347,8 +364,7 @@ def build_sscd_resnet50(state_dict: Dict[str, torch.Tensor], max_batch: int = 64
             raise _lib.DcrError("stem='toeplitz' needs the one-plane (fast) mode and a 64-channel stem")
         units = int(net.lib.dcr_stem_plane_units(s, s))
         t_rows = net.tensor(2 * units, 8)
-        net.op(OP_STEM_ROWS, [t_rows, in_size, in_size, off, off, src_crop, src_crop] + stem_i,
-               list(mean) + list(std) + [1.0, 0.0] + stem_f)
+        _input_op(net, OP_STEM_ROWS, t_rows, in_size, src_crop, mean, std, scale_factor=scale_factor)
         w_id = net.param(_stem_toeplitz_weight(sd["conv1.weight"]).to(torch.bfloat16))
         pooled = stem == "toeplitz_pool"
         t_stem = net.tensor(hw * hw if pooled else s * s, 64)
@@ -362,7 +378,7 @@ def build_sscd_resnet50(state_dict: Dict[str, torch.Tensor], max_batch: int = 64
     else:
         t_stem = net.tensor(s * s, 64)
         t_z = net.tensor(u * u, 16)
-        net.op(OP_STEM_S2D, [t_z, in_size, in_size, off, off, src_crop, src_crop] + stem_i, list(mean) + list(std) + [1.0, 0.0] + stem_f)
+        _input_op(net, OP_STEM_S2D, t_z, in_size, src_crop, mean, std, scale_factor=scale_factor)
         net.conv(t_z, t_stem, u, u - 3, 64, _stem_s2d_weight(sd["conv1.weight"]), scale=sc, bias=bi, act=1, window=(16, u))
         net.flops_per_image += 2.0 * s * s * 64 * (147 - 256)   # count the real 147-tap work, not the zero padding
         t = net.tensor(hw * hw, 64)
@@ -446,8 +462,7 @@ def build_dino_vit(state_dict: Dict[str, torch.Tensor], max_batch: int = 64, pre
     global_pool: 'token' -> the CLS row [B, dim] (dino_vits.py:253-254); '' -> every token, flattened to
       [B, tokens * dim] as `rearrange(feats, 'b h w -> b (h w)')` does for --similarity_metric splitloss
       (dino_vits.py:255-256, utils_ret.py:728-737)."""
-    import math
-    sd = _strip({k: v.detach().cpu() for k, v in state_dict.items()}, ["module.", "backbone."])
+    sd =_strip({k: v.detach().cpu() for k, v in state_dict.items()}, ["module.", "backbone."])
     dim = sd["cls_token"].shape[-1]
     depth = 1 + max(int(k.split(".")[1]) for k in sd if k.startswith("blocks."))
     if not 1 <= n_last_layers <= depth:
@@ -457,12 +472,7 @@ def build_dino_vit(state_dict: Dict[str, torch.Tensor], max_batch: int = 64, pre
     depth_used = depth - n_last_layers + 1
     patch = int(sd["patch_embed.proj.weight"].shape[-1]) if patch is None else patch
     heads = dim // 64 if heads is None else heads
-    net_in = crop
-    rs_i, rs_f = [], []
-    if scale_factor is not None and scale_factor != 1:
-        net_in = int(math.floor(float(crop) * float(scale_factor)))
-        rs_i = [net_in, net_in]
-        rs_f = [float(np.float32(1.0 / float(scale_factor)))]
+    net_in = _scaled_size(crop, scale_factor)
     grid = (net_in - patch) // patch + 1
     n_patch = grid * grid
     tokens = n_patch + 1
@@ -474,11 +484,9 @@ def build_dino_vit(state_dict: Dict[str, torch.Tensor], max_batch: int = 64, pre
     net = DcrNet(max_batch, precision)
     net.in_shape = (in_size, in_size)
     net.net_input = (crop, crop)
-    off = (in_size - crop) // 2
     k_pad = first_conv_k_pad(patch, patch)
     t_cols = net.tensor(n_patch, k_pad)
-    net.op(OP_IM2COL_U8, [t_cols, in_size, in_size, off, off, crop, crop, patch, patch, patch, 0, k_pad] + rs_i,
-           list(mean) + list(std) + [1.0, 0.0] + rs_f)
+    _input_op(net, OP_IM2COL_U8, t_cols, in_size, crop, mean, std, [patch, patch, patch, 0, k_pad], scale_factor=scale_factor)
     t_patch = net.tensor(n_patch, dim)
     net.conv(t_cols, t_patch, n_patch, 1, k_pad, _first_conv_weight(sd["patch_embed.proj.weight"], k_pad),
              bias=sd["patch_embed.proj.bias"])
@@ -565,11 +573,9 @@ def build_clip_visual(state_dict: Dict[str, torch.Tensor], max_batch: int = 64, 
         raise _lib.DcrError("CLIP visual tower: positional embedding does not match the input size")
     net = DcrNet(max_batch, precision)
     net.in_shape, net.net_input = (in_size, in_size), (crop, crop)
-    off = (in_size - crop) // 2
     k_pad = first_conv_k_pad(patch, patch)
     t_cols = net.tensor(n_patch, k_pad)
-    net.op(OP_IM2COL_U8, [t_cols, in_size, in_size, off, off, crop, crop, patch, patch, patch, 0, k_pad],
-           list(mean) + list(std) + [1.0, 0.0])
+    _input_op(net, OP_IM2COL_U8, t_cols, in_size, crop, mean, std, [patch, patch, patch, 0, k_pad])
     t_patch = net.tensor(n_patch, dim)
     net.conv(t_cols, t_patch, n_patch, 1, k_pad, _first_conv_weight(w, k_pad))
     x0 = net.tensor(tokens, dim)
@@ -626,7 +632,7 @@ def build_vgg16_fc2(state_dict: Dict[str, torch.Tensor], max_batch: int = 50, pr
     h = 224
     k_pad = first_conv_k_pad(3, 3)
     t_cols = net.tensor(h * h, k_pad)
-    net.op(OP_IM2COL_U8, [t_cols, 224, 224, 0, 0, 224, 224, 3, 3, 1, 1, k_pad], list(mean) + list(std) + [1.0, 0.0])
+    _input_op(net, OP_IM2COL_U8, t_cols, 224, 224, mean, std, [3, 3, 1, 1, k_pad])
     w0 = sd["features.0.weight"]
     t = net.tensor(h * h, 64)
     net.conv(t_cols, t, h * h, 1, k_pad, _first_conv_weight(w0, k_pad), bias=sd["features.0.bias"], act=1)
@@ -689,7 +695,7 @@ def build_fid_inception(state_dict: Dict[str, torch.Tensor], max_batch: int = 50
     k_pad = first_conv_k_pad(3, 3)
     s = (299 - 3) // 2 + 1   # 149
     t_cols = net.tensor(s * s, k_pad)
-    net.op(OP_IM2COL_U8, [t_cols, 299, 299, 0, 0, 299, 299, 3, 3, 2, 0, k_pad], [0.5] * 3 + [0.5] * 3 + [2.0, -1.0])
+    _input_op(net, OP_IM2COL_U8, t_cols, 299, 299, [0.5] * 3, [0.5] * 3, [3, 3, 2, 0, k_pad], post=(2.0, -1.0))
     w1 = sd["Conv2d_1a_3x3.conv.weight"]
     sc, bi = _fold_bn(sd, "Conv2d_1a_3x3.bn", eps)
     t = net.tensor(s * s, 32)
