@@ -48,6 +48,7 @@ SIGNATURES = {
     "dcr_net_set_output": (C.c_int, [C.c_void_p, C.c_int]),
     "dcr_net_add_op": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_float), C.c_int]),
     "dcr_net_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "dcr_net_tensor": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
     "dcr_stem_plane_units": (C.c_int64, [C.c_int, C.c_int]),
     "dcr_net_forward_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "dcr_fid_create": (C.c_int, [C.c_int, C.POINTER(C.c_void_p)]),

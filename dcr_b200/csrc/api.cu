@@ -240,6 +240,14 @@ int dcr_net_forward(dcr_net* net, const uint8_t* images, int n, float* out, void
   return dcr::net_forward(reinterpret_cast<dcr::Net*>(net), images, n, out, as_stream(stream));
 }
 
+int dcr_net_tensor(const dcr_net* net, int t, void** ptr, int64_t* plane_stride) {
+  DCR_REQUIRE(ptr != nullptr && plane_stride != nullptr, "dcr_net_tensor: null out pointer");
+  long long ps = 0;
+  const int rc = dcr::net_tensor(reinterpret_cast<const dcr::Net*>(net), t, ptr, &ps);
+  *plane_stride = ps;
+  return rc;
+}
+
 int64_t dcr_stem_plane_units(int out_h, int out_w) { return dcr::stem_fused_plane_units(out_h, out_w); }
 int dcr_net_forward_f32(dcr_net* net, const float* x_nchw, int n, float* out, void* stream) {
   DCR_REQUIRE(x_nchw != nullptr, "dcr_net_forward_f32: null input");

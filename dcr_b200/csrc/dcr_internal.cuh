@@ -145,6 +145,7 @@ int net_fork(const Net* src, Net** out);
 int net_add_tensor(Net* n, long long rows_per_image, int C);
 int net_alias_tensor(Net* n, int src, long long rows_per_image, int C);
 int net_add_param(Net* n, const void* host, size_t bytes);
+int net_tensor(const Net* n, int t, void** ptr, long long* plane_stride);
 int net_set_output(Net* n, int dim);
 int net_add_op(Net* n, int kind, const int* iargs, int ni, const float* fargs, int nf);
 // images: uint8 NHWC [B,IH,IW,3] (raw, the transform is fused) -- or, when images_f32 != nullptr, fp32 NCHW

@@ -187,6 +187,13 @@ int net_alias_tensor(Net* n, int src, long long rows_per_image, int C) {
   return static_cast<int>(n->tensors.size()) - 1;
 }
 
+int net_tensor(const Net* n, int t, void** ptr, long long* plane_stride) {
+  DCR_REQUIRE(n && t >= 0 && t < static_cast<int>(n->tensors.size()), "net_tensor: bad tensor id %d", t);
+  *ptr = n->tensors[t].ptr;
+  *plane_stride = n->tensors[t].plane_stride;
+  return 0;
+}
+
 int net_add_param(Net* n, const void* host, size_t bytes) {
   DCR_REQUIRE(n && host && bytes > 0, "net_add_param: bad arguments");
   void* p = nullptr;

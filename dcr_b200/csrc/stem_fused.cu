@@ -52,6 +52,7 @@ struct StemParams {
   int OHp, OWp, prow_per_part;   // pooling: pooled output size, pooled rows per part
   int win_units;                 // units copied per plane and tile: 512 + 3 * PW + 3, rounded up to 8
   int win_stages;
+  int ring_rows;                 // pooling: conv rows in the shared-memory ring (a power of two, see stem_ring_rows)
   const float* scale;
   const float* bias;
   __nv_bfloat16* out;            // NHWC [B][OH][OW][64]
@@ -86,7 +87,7 @@ DCR_DEVICE int unit_begin(const StemParams& p, int part, bool pool) {
 }
 
 // kPool: the 3x3 / stride 2 / pad 1 max pool that follows the stem (torchvision ResNet.maxpool) is taken in the epilogue:
-// conv outputs (post BN + ReLU, bf16) go into a ring of 8 conv rows in shared memory and a pooled row is emitted as soon
+// conv outputs (post BN + ReLU, bf16) go into a ring of conv rows in shared memory and a pooled row is emitted as soon
 // as its three conv rows are complete -- the 112 x 112 x 64 stem activation (411 MB at batch 256) never reaches HBM.
 template <bool kPool>
 __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_constant__ CUtensorMap tmap_w, const StemParams p) {
@@ -96,9 +97,10 @@ __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_co
   const int stage_bytes = (2 * win_bytes + 1023) & ~1023;
   uint8_t* s_w = smem;                                          // 32 KB, 4 k-blocks
   uint8_t* s_win = s_w + kWBytes;                               // win_stages x [even | odd]
-  uint8_t* s_out = s_win + p.win_stages * stage_bytes;          // 2 x [128 positions x 128 B] | kPool: ring of 8 conv rows
+  uint8_t* s_out = s_win + p.win_stages * stage_bytes;          // 2 x [128 positions x 128 B] | kPool: ring of conv rows
   const int ring_row_bytes = p.OW * 128;
-  uint8_t* acc_xpose = s_out + (kPool ? ((8 * ring_row_bytes + 1023) & ~1023) : 2 * 16384);   // [8 warps]
+  const int ring_mask = p.ring_rows - 1;
+  uint8_t* acc_xpose = s_out + (kPool ? ((p.ring_rows * ring_row_bytes + 1023) & ~1023) : 2 * 16384);   // [8 warps]
   float* sb = reinterpret_cast<float*>(acc_xpose + 8 * kAccXposeWarpBytes);   // scale[64] | bias[64]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sb + 128);
   uint64_t* w_full = bars;
@@ -243,25 +245,26 @@ __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_co
             }
             // the staging buffer (blk & 1) is rewritten two blocks later: the barrier of the next block orders that
           } else {
-            // conv row ring: ring[(y & 7)][x][64 ch], 16-byte chunks XOR-swizzled by x
+            // conv row ring: ring[y mod ring_rows][x][64 ch], 16-byte chunks XOR-swizzled by x
             const int m = mblk + static_cast<int>(row);
             const int y = m / p.PW, x = m - y * p.PW;
             if (x < p.OW && y >= row_lo && y < row_hi) {
-              const uint32_t rrow = so_addr + (y & 7) * ring_row_bytes + x * 128;
+              const uint32_t rrow = so_addr + (y & ring_mask) * ring_row_bytes + x * 128;
 #pragma unroll
               for (int q = 0; q < 4; ++q) st_shared_v4(rrow + (((half * 4 + q) ^ (x & 7)) << 4), v[q]);
             }
             asm volatile("bar.sync 2, 256;" ::: "memory");
-            // rows <= yc are complete; emit every pooled row whose last conv row is in (ring depth 8 keeps the rows a slower
-            // thread is still pooling apart from the rows the next block writes)
+            // rows <= yc are complete; emit every pooled row whose last conv row is in (the ring depth keeps the rows a
+            // slower thread is still pooling, and the rows of the pending pooled row, apart from the rows the next block
+            // writes: stem_ring_rows)
             const int yc = min((mblk + 128) / p.PW - 1, row_hi - 1);
             while (next_yp < yp_end && min(2 * next_yp + 1, p.OH - 1) <= yc) {
               // taps outside the image are replaced by the nearest tap INSIDE the window (the maximum is idempotent), so
               // there is no branching and the nine 16-byte loads of an item are independent and all in flight together
               const int y1 = 2 * next_yp;
-              const uint32_t r0 = so_addr + (max(y1 - 1, 0) & 7) * ring_row_bytes;
-              const uint32_t r1 = so_addr + (y1 & 7) * ring_row_bytes;
-              const uint32_t r2 = so_addr + (min(y1 + 1, p.OH - 1) & 7) * ring_row_bytes;
+              const uint32_t r0 = so_addr + (max(y1 - 1, 0) & ring_mask) * ring_row_bytes;
+              const uint32_t r1 = so_addr + (y1 & ring_mask) * ring_row_bytes;
+              const uint32_t r2 = so_addr + (min(y1 + 1, p.OH - 1) & ring_mask) * ring_row_bytes;
               for (int idx = etid; idx < p.OWp * 8; idx += 256) {
                 const int xp = idx >> 3, c = idx & 7;
                 const int x1 = 2 * xp, x0 = max(x1 - 1, 0), x2 = min(x1 + 1, p.OW - 1);
@@ -300,6 +303,18 @@ __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_co
 
 }
 
+// Conv rows the pooling ring must hold.  While some threads still pool the rows of block k, others already write block
+// k+1 (there is no barrier between the pooling loop and the next block's ring stores).  The rows block k may still read
+// start at yc(k-1) - 1 >= floor(m_k / PW) - 2 (m_k: first position of block k), and block k+1 writes rows up to
+// floor((m_k + 255) / PW) <= floor(m_k / PW) + floor(255 / PW) + 1.  Those rows must fall in distinct ring slots:
+// depth >= floor(255 / PW) + 4.  8 rows suffice from PW >= 52 (stem output width 48, a 96-pixel network input); a
+// narrower image takes 16, 32 or 64.
+int stem_ring_rows(int PW) {
+  int r = 8;
+  while (r < 255 / PW + 4) r *= 2;
+  return r;
+}
+
 }  // namespace
 
 // geometry shared by the host graph builder (through dcr_stem_plane_units), stem_rows (image_in.cu) and stem_conv
@@ -328,6 +343,7 @@ int stem_conv(const __nv_bfloat16* planes, int B, int OH, int OW, const __nv_bfl
   p.scale = scale; p.bias = bias; p.out = out;
   p.OHp = (OH - 1) / 2 + 1;
   p.OWp = (OW - 1) / 2 + 1;
+  p.ring_rows = stem_ring_rows(p.PW);
   if (pool) {
     const int parts = (p.OHp % 4 == 0) ? 4 : ((p.OHp % 2 == 0) ? 2 : 1);
     p.units_per_img = parts;
@@ -348,7 +364,7 @@ int stem_conv(const __nv_bfloat16* planes, int B, int OH, int OW, const __nv_bfl
   CUtensorMap tw;
   if (int rc = make_tmap_2d_bf16(&tw, weight, kSN, 256, 256, kSN, 64)) return rc;
   const size_t stage = (static_cast<size_t>(2) * p.win_units * 16 + 1023) & ~size_t(1023);
-  const size_t out_bytes = pool ? ((static_cast<size_t>(8) * OW * 128 + 1023) & ~size_t(1023)) : 2 * 16384;
+  const size_t out_bytes = pool ? ((static_cast<size_t>(p.ring_rows) * OW * 128 + 1023) & ~size_t(1023)) : 2 * 16384;
   const size_t fixed = 1024 + kWBytes + out_bytes + 8 * kAccXposeWarpBytes + 512 + 256;
   // with the pooling ring of a 224-pixel image only one window stage fits: the next tile's window is loaded once the
   // current tile's MMAs have completed

@@ -195,6 +195,9 @@ int dcr_net_set_output(dcr_net* net, int dim);
 int dcr_net_add_op(dcr_net* net, int kind, const int* iargs, int n_iargs, const float* fargs, int n_fargs);
 /* images: DEVICE uint8 [n, IH, IW, 3]; out: DEVICE fp32 [n, dim]; n <= max_batch */
 int dcr_net_forward(dcr_net* net, const uint8_t* images, int n, float* out, void* stream);
+/* device address and plane stride (elements) of activation tensor t: read/write, for tests and tools.  The buffer holds
+ * `planes` planes of [max_batch, rows_per_image, channels] bf16, plane p at *ptr + p * plane_stride elements. */
+int dcr_net_tensor(const dcr_net* net, int t, void** ptr, int64_t* plane_stride);
 /* units (16-byte pixels) per image and plane of the STEM_ROWS tensor for an OH x OW stem output (includes read slack) */
 int64_t dcr_stem_plane_units(int out_h, int out_w);
 /* Same network, fed with what the reference's own loop feeds `model(samples)` (utils_ret.py:751; embedding_search/
