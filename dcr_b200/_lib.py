@@ -55,6 +55,9 @@ SIGNATURES = {
     "dcr_fid_destroy": (None, [C.c_void_p]),
     "dcr_fid_accumulate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "dcr_fid_finalize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "dcr_fid_packed_size": (C.c_size_t, [C.c_int]),
+    "dcr_fid_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dcr_fid_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "dcr_split_rescore": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                     C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dcr_topk_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

@@ -160,7 +160,8 @@ def main_worker(gpu, ngpus_per_node, args) -> int:
     """diff_retrieval.py:224-483 restricted to the hot path.  Distributed runs shard BOTH image sets contiguously over
     the ranks (the reference shards the gallery loader with a DistributedSampler, :345-348, and funnels every batch to
     rank 0); every rank embeds its shards, scores all queries against its gallery shard and the per-shard top-k lists
-    are all-gathered and merged (dcr_b200/dist.py) -- same result as the single-process run, on every rank."""
+    are all-gathered and merged (dcr_b200/dist.py) -- same result as the single-process run, on every rank.  With
+    --fid_weights the FID statistics are sharded the same way and their float64 states merged over the ranks."""
     args.gpu = gpu
     if args.multiprocessing_distributed and args.gpu != 0:                                    # :229-232
         import builtins
@@ -208,6 +209,14 @@ def main_worker(gpu, ngpus_per_node, args) -> int:
                                    query_sizes=v_sizes)                                         # :403, :418
         out = {"values": main_v, "indices": main_l, "bg_values": bg[:, -1],
                "stats": retrieval.retrieval_stats(main_v[:, 0], bg[:, -1])}
+    fid_val = None
+    if args.fid_weights and world > 1:
+        # every rank embeds its shard of both folders; the fp64 statistics are merged over the ranks (dcr_b200/fid.py)
+        from . import fid, nets
+        inc = nets.build_fid_inception(load_state_dict(args.fid_weights), max_batch=50)
+        m1, s1 = fid.compute_statistics_of_path(args.val_dir, inc, 50, num_workers=args.workers, distributed=True)
+        m2, s2 = fid.compute_statistics_of_path(args.query_dir, inc, 50, num_workers=args.workers, distributed=True)
+        fid_val = fid.frechet_distance(m1, s1, m2, s2)
     if rank == 0:                                                                             # :375 only rank 0 writes
         dp = os.sep.join(os.path.normpath(args.query_dir).split(os.sep)[-3:])                  # :378
         save = f"ret_plots/{dp}/images/{args.pt_style}_{args.arch}_{args.similarity_metric}{args.stype}/"   # :408
@@ -217,11 +226,12 @@ def main_worker(gpu, ngpus_per_node, args) -> int:
         print("Simscores @x% part done")                                                      # :470
         print(out["stats"])
         if args.fid_weights:
-            from . import fid, nets
-            inc = nets.build_fid_inception(load_state_dict(args.fid_weights), max_batch=50)
-            val = fid.fid_from_images(inc, fid.load_resized(args.val_dir), fid.load_resized(args.query_dir))   # :597-600
-            print({"fid": val})
-            out["stats"]["fid"] = val
+            if fid_val is None:
+                from . import fid, nets
+                inc = nets.build_fid_inception(load_state_dict(args.fid_weights), max_batch=50)
+                fid_val = fid.fid_from_images(inc, fid.load_resized(args.val_dir), fid.load_resized(args.query_dir))   # :597-600
+            print({"fid": fid_val})
+            out["stats"]["fid"] = fid_val
         with open(os.path.join(save, "stats.json"), "w") as f:
             json.dump(out["stats"], f)
     if args.distributed:

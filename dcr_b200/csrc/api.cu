@@ -269,5 +269,16 @@ int dcr_fid_finalize(dcr_fid* st, double* mu, double* sigma, int64_t* n_out, voi
   if (n_out) *n_out = n;
   return rc;
 }
+size_t dcr_fid_packed_size(int d) {
+  const size_t bytes = dcr::fid_packed_size(d);
+  if (bytes == 0) dcr::set_error(-1, "dcr_fid_packed_size: bad dim %d", d);
+  return bytes;
+}
+int dcr_fid_export(const dcr_fid* st, void* packed, void* stream) {
+  return dcr::fid_export(reinterpret_cast<const dcr::FidState*>(st), packed, as_stream(stream));
+}
+int dcr_fid_merge(dcr_fid* st, const void* packed, int count, void* stream) {
+  return dcr::fid_merge(reinterpret_cast<dcr::FidState*>(st), packed, count, as_stream(stream));
+}
 
 }  // extern "C"

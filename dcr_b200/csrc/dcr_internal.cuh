@@ -159,5 +159,8 @@ int fid_create(int d, FidState** out);
 void fid_destroy(FidState* s);
 int fid_accumulate(FidState* s, const float* act, int n, cudaStream_t stream);
 int fid_finalize(FidState* s, double* mu_host, double* sigma_host, long long* n_out, cudaStream_t stream);
+size_t fid_packed_size(int d);
+int fid_export(const FidState* s, void* packed, cudaStream_t stream);
+int fid_merge(FidState* s, const void* packed, int count, cudaStream_t stream);
 
 }  // namespace dcr

@@ -78,7 +78,111 @@ __global__ void __launch_bounds__(256)
     }
   if (ti == tj && threadIdx.x < kTile && ti * kTile + threadIdx.x < d) sum[ti * kTile + threadIdx.x] += colsum;
 }
+
+// Packed state (include/dcr_b200.h): int64 header {kPackedMagic, d, n, 0}, then double shift[d], sum[d], xtx[d*d].
+constexpr long long kPackedMagic = 0x31444946524344LL;   // "DCRFID1"
+constexpr int kHeaderWords = 4;
+
+__host__ __device__ inline const double* packed_shift(const unsigned char* p) {
+  return reinterpret_cast<const double*>(p + kHeaderWords * sizeof(long long));
+}
+
+// Folds `count` packed states into (shift, sum, xtx) in order, one thread per element (i, j >= i) of the triangle.
+// n_state: the state's count before the fold.  When it is 0, the first non-empty peer is copied (its shift included)
+// and later peers are rebased onto that shift, so no thread reads `shift` then and the diagonal threads may write it.
+// Every element sees the peers in the same fixed order: the result does not depend on scheduling.
+__global__ void fid_merge_kernel(const unsigned char* __restrict__ packed, size_t stride, int count, int d,
+                                 long long n_state, double* __restrict__ shift, double* __restrict__ sum,
+                                 double* __restrict__ xtx) {
+  const size_t e = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (e >= static_cast<size_t>(d) * d) return;
+  const int i = static_cast<int>(e / d), j = static_cast<int>(e % d);
+  if (j < i) return;
+  long long na = n_state;
+  double ci = 0.0, cj = 0.0, si = 0.0, sij = 0.0;
+  if (na > 0) {
+    ci = shift[i];
+    cj = shift[j];
+    si = sum[i];
+    sij = xtx[e];
+  }
+  for (int p = 0; p < count; ++p) {
+    const unsigned char* b = packed + static_cast<size_t>(p) * stride;
+    const long long nb = reinterpret_cast<const long long*>(b)[2];
+    if (nb == 0) continue;
+    const double* cb = packed_shift(b);
+    const double* sb = cb + d;
+    const double* xb = sb + d;
+    if (na == 0) {
+      ci = cb[i];
+      cj = cb[j];
+      si = sb[i];
+      sij = xb[e];
+    } else {
+      // delta = c_a - c_b:  S_a += S_b - s_b delta^T - delta s_b^T + n_b delta delta^T,  s_a += s_b - n_b delta
+      const double di = ci - cb[i], dj = cj - cb[j], sbi = sb[i], sbj = sb[j], fn = static_cast<double>(nb);
+      sij += xb[e] - sbi * dj - di * sbj + fn * di * dj;
+      si += sbi - fn * di;
+    }
+    na += nb;
+  }
+  xtx[e] = sij;
+  if (i == j) {
+    sum[i] = si;
+    if (n_state == 0) shift[i] = ci;
+  }
+}
 }  // namespace
+
+size_t fid_packed_size(int d) {
+  if (d < 1 || d > 16384) return 0;
+  return kHeaderWords * sizeof(long long) + sizeof(double) * (2 * static_cast<size_t>(d) + static_cast<size_t>(d) * d);
+}
+
+int fid_export(const FidState* s, void* packed, cudaStream_t stream) {
+  DCR_REQUIRE(s && packed, "fid_export: null argument");
+  DCR_REQUIRE((reinterpret_cast<uintptr_t>(packed) & 7) == 0, "fid_export: packed buffer must be 8-byte aligned");
+  const int d = s->d;
+  const long long hdr[kHeaderWords] = {kPackedMagic, d, s->n, 0};
+  unsigned char* p = static_cast<unsigned char*>(packed);
+  double* shift = reinterpret_cast<double*>(p + kHeaderWords * sizeof(long long));
+  // pageable source: the copy has been staged when the call returns, so `hdr` may go out of scope
+  DCR_CUDA_CHECK(cudaMemcpyAsync(p, hdr, sizeof(hdr), cudaMemcpyHostToDevice, stream));
+  DCR_CUDA_CHECK(cudaMemcpyAsync(shift, s->shift, sizeof(double) * d, cudaMemcpyDeviceToDevice, stream));
+  DCR_CUDA_CHECK(cudaMemcpyAsync(shift + d, s->sum, sizeof(double) * d, cudaMemcpyDeviceToDevice, stream));
+  DCR_CUDA_CHECK(cudaMemcpyAsync(shift + 2 * d, s->xtx, sizeof(double) * d * d, cudaMemcpyDeviceToDevice, stream));
+  return 0;
+}
+
+int fid_merge(FidState* s, const void* packed, int count, cudaStream_t stream) {
+  DCR_REQUIRE(s && (packed || count == 0), "fid_merge: null argument");
+  DCR_REQUIRE(count >= 0, "fid_merge: bad count %d", count);
+  if (count == 0) return 0;
+  DCR_REQUIRE((reinterpret_cast<uintptr_t>(packed) & 7) == 0, "fid_merge: packed buffer must be 8-byte aligned");
+  const int d = s->d;
+  const size_t stride = fid_packed_size(d);
+  // the headers: one strided device-to-host copy, so that the state's host-side count is right on return
+  std::vector<long long> hdr(static_cast<size_t>(count) * kHeaderWords);
+  DCR_CUDA_CHECK(cudaMemcpy2DAsync(hdr.data(), kHeaderWords * sizeof(long long), packed, stride,
+                                   kHeaderWords * sizeof(long long), count, cudaMemcpyDeviceToHost, stream));
+  DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
+  long long n = s->n;
+  for (int p = 0; p < count; ++p) {
+    const long long* h = &hdr[static_cast<size_t>(p) * kHeaderWords];
+    DCR_REQUIRE(h[0] == kPackedMagic, "fid_merge: packed state %d is not an exported dcr_fid state", p);
+    DCR_REQUIRE(h[1] == d, "fid_merge: packed state %d has d = %lld, this state has d = %d", p, h[1], d);
+    DCR_REQUIRE(h[2] >= 0, "fid_merge: packed state %d has a negative count %lld", p, h[2]);
+    n += h[2];
+  }
+  if (n == s->n) return 0;   // only empty states
+  const size_t elems = static_cast<size_t>(d) * d;
+  fid_merge_kernel<<<static_cast<unsigned>((elems + 255) / 256), 256, 0, stream>>>(
+      static_cast<const unsigned char*>(packed), stride, count, d, s->n, s->shift, s->sum, s->xtx);
+  count_launch();
+  DCR_CUDA_CHECK(cudaGetLastError());
+  s->n = n;
+  return 0;
+}
 
 int fid_create(int d, FidState** out) {
   DCR_REQUIRE(d >= 1 && d <= 16384, "fid_create: bad dim %d", d);

@@ -216,6 +216,26 @@ void dcr_fid_destroy(dcr_fid* st);
 int dcr_fid_accumulate(dcr_fid* st, const float* act, int n, void* stream);
 int dcr_fid_finalize(dcr_fid* st, double* mu, double* sigma, int64_t* n_out, void* stream);
 
+/* Statistics of one image set computed on several devices (each rank accumulates its shard): export every state, exchange
+ * the packed states (an all-gather), and fold them into one state.  A state keeps a shift c (the mean of its first batch),
+ * s = sum(x - c), S = sum((x - c)(x - c)^T) (upper triangle) and n; folding peer b into a rebases b onto a's shift,
+ * delta = c_a - c_b:
+ *     s_a += s_b - n_b delta,   S_a += S_b - s_b delta^T - delta s_b^T + n_b delta delta^T,   n_a += n_b
+ * (an empty a takes b as it is, shift included).
+ * Packed layout, dcr_fid_packed_size(d) bytes, 8-byte aligned (DEVICE memory):
+ *     int64 header[4] = {0x31444946524344 ("DCRFID1" in memory), d, n, 0}
+ *     double shift[d], sum[d], xtx[d*d]   (row-major; only the upper triangle i <= j is meaningful; shift is undefined
+ *                                          when n = 0)
+ * dcr_fid_packed_size returns 0 for a bad d.  dcr_fid_export enqueues device-to-device copies on `stream`.
+ * dcr_fid_merge folds `count` packed states laid out back to back (state p at packed + p * dcr_fid_packed_size(d)) into
+ * `st`, in order p = 0, 1, ...: one float64 kernel, each element of the triangle loops over the peers in that order, so
+ * the result is the same on every run and every rank that folds the same states.  States with n = 0 are skipped; a
+ * state of another d (or not produced by dcr_fid_export) is an error and nothing is merged.  It reads the headers with
+ * one synchronous device-to-host copy on `stream`.  dcr_fid_accumulate and dcr_fid_finalize work on the merged state. */
+size_t dcr_fid_packed_size(int d);
+int dcr_fid_export(const dcr_fid* st, void* packed, void* stream);
+int dcr_fid_merge(dcr_fid* st, const void* packed, int count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
