@@ -288,7 +288,7 @@ bool conv3x3_halo_eligible(const ConvGemmDesc& d) {
   const bool shape = d.kh == 3 && d.kw == 3 && d.stride == 1 && d.pad_h == 1 && d.pad_w == 1 && d.in_stride_w == 0;
   const bool fast = d.n_terms == 1 && d.term_a[0] == 0 && d.term_w[0] == 0 && !d.exact && d.out != nullptr &&
                     d.out_planes <= 1 && d.out_f32 == nullptr && d.res == nullptr && (d.act == 0 || d.act == 1);
-  const bool dims = d.C % 64 == 0 && d.ld_in == d.C && d.N % 64 == 0 && d.N <= (tuning_flag("DCR_CONV_HALO_N256") ? 256 : 128) && d.ld_out % 8 == 0 &&
+  const bool dims = d.C % 64 == 0 && d.ld_in == d.C && d.N % 64 == 0 && d.N <= 128 && d.ld_out % 8 == 0 &&
                     d.out_col_off % 8 == 0 && d.W + 2 <= 64 && d.W >= 8 && d.H >= 2 && d.B >= 1;
   return shape && fast && dims;
 }
@@ -311,16 +311,15 @@ int conv3x3_halo(const ConvGemmDesc& d, cudaStream_t stream) {
   HaloMaps maps;
   memset(&maps, 0, sizeof(maps));
   if (int rc = make_tmap_nhwc_box_bf16(&maps.a, d.in, d.B, d.H, d.W, d.C, d.C, p.Wp, p.R + 2)) return rc;
-  const int BN = d.N <= 64 ? 64 : (d.N <= 128 ? 128 : 256);
+  const int BN = d.N <= 64 ? 64 : 128;
   const int ktot = 9 * p.cblocks * 64;
   if (int rc = make_tmap_2d_bf16(&maps.w, d.weight, d.N, ktot, ktot, BN, 64)) return rc;
   if (int rc = make_tmap_nhwc_box_bf16(&maps.out, d.out, d.B, d.H, d.W, d.ld_out, d.ld_out, d.W, p.R)) return rc;
   // all taps resident when the weights are small (ResNet layer1: 9 x [64 x 64] = 72 KB)
-  const bool resident = BN == 64 && static_cast<size_t>(9) * p.cblocks * BN * 128 <= 80 * 1024 && !tuning_flag("DCR_HALO_NO_RESIDENT");
+  const bool resident = BN == 64 && static_cast<size_t>(9) * p.cblocks * BN * 128 <= 80 * 1024;
   if (BN == 64) return resident ? launch_halo<64, true>(maps, p, di->num_sms, di->max_smem_optin, stream)
                                 : launch_halo<64, false>(maps, p, di->num_sms, di->max_smem_optin, stream);
-  if (BN == 128) return launch_halo<128, false>(maps, p, di->num_sms, di->max_smem_optin, stream);
-  return launch_halo<256, false>(maps, p, di->num_sms, di->max_smem_optin, stream);
+  return launch_halo<128, false>(maps, p, di->num_sms, di->max_smem_optin, stream);
 }
 
 }  // namespace dcr

@@ -538,7 +538,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 bool wants_a_resident(const GemmParams& p, int BN, bool im2col, size_t max_smem) {
   const int k_iters_h = p.n_terms * p.taps * p.cblocks;
   if (!(!im2col && p.tma_epi && p.n_terms == 1 && p.num_n_tiles >= 2 && (p.res != nullptr || p.num_n_tiles >= 4) &&
-        k_iters_h * kAStage <= 64 * 1024 && p.num_n_tiles * BN <= 4096 && !tuning_flag("DCR_GEMM_NO_ARES")))
+        k_iters_h * kAStage <= 64 * 1024 && p.num_n_tiles * BN <= 4096))
     return false;
   // the resident rows, the all-blocks affine table and the staging tiles must leave at least three W stages; otherwise
   // the layer runs with the default schedule
@@ -634,11 +634,6 @@ int conv_gemm(const ConvGemmDesc& d, cudaStream_t stream) {
     const long long m_tiles = (M + kBM - 1) / kBM;
     while (BN > 64 && ktot >= 1024 && m_tiles * ((d.N + BN - 1) / BN) * 4 <= di->num_sms) BN /= 2;
   }
-  if (d.force_bn) BN = d.force_bn;
-  {
-    const int bn_im2col = tuning_int("DCR_GEMM_BN_IM2COL", 0);   // tuning experiments: tile width of the k x k convolutions
-    if (im2col && (bn_im2col == 64 || bn_im2col == 128 || bn_im2col == 256) && d.N >= bn_im2col) BN = bn_im2col;
-  }
   for (int pl = 0; pl < 3; ++pl) {
     const int pa = std::min(pl, a_planes - 1), pw = std::min(pl, w_planes - 1);
     const __nv_bfloat16* abase = d.in + pa * d.in_plane_stride;
@@ -686,7 +681,7 @@ int conv_gemm(const ConvGemmDesc& d, cudaStream_t stream) {
   p.out_f32 = d.out_f32;
   p.ld_out_f32 = d.ld_out_f32;
   p.act = d.act;
-  p.fast_gelu = (d.n_terms == 1 && p.out_planes <= 1 && !tuning_flag("DCR_GELU_ERF")) ? 1 : 0;
+  p.fast_gelu = (d.n_terms == 1 && p.out_planes <= 1) ? 1 : 0;
   // tile order: with several column blocks and an A matrix larger than what L2 keeps between the passes, m-fastest order
   // streams A from HBM once per column block
   const double a_bytes = 2.0 * a_planes * (im2col ? static_cast<double>(d.B) * d.H * d.W * d.C : static_cast<double>(M) * d.C);

@@ -68,7 +68,6 @@ struct ConvGemmDesc {
   float* out_f32 = nullptr;
   int ld_out_f32 = 0;
   int act = 0;        // 0 none, 1 relu, 2 gelu(erf)
-  int force_bn = 0;   // 0 = auto tile width
   int exact = 0;      // 1 = float64 accumulation on the CUDA cores (conv_exact.cu) instead of the tensor cores
 };
 int conv_gemm(const ConvGemmDesc& d, cudaStream_t stream);

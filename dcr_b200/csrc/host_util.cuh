@@ -37,10 +37,11 @@ struct DeviceInfo {
 void count_launch(int n = 1);
 long long launch_count();
 
-// Tuning knobs (DCR_SIM_KP0, DCR_SIM_SETS, DCR_GEMM_NO_ARES, ...) are honoured ONLY when DCR_B200_TUNING=1 is set in the
-// environment: a stray variable cannot change what a benchmark or a test runs.  Every knob selects between variants
-// that produce identical results.  (The timing-experiment modes that produce garbage results are compile-time only:
-// -DDCR_SIM_TIMING_MODE / -DDCR_GEMM_TIMING_MODE / -DDCR_HALO_TIMING_MODE, all 0 in the shipped library.)
+// Test switches: they exist so that the tests can run a second path on the same input and compare it with the one the
+// library picks.  They are DCR_ATTN_FP32, DCR_LN_GENERIC, DCR_POOL_GENERIC, DCR_NO_BLOCK_FUSION, DCR_SIM_RESCORE_BLOCK,
+// DCR_CONV_NO_HALO, DCR_GEMM_DIRECT_EPILOGUE and DCR_GEMM_TILE_ORDER, and they are honoured ONLY when DCR_B200_TUNING=1
+// is set in the environment: a stray variable cannot change what a benchmark or a user's run computes.  Every other
+// choice of path is made from the problem and the device.
 bool tuning_enabled();
 int tuning_int(const char* name, int dflt);
 bool tuning_flag(const char* name);   // true when tuning is enabled and the variable is set (to anything)

@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (tiled + im2col), wgmma, cluster helpers.  Everything here is device-only and header-only.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (tiled + im2col), wgmma.  Everything here is device-only and header-only.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -9,7 +9,6 @@ namespace dcr {
 #define DCR_DEVICE __device__ __forceinline__
 
 DCR_DEVICE uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-DCR_DEVICE uint32_t lane_id() { uint32_t l; asm volatile("mov.u32 %0, %%laneid;" : "=r"(l)); return l; }
 
 DCR_DEVICE bool elect_one() {
   uint32_t pred = 0;
@@ -22,19 +21,6 @@ DCR_DEVICE bool elect_one() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// cluster helpers
-DCR_DEVICE uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-DCR_DEVICE void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-DCR_DEVICE void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-DCR_DEVICE void cluster_sync() { cluster_arrive(); cluster_wait(); }
-// map a local shared address to the same offset in CTA `rank` of the cluster (shared::cluster window)
-DCR_DEVICE uint32_t mapa(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-
-// ----------------------------------------------------------------------------------------------
 // mbarrier
 DCR_DEVICE void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
@@ -44,11 +30,6 @@ DCR_DEVICE void fence_proxy_async() { asm volatile("fence.proxy.async.shared::ct
 
 DCR_DEVICE void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// arrive on the barrier at the same smem offset in CTA `rank` of the cluster
-DCR_DEVICE void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  uint32_t remote = mapa(smem_u32(bar), rank);
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 DCR_DEVICE void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -88,22 +69,6 @@ struct PipeState {
     }
   }
 };
-// acquire at cluster scope: needed when the arrival came from the peer CTA / a multicast commit
-DCR_DEVICE bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-DCR_DEVICE void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  while (!mbar_try_wait_cluster(bar, parity)) {
-  }
-}
 
 // ----------------------------------------------------------------------------------------------
 // TMA
@@ -121,14 +86,6 @@ DCR_DEVICE void tma_load_2d(void* dst, const void* tmap, uint64_t* bar, int c0, 
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
       " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
-      : "memory");
-}
-
-DCR_DEVICE void tma_load_3d(void* dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2, uint64_t hint) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(hint)
       : "memory");
 }
 

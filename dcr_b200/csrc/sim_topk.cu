@@ -58,10 +58,10 @@ struct SimParams {
   int* cand_cnt;       // [n_slots][rows_per_qtile]
   float* cand_thr;     // [n_slots][rows_per_qtile]
   const int* bias_flag;    // device flag: 0 = ignore col_bias (query centring switched off for this data)
-  const float* col_bias;   // [ng_pad] per-gallery-row score offset nu.(g-mu) added to every accumulator column; null = none
+  const float* col_bias;   // [ng_pad] per-gallery-row score offset nu.(g-mu) added to every accumulator column
   const float* thr_init;   // per query row: start thresholds (second-chance pass); null = seed by warm-up replay
   unsigned int* gthr;      // [nq_pad] per query row: best threshold any unit has reached so far, as an order-preserving
-                           // unsigned key (0 = none); null = no sharing
+                           // unsigned key (0 = none)
   unsigned long long* clk; // [4] clock64 / globaltimer at the start and end of CTA 0 (SM clock under this kernel); null = off
 };
 
@@ -505,7 +505,7 @@ template <bool kBias, int kSets>
 __global__ void __launch_bounds__(32 + 128 * kSets, 1)
     sim_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_g,
                     const SimParams p) {
-  if (((p.col_bias != nullptr) && (p.bias_flag != nullptr) && (*p.bias_flag != 0)) != kBias) return;
+  if (((p.bias_flag != nullptr) && (*p.bias_flag != 0)) != kBias) return;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // carve-up (all tile bases 1024-byte aligned for the 128B swizzle)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -625,7 +625,7 @@ __global__ void __launch_bounds__(32 + 128 * kSets, 1)
       // in the gallery) is a valid drop bound for every other unit sweeping the same query tile.  Read once per tile
       // (the load is issued before the main loop), published when it has risen.
       const int qrow_s = qi * rows_per_qtile + static_cast<int>(row);
-      unsigned int* gslot = (p.gthr && qrow_s < p.nq) ? p.gthr + qrow_s : nullptr;
+      unsigned int* gslot = qrow_s < p.nq ? p.gthr + qrow_s : nullptr;
       float published = gslot ? thr_from_key(*reinterpret_cast<volatile unsigned int*>(gslot)) : INFINITY;
       if (gslot) thr = fmaxf(thr, published);
       if (!stream_a) mbar_wait(a_full, seg & 1);
@@ -895,7 +895,7 @@ struct RescoreParams {
   const int* cand_cnt;
   const float* cand_thr;
   const int* qmap;                  // pass row -> caller's row; null = identity
-  const float* mu;                  // gallery centre; null = no centring
+  const float* mu;                  // gallery centre
   const float* nu;                  // query centre, used when *nu_flag != 0; null = none
   const int* nu_flag;
   const float* q_norm_hat;          // per caller row, from stage 1
@@ -1082,7 +1082,7 @@ __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const R
     eps += 3e-7f * (qx + nun) * g_norm;
   }
   double qmu = 0.0;   // q . mu in fp64: the constant the centred approximate scores are offset by
-  if (p.mu) {
+  {
     float mu2 = 0.f;
     for (int c = lane; c < d; c += 32) {
       qmu = fma(qs[c], static_cast<double>(p.mu[c]), qmu);
@@ -1339,7 +1339,6 @@ __global__ void __launch_bounds__(256)
 }
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-int env_int(const char* name, int dflt);
 
 // launch geometry of one fused pass over nq queries
 struct PassPlan {
@@ -1377,13 +1376,11 @@ int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, i
   int sets = (sp.max_sets >= 2 && fits(3, kp + 8, 2)) ? 2 : 1;
   int cap = kp + (sets == 2 ? 8 : 16);
   if (!fits(2, cap, sets)) cap = kp + 8;   // d = 512 with k > 10: the resident query tile leaves room for 8 spare entries
-  const int cap_max = std::max(cap, std::min(64, env_int("DCR_SIM_CAP", 64)));
+  const int cap_max = std::max(cap, 64);
   int stages = 2;
   DCR_REQUIRE(fits(stages, cap, sets), "sim_topk: not enough shared memory (%zu B) for d=%d k=%d", max_smem, d, k);
   // priorities: 3 B stages, then list capacity up to 64 (fewer compactions), then more stages (up to 8)
   if (fits(3, cap, sets)) stages = 3;
-  const int want_stages = env_int("DCR_SIM_STAGES", 0);
-  if (want_stages > 3 && fits(want_stages, cap, sets)) stages = want_stages;
   while (cap < cap_max && fits(stages, cap + 1, sets)) ++cap;
   while (stages < 8 && fits(stages + 1, cap, sets)) ++stages;
   pp->cap = cap;
@@ -1425,8 +1422,6 @@ int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, i
   return 0;
 }
 
-int env_int(const char* name, int dflt) { return tuning_int(name, dflt); }   // honoured only under DCR_B200_TUNING=1
-
 int make_plan(int nq, int ng, int d, int k, int num_sms, size_t max_smem, SimPlan* pl) {
   DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "sim_topk: empty problem (nq=%d ng=%d d=%d)", nq, ng, d);
   DCR_REQUIRE(d <= kMaxDim, "sim_topk: descriptor dim %d > %d not supported", d, kMaxDim);
@@ -1438,12 +1433,12 @@ int make_plan(int nq, int ng, int d, int k, int num_sms, size_t max_smem, SimPla
   pl->rows_per_qtile = kBlockM;
   // Two consumer warpgroups (two warps per 32-row block, each with its own lists for one column half) when few
   // candidates are kept (k <= 2: each segment keeps 2 x 4 candidates); with larger k the lists of two sets only fit with
-  // a small capacity.  DCR_SIM_SETS=1|2 overrides.
-  pl->max_sets = std::max(1, std::min(2, env_int("DCR_SIM_SETS", k <= 2 ? 2 : 1)));
+  // a small capacity.
+  pl->max_sets = k <= 2 ? 2 : 1;
   pl->n_gtiles = (ng + kBlockN - 1) / kBlockN;
   pl->ng_pad = pl->n_gtiles * kBlockN;
-  // gallery chunks of ~DCR_SIM_CHUNK_MB of bf16 rows: the units sweep one chunk at a time so that it stays L2 resident
-  const long long chunk_bytes = static_cast<long long>(env_int("DCR_SIM_CHUNK_MB", 40)) << 20;
+  // gallery chunks of ~40 MB of bf16 rows: the units sweep one chunk at a time so that it stays L2 resident
+  const long long chunk_bytes = 40ll << 20;
   int gchunk = static_cast<int>(std::max<long long>(16, chunk_bytes / (static_cast<long long>(kBlockN) * pl->d_pad * 2)));
   int n_chunks = (pl->n_gtiles + gchunk - 1) / gchunk;
   if (n_chunks > 64) n_chunks = 64;
@@ -1454,10 +1449,7 @@ int make_plan(int nq, int ng, int d, int k, int num_sms, size_t max_smem, SimPla
   // first pass keeps few candidates per (query, segment) -- enough unless many gallery rows sit within the error
   // bound of the k-th score; such queries get a second chance with 32 candidates before the brute-force path
   // k in 6..10 keeps 12 (two spare candidates per segment keep the second-chance pass rare)
-  int kp0 = (k <= 2) ? 4 : (k <= 5 ? 8 : (k <= 10 ? 12 : 32));
-  kp0 = env_int("DCR_SIM_KP0", kp0);
-  DCR_REQUIRE(kp0 >= 1 && kp0 <= kKPMax, "sim_topk: DCR_SIM_KP0 must be in [1, 32]");
-  DCR_REQUIRE(kp0 >= k, "sim_topk: first-pass candidate count %d < k=%d", kp0, k);
+  const int kp0 = (k <= 2) ? 4 : (k <= 5 ? 8 : (k <= 10 ? 12 : 32));   // k <= kp0 <= kKPMax for every k <= 16
   pl->kp0 = kp0;
   pl->kp1 = (kp0 < kKPMax) ? kKPMax : 0;
   if (int rc = plan_pass(nq, pl->kp0, *pl, num_sms, max_smem, d, k, &pl->p0)) return rc;
@@ -1531,7 +1523,7 @@ int launch_fused(const SimPlan& pl, const PassPlan& pp, const __nv_bfloat16* qb,
   p.thr_init = thr_init;
   p.clk = clk;
   p.gthr = gthr;
-  if (gthr) DCR_CUDA_CHECK(cudaMemsetAsync(gthr, 0, static_cast<size_t>(pp.nq_pad) * 4, stream));
+  DCR_CUDA_CHECK(cudaMemsetAsync(gthr, 0, static_cast<size_t>(pp.nq_pad) * 4, stream));
   auto launch = [&](auto kern) -> int {
     DCR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pp.smem_bytes)));
     kern<<<pp.n_units, 32 + 128 * pp.n_sets, pp.smem_bytes, stream>>>(tq, tg, p);
@@ -1539,16 +1531,13 @@ int launch_fused(const SimPlan& pl, const PassPlan& pp, const __nv_bfloat16* qb,
     DCR_CUDA_CHECK(cudaGetLastError());
     return 0;
   };
-  // the variant without the offset path always runs unless the device flag says otherwise; the offset variant is only
-  // launched when query centring is possible at all (it returns immediately when the flag is 0)
+  // both variants are launched; the one that does not match the device flag (query centring on / off) returns at once
   if (pp.n_sets == 2) {
     if (int rc = launch(sim_topk_kernel<false, 2>)) return rc;
-    if (col_bias) return launch(sim_topk_kernel<true, 2>);
-  } else {
-    if (int rc = launch(sim_topk_kernel<false, 1>)) return rc;
-    if (col_bias) return launch(sim_topk_kernel<true, 1>);
+    return launch(sim_topk_kernel<true, 2>);
   }
-  return 0;
+  if (int rc = launch(sim_topk_kernel<false, 1>)) return rc;
+  return launch(sim_topk_kernel<true, 1>);
 }
 
 }  // namespace
@@ -1611,9 +1600,8 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
   auto* counts = reinterpret_cast<int*>(w + pl.off_counts);   // [0] flagged by pass 0, [1] flagged by pass 1
   auto* exact = reinterpret_cast<double*>(w + pl.off_exact);
   auto* clk = reinterpret_cast<unsigned long long*>(w + pl.off_clk);
-  unsigned int* gthr = env_int("DCR_SIM_SHARE_THR", 1) ? reinterpret_cast<unsigned int*>(w + pl.off_gthr) : nullptr;
+  auto* gthr = reinterpret_cast<unsigned int*>(w + pl.off_gthr);
 
-  const bool centre = env_int("DCR_SIM_CENTER", 1) != 0;
   DCR_CUDA_CHECK(cudaMemsetAsync(gmax, 0, 16, stream));
   DCR_CUDA_CHECK(cudaMemsetAsync(counts, 0, 16, stream));   // [0],[1] flagged counts, [2] query-centring flag
   const int conv_blocks = di->num_sms * 8;
@@ -1634,22 +1622,19 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     }
     return 0;
   };
-  if (centre) {
-    if (int rc = sampled_mean(g, ng, mu, false)) return rc;    // gallery centre mu (always used)
-    if (int rc = sampled_mean(q, nq, nu, true)) return rc;     // query centre nu + the decision whether to use it
-  }
+  if (int rc = sampled_mean(g, ng, mu, false)) return rc;    // gallery centre mu (always used)
+  if (int rc = sampled_mean(q, nq, nu, true)) return rc;     // query centre nu + the decision whether to use it
   // q' = q - nu, g' = g - mu:  q.g = q'.g' + nu.g' + q.mu  -- the tensor cores see only the centred parts, nu.g' is a
   // per-gallery-row offset added to the accumulator columns, q.mu a per-query constant that cannot change the ranking
   // d_pad <= 256: 2 loads per lane cover the row; otherwise 4 per round (512 dims = one round)
   auto convert = (pl.d_pad <= 256) ? to_bf16_rows_kernel<2> : to_bf16_rows_kernel<4>;
-  convert<<<conv_blocks, 256, 0, stream>>>(q, nq, d, pl.p0.nq_pad, pl.d_pad, centre ? nu : nullptr, qb, qnh, qnr, qnx, nullptr,
+  convert<<<conv_blocks, 256, 0, stream>>>(q, nq, d, pl.p0.nq_pad, pl.d_pad, nu, qb, qnh, qnr, qnx, nullptr,
                                            nullptr, nullptr, qflag, nullptr);
   count_launch();
-  convert<<<conv_blocks, 256, 0, stream>>>(g, ng, d, pl.ng_pad, pl.d_pad, centre ? mu : nullptr, gb, nullptr, nullptr, nullptr,
-                                           gmax, centre ? nu : nullptr, centre ? bias : nullptr, nullptr, qflag);
+  convert<<<conv_blocks, 256, 0, stream>>>(g, ng, d, pl.ng_pad, pl.d_pad, mu, gb, nullptr, nullptr, nullptr,
+                                           gmax, nu, bias, nullptr, qflag);
   count_launch();
   DCR_CUDA_CHECK(cudaGetLastError());
-  const float* col_bias = centre ? bias : nullptr;
 
   // CUDA events around the first fused pass only (thread-local, created once): bench.py's roofline numerator
   // (events belong to the device that was current when they were created: one pair per device)
@@ -1661,7 +1646,7 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     DCR_CUDA_CHECK(cudaEventCreate(&ev1));
   }
   DCR_CUDA_CHECK(cudaEventRecord(ev0, stream));
-  if (int rc = launch_fused(pl, pl.p0, qb, gb, ng, pb, col_bias, qflag, nullptr, clk, gthr, stream)) return rc;
+  if (int rc = launch_fused(pl, pl.p0, qb, gb, ng, pb, bias, qflag, nullptr, clk, gthr, stream)) return rc;
   DCR_CUDA_CHECK(cudaEventRecord(ev1, stream));
 
   auto rescore = [&](const PassPlan& pp, const int* qmap, int* flagged, int* n_flagged, float* thr_next) -> int {
@@ -1670,7 +1655,7 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     rp.n_qtiles = pp.n_qtiles, rp.n_gtiles = pl.n_gtiles, rp.gchunk = pp.gchunk, rp.n_chunks = pp.n_chunks;
     rp.n_units = pp.n_units, rp.n_sets = pp.n_sets, rp.max_cand = pp.max_cand;
     rp.cand = pb.cand, rp.cand_cnt = pb.ccnt, rp.cand_thr = pb.cthr, rp.qmap = qmap;
-    rp.mu = centre ? mu : nullptr, rp.nu = centre ? nu : nullptr, rp.nu_flag = qflag;
+    rp.mu = mu, rp.nu = nu, rp.nu_flag = qflag;
     rp.q_norm_hat = qnh, rp.q_norm_res = qnr, rp.q_norm_x = qnx, rp.g_max = gmax;
     rp.g_index_base = g_index_base, rp.g_index_stride = g_index_stride, rp.out_scores = out_scores, rp.out_idx = out_idx;
     rp.flagged = flagged, rp.n_flagged = n_flagged, rp.thr_next = thr_next;
@@ -1706,7 +1691,7 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     gather_rows_kernel<<<std::min(di->num_sms * 8, (p1.nq_pad * (pl.d_pad / 8) + 255) / 256), 256, 0, stream>>>(
         qb, flag0, n_second, p1.nq_pad, pl.d_pad, qb1);
     count_launch();
-    if (int rc = launch_fused(pl, p1, qb1, gb, ng, pb, col_bias, qflag, thr1, nullptr, gthr, stream)) return rc;
+    if (int rc = launch_fused(pl, p1, qb1, gb, ng, pb, bias, qflag, thr1, nullptr, gthr, stream)) return rc;
     if (int rc = rescore(p1, flag0, flag1, counts + 1, nullptr)) return rc;
     DCR_CUDA_CHECK(cudaMemcpyAsync(h_counts, counts, 8, cudaMemcpyDeviceToHost, stream));
     DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
