@@ -14,6 +14,9 @@ class DcrError(RuntimeError):
     pass
 
 
+ERR_CAPACITY = -3   # DCR_ERR_CAPACITY: dcr_sim_range found more candidate pairs than its max_pairs
+
+
 # name -> (restype, argtypes); mirrors include/dcr_b200.h one to one (tests check the header against this table)
 SIGNATURES = {
     "dcr_version": (C.c_int, []),
@@ -28,6 +31,10 @@ SIGNATURES = {
     "dcr_sim_topk_sharded_workspace_size": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "dcr_sim_topk_sharded": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dcr_sim_range_workspace_size": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int64]),
+    "dcr_sim_range": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int64, C.c_int64,
+                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p,
+                                C.c_size_t, C.c_void_p]),
     "dcr_sim_topk_last_stats": (C.c_int, [C.POINTER(C.c_int)]),
     "dcr_sim_topk_last_kernel_ms": (C.c_float, []),
     "dcr_sim_topk_last_sm_mhz": (C.c_float, []),

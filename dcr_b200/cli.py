@@ -65,6 +65,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--precision", default="fast", choices=["fast", "bf16x3", "parity", "exact"],
                    help="fast: bf16 tensor cores; bf16x3 / parity: 3- / 6-term split-bf16 tensor cores (fp32-level); exact: float64 accumulation")
     p.add_argument("--topk", default=10, type=int, help="matches kept per query (reference: 1 for the statistics, 10 for the galleries)")
+    p.add_argument("--sim_threshold", default=None, type=float,
+                   help="also write every pair scoring at least this much (matches.pth, and matches_wtrain.pth for the "
+                        "gallery self-join): sparse CSR in place of the reference's similarity*.pth matrices; "
+                        "--sim_threshold=-inf gives every pair.  Dot-product metric, one process")
     p.add_argument("--fid_weights", default="", type=str, help="pt_inception-2015-12-05 state_dict; enables FID")
     return p
 
@@ -132,6 +136,11 @@ def main(argv=None) -> int:
     if args.dist_url == "env://" and args.world_size == -1:                                   # :204-205
         args.world_size = int(os.environ["WORLD_SIZE"])
     args.distributed = args.world_size > 1 or args.multiprocessing_distributed               # :207
+    if args.sim_threshold is not None:
+        if args.similarity_metric == "splitloss":
+            raise NotImplementedError("--sim_threshold is implemented for --similarity_metric dotproduct")
+        if args.distributed:
+            raise NotImplementedError("--sim_threshold runs in one process (no sharded threshold search)")
     ngpus_per_node = torch.cuda.device_count()
     if args.multiprocessing_distributed:                                                     # :210-216
         args.world_size = ngpus_per_node * max(1, args.world_size)
@@ -195,7 +204,7 @@ def main_worker(gpu, ngpus_per_node, args) -> int:
         # splitloss: the reference never defines sim2 on that branch (:393-403) and stops at :412; background statistics
         # are only produced for the dot-product metric
         out = retrieval.run_retrieval(net, query_u8, values_u8, k=k, with_background=(split == 1), num_loss_chunks=split,
-                                      cross=cross)
+                                      cross=cross, threshold=args.sim_threshold)
     else:
         if split > 1:
             raise NotImplementedError("--similarity_metric splitloss runs on one GPU (the sharded path merges dot-product lists)")
@@ -223,7 +232,14 @@ def main_worker(gpu, ngpus_per_node, args) -> int:
         os.makedirs(save, exist_ok=True)
         torch.save({"values": out["values"].cpu(), "indices": out["indices"].cpu(), "query_files": q_files,
                     "gallery_files": v_files}, os.path.join(save, "topk.pth"))
-        print("Simscores @x% part done")                                                      # :470
+        # torch.sparse_csr_tensor(d["crow_indices"], d["col_indices"], d["values"], size=d["size"]) rebuilds a matrix;
+        # with --sim_threshold=-inf, .to_dense() of matches.pth is the reference's query-major similarity.pth (:414)
+        for key, name, n_rows in (("matches", "matches.pth", len(q_files)), ("bg_matches", "matches_wtrain.pth", len(v_files))):
+            if key in out:
+                offsets, idx, scores = out[key]
+                torch.save({"crow_indices": offsets.cpu(), "col_indices": idx.cpu(), "values": scores.cpu(),
+                            "size": (n_rows, len(v_files)), "threshold": args.sim_threshold}, os.path.join(save, name))
+        print("Simscores @x% part done")                                                     # :470
         print(out["stats"])
         if args.fid_weights:
             if fid_val is None:

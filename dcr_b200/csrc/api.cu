@@ -146,6 +146,20 @@ int dcr_sim_topk_sharded(const float* q, int nq, const float* g, int ng_local, i
   return dcr::topk_merge(all_s, all_i, nq, world, k, k, out_scores, reinterpret_cast<long long*>(out_idx), st);
 }
 
+size_t dcr_sim_range_workspace_size(int nq, int ng, int d, int64_t max_pairs) {
+  return dcr::sim_range_workspace_size(nq, ng, d, max_pairs);
+}
+
+int dcr_sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, int64_t g_index_base,
+                  int64_t g_index_stride, int64_t* row_offsets, int64_t* out_idx, float* out_scores, int64_t max_pairs,
+                  int64_t* counts, void* workspace, size_t workspace_bytes, void* stream) {
+  DCR_REQUIRE(q && g && row_offsets && counts && (max_pairs == 0 || (out_idx && out_scores)),
+              "dcr_sim_range: null pointer argument");
+  return dcr::sim_range(q, nq, g, ng, d, threshold, g_index_base, g_index_stride, reinterpret_cast<long long*>(row_offsets),
+                        reinterpret_cast<long long*>(out_idx), out_scores, max_pairs, reinterpret_cast<long long*>(counts),
+                        workspace, workspace_bytes, as_stream(stream));
+}
+
 int dcr_sim_topk_last_stats(int* out8) {
   DCR_REQUIRE(out8 != nullptr, "dcr_sim_topk_last_stats: null pointer");
   out8[0] = g_last_stats.cta_group;

@@ -28,6 +28,11 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
              long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
              cudaStream_t stream, SimStats* stats);
 
+size_t sim_range_workspace_size(int nq, int ng, int d, long long max_pairs);
+int sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, long long g_index_base,
+              long long g_index_stride, long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,
+              long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream);
+
 int split_rescore(const float* q, const float* g, int nq, int d, int n_chunks, int cross, const long long* cand, int n_cand,
                   int k, float* out_scores, long long* out_idx, cudaStream_t stream);
 

@@ -18,12 +18,18 @@
 //                            compute the same values.  Queries failing the certificate are recomputed by brute force in
 //                            fp64 (exact_scan_kernel / exact_select_kernel).
 // Result: indices identical to ranking all G exact dot products with ties broken by lowest index.
+//
+// The same stages 1 and 2 also serve the threshold search (sim_range: every pair scoring at least tau, exact, in CSR
+// form; it replaces the saved score matrices of diff_retrieval.py:402-403, 414-415 and the threshold of :454): the
+// fused sweep's epilogue then compares each approximate score against a per-row threshold that no qualifying pair can
+// fall below, and the candidates are re-scored with the same fp64 dot products.
 #include <cuda_bf16.h>
 
 #include <algorithm>
 #include <cmath>
 #include <type_traits>
 
+#include "../../include/dcr_b200.h"
 #include "dcr_internal.cuh"
 #include "host_util.cuh"
 #include "ptx.cuh"
@@ -41,6 +47,7 @@ constexpr int kKPMax = 32;        // max candidates kept per (query, segment)
 constexpr int kWarmTiles = 4;     // tiles replayed at the start of every segment to seed the threshold
 constexpr uint32_t kFull = 0xffffffffu;
 constexpr int kATileBytes = kBlockM * kBlockK * 2;  // 16 KB
+constexpr int kBTileBytes = kBlockN * kBlockK * 2;  // 16 KB
 constexpr int kMaxSlotsPerQuery = 512;  // (chunk, unit) segments that may cover one q-tile
 
 struct SimParams {
@@ -490,6 +497,124 @@ struct SegWalker {
   }
 };
 
+// Shared-memory pipeline of a fused sweep (sim_topk_kernel, sim_range_kernel):
+//   resident mode: [num_kb x 16 KB query tile][stages x gallery tile]; streamed mode (d_pad > 512, the query tile no
+//   longer fits): [stages x (gallery tile | 16 KB query k-block)] -- twice the L2->SMEM traffic per FLOP
+// followed by `list_bytes` of the caller's own, the barriers, and whatever the caller puts after them (`tail`).
+struct FusedPipe {
+  bool stream_a;
+  int num_kb, stage_bytes;
+  uint8_t* smem_a;     // num_kb x 16 KB (resident mode)
+  uint8_t* smem_b;     // stages x stage_bytes
+  uint8_t* lists;
+  uint64_t *b_full, *b_empty, *a_full, *a_empty;
+  uint8_t* tail;
+  DCR_DEVICE FusedPipe(uint8_t* smem_raw, int nkb, int stream, int stages, size_t list_bytes) {
+    // all tile bases 1024-byte aligned for the 128B swizzle
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    stream_a = stream != 0;
+    num_kb = nkb;
+    stage_bytes = kBlockN * kBlockK * 2 + (stream_a ? kATileBytes : 0);
+    smem_a = smem;
+    smem_b = smem_a + (stream_a ? 0 : num_kb * kATileBytes);
+    lists = smem_b + stages * stage_bytes;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(lists + list_bytes);
+    b_full = bars;          // [stages]
+    b_empty = bars + 8;     // [stages]
+    a_full = bars + 16;
+    a_empty = bars + 17;
+    tail = reinterpret_cast<uint8_t*>(bars + 32);
+  }
+  // producer warp = consumer_warps (the last warp); every thread of the CTA calls this
+  DCR_DEVICE void init(const CUtensorMap* tq, const CUtensorMap* tg, int stages, uint32_t consumer_warps) const {
+    const uint32_t warp = threadIdx.x >> 5;
+    if (warp == consumer_warps && elect_one()) {
+      tma_prefetch_desc(tq);
+      tma_prefetch_desc(tg);
+    }
+    if (warp == 0 && elect_one()) {
+      for (int s = 0; s < stages; ++s) {
+        mbar_init(&b_full[s], 1);
+        mbar_init(&b_empty[s], consumer_warps);   // one arrive per consumer warp
+      }
+      mbar_init(a_full, 1);
+      mbar_init(a_empty, consumer_warps);
+      fence_mbar_init();
+    }
+    __syncthreads();
+  }
+};
+
+// TMA producer of a fused sweep.  The whole warp walks the loop (warp-uniform values stay in uniform registers) and one
+// elected lane issues.  Per segment: the query tile (resident mode), then warm + ntiles gallery tiles of num_kb k-blocks,
+// the first `warm` of them replayed from the segment start; warm_of(walker) says how many.
+template <class WarmOf>
+DCR_DEVICE void fused_producer(const FusedPipe& pp, const CUtensorMap* tq, const CUtensorMap* tg, int stages, SegWalker& w,
+                               WarmOf warm_of) {
+  uint32_t seg = 0;
+  PipeState st(stages);
+  while (w.next()) {
+    const int qi = w.qi, g_begin = w.g_begin, ntiles = w.ntiles;
+    const int warm = warm_of(w);
+    const int q_row = qi * kBlockM;
+    if (!pp.stream_a) {   // resident query tile
+      mbar_wait(pp.a_empty, (seg & 1) ^ 1);
+      if (elect_one()) {
+        mbar_arrive_expect_tx(pp.a_full, pp.num_kb * kATileBytes);
+        for (int kb = 0; kb < pp.num_kb; ++kb)
+          tma_load_2d(pp.smem_a + kb * kATileBytes, tq, pp.a_full, kb * kBlockK, q_row, kEvictNormal);
+      }
+      __syncwarp();
+    }
+    for (int j = 0; j < warm + ntiles; ++j) {
+      const int gi = g_begin + (j < warm ? j : j - warm);
+      const int g_row = gi * kBlockN;
+      for (int kb = 0; kb < pp.num_kb; ++kb, st.next()) {
+        const uint32_t s = st.s, ph = st.ph;
+        mbar_wait(&pp.b_empty[s], ph ^ 1);
+        if (elect_one()) {
+          mbar_arrive_expect_tx(&pp.b_full[s], pp.stage_bytes);
+          tma_load_2d(pp.smem_b + s * pp.stage_bytes, tg, &pp.b_full[s], kb * kBlockK, g_row, kEvictNormal);
+          if (pp.stream_a)
+            tma_load_2d(pp.smem_b + s * pp.stage_bytes + kBTileBytes, tq, &pp.b_full[s], kb * kBlockK, q_row, kEvictNormal);
+        }
+        __syncwarp();
+      }
+    }
+    ++seg;
+  }
+}
+
+// One 128-row accumulator tile of a consumer warpgroup: the wgmma k-loop over the pipeline stages.  The stage of k-block
+// kb is released once wgmma_wait<1> in k-block kb+1 has seen its MMAs complete; `last` also releases the resident query
+// tile (last tile of the segment).  a_base / b_base: shared addresses of the query tile and of this warpgroup's columns
+// of gallery stage 0.
+template <int kCols>
+DCR_DEVICE void fused_tile_mma(WgAcc<kCols>& acc, PipeState& st, const FusedPipe& pp, uint32_t a_base, uint32_t b_base,
+                               bool last, uint32_t lane) {
+  const uint32_t a_step = pp.stream_a ? 0u : static_cast<uint32_t>(kATileBytes);   // per k-block (resident query tile)
+  uint32_t prev_s = 0;
+  for (int kb = 0; kb < pp.num_kb; ++kb, st.next()) {
+    const uint32_t s = st.s;
+    mbar_wait(&pp.b_full[s], st.ph);
+    const uint32_t a_addr = a_base + (pp.stream_a ? s * static_cast<uint32_t>(pp.stage_bytes) : static_cast<uint32_t>(kb) * a_step);
+    const uint32_t b_addr = b_base + s * static_cast<uint32_t>(pp.stage_bytes);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBlockK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), (kb | k) != 0);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (kb > 0 && lane == 0) mbar_arrive(&pp.b_empty[prev_s]);
+    prev_s = s;
+  }
+  wgmma_wait<0>();
+  acc.fence_regs();
+  if (lane == 0) {
+    mbar_arrive(&pp.b_empty[prev_s]);
+    if (!pp.stream_a && last) mbar_arrive(pp.a_empty);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // stage 2: the fused kernel.  One CTA per work unit; kSets consumer warpgroups (warps 0 .. 4 kSets - 1) each issue the
 // wgmma for their column range of every 128 x 128 tile (fp32 accumulators in registers) and filter it; the last warp is
@@ -507,43 +632,19 @@ __global__ void __launch_bounds__(32 + 128 * kSets, 1)
                     const SimParams p) {
   if (((p.bias_flag != nullptr) && (*p.bias_flag != 0)) != kBias) return;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve-up (all tile bases 1024-byte aligned for the 128B swizzle)
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr int kBTileBytes = kBlockN * kBlockK * 2;
   constexpr int kSetCols = kBlockN / kSets;
-  // resident mode: [num_kb x 16 KB query tile][stages x gallery tile]; streamed mode (d_pad > 512, the query tile no
-  // longer fits): [stages x (gallery tile | 16 KB query k-block)] -- twice the L2->SMEM traffic per FLOP
-  const bool stream_a = p.stream_a != 0;
-  const int stage_bytes = kBTileBytes + (stream_a ? kATileBytes : 0);
-  uint8_t* smem_a = smem;                                                  // num_kb x 16 KB (resident mode)
-  uint8_t* smem_b = smem_a + (stream_a ? 0 : p.num_kb * kATileBytes);      // stages x stage_bytes
-  uint2* cand = reinterpret_cast<uint2*>(smem_b + p.stages * stage_bytes);  // [kSets][cap][128]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(cand) + kSets * p.cap * 128 * 8);
-  uint64_t* b_full = bars;              // [stages]
-  uint64_t* b_empty = bars + 8;         // [stages]
-  uint64_t* a_full = bars + 16;
-  uint64_t* a_empty = bars + 17;
-  float* carry = reinterpret_cast<float*>(bars + 32);   // [kSets][4][128] thresholds carried to the next chunk, by q-tile & 3
+  // the pipeline, then [kSets][cap][128] candidate lists, barriers, carried thresholds and transpose buffers
+  const FusedPipe pp(smem_raw, p.num_kb, p.stream_a, p.stages, static_cast<size_t>(kSets) * p.cap * 128 * 8);
+  const bool stream_a = pp.stream_a;
+  uint2* cand = reinterpret_cast<uint2*>(pp.lists);   // [kSets][cap][128]
+  float* carry = reinterpret_cast<float*>(pp.tail);   // [kSets][4][128] thresholds carried to the next chunk, by q-tile & 3
   uint8_t* acc_xpose = reinterpret_cast<uint8_t*>(carry + kSets * 4 * kBlockM);   // [4 kSets warps] accumulator transposes
 
   const uint32_t warp = threadIdx.x >> 5;
   const uint32_t lane = threadIdx.x & 31;
   constexpr uint32_t kProducerWarp = 4 * kSets;
 
-  if (warp == kProducerWarp && elect_one()) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_g);
-  }
-  if (warp == 0 && elect_one()) {
-    for (int s = 0; s < p.stages; ++s) {
-      mbar_init(&b_full[s], 1);
-      mbar_init(&b_empty[s], 4 * kSets);   // one arrive per consumer warp
-    }
-    mbar_init(a_full, 1);
-    mbar_init(a_empty, 4 * kSets);
-    fence_mbar_init();
-  }
-  __syncthreads();
+  pp.init(&tmap_q, &tmap_g, p.stages, kProducerWarp);
   if (p.clk && blockIdx.x == 0 && threadIdx.x == 0) {
     p.clk[0] = clock64();
     p.clk[1] = global_timer_ns();
@@ -556,40 +657,9 @@ __global__ void __launch_bounds__(32 + 128 * kSets, 1)
 
   if (warp == kProducerWarp) {
     // ===================================== TMA producer =====================================
-    // The whole warp walks the loop (warp-uniform values stay in uniform registers) and one elected lane issues.
-    uint32_t seg = 0;
-    PipeState st(p.stages);
     SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
-    while (w.next()) {
-      const int qi = w.qi, g_begin = w.g_begin, ntiles = w.ntiles;
-      const int warm = (p.thr_init || w.carried) ? 0 : min(kWarmTiles, ntiles);
-      const int q_row = qi * rows_per_qtile;
-      if (!stream_a) {   // resident query tile
-        mbar_wait(a_empty, (seg & 1) ^ 1);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(a_full, p.num_kb * kATileBytes);
-          for (int kb = 0; kb < p.num_kb; ++kb)
-            tma_load_2d(smem_a + kb * kATileBytes, &tmap_q, a_full, kb * kBlockK, q_row, kEvictNormal);
-        }
-        __syncwarp();
-      }
-      for (int j = 0; j < warm + ntiles; ++j) {
-        const int gi = g_begin + (j < warm ? j : j - warm);
-        const int g_row = gi * kBlockN;
-        for (int kb = 0; kb < p.num_kb; ++kb, st.next()) {
-          const uint32_t s = st.s, ph = st.ph;
-          mbar_wait(&b_empty[s], ph ^ 1);
-          if (elect_one()) {
-            mbar_arrive_expect_tx(&b_full[s], stage_bytes);
-            tma_load_2d(smem_b + s * stage_bytes, &tmap_g, &b_full[s], kb * kBlockK, g_row, kEvictNormal);
-            if (stream_a)
-              tma_load_2d(smem_b + s * stage_bytes + kBTileBytes, &tmap_q, &b_full[s], kb * kBlockK, q_row, kEvictNormal);
-          }
-          __syncwarp();
-        }
-      }
-      ++seg;
-    }
+    fused_producer(pp, &tmap_q, &tmap_g, p.stages, w,
+                   [&](const SegWalker& s) { return (p.thr_init || s.carried) ? 0 : min(kWarmTiles, s.ntiles); });
   } else {
     // ===================================== consumer warpgroups =====================================
     // kSets = 2: two warps per 32-row block, each owning one column half ("set") of every tile and its own candidate
@@ -604,9 +674,8 @@ __global__ void __launch_bounds__(32 + 128 * kSets, 1)
     float* my_carry = carry + set * 4 * kBlockM;
     const int kp = p.kp, cap = p.cap;
     const float* colbias = kBias ? p.col_bias : nullptr;
-    const uint32_t a_base = smem_u32(stream_a ? smem_b + kBTileBytes : smem_a);
-    const uint32_t b_base = smem_u32(smem_b) + set * kSetCols * 128;
-    const uint32_t a_step = stream_a ? 0u : static_cast<uint32_t>(kATileBytes);   // per k-block (resident query tile)
+    const uint32_t a_base = smem_u32(stream_a ? pp.smem_b + kBTileBytes : pp.smem_a);
+    const uint32_t b_base = smem_u32(pp.smem_b) + set * kSetCols * 128;
     PipeState st(p.stages);
     uint32_t seg = 0;
     SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
@@ -628,7 +697,7 @@ __global__ void __launch_bounds__(32 + 128 * kSets, 1)
       unsigned int* gslot = qrow_s < p.nq ? p.gthr + qrow_s : nullptr;
       float published = gslot ? thr_from_key(*reinterpret_cast<volatile unsigned int*>(gslot)) : INFINITY;
       if (gslot) thr = fmaxf(thr, published);
-      if (!stream_a) mbar_wait(a_full, seg & 1);
+      if (!stream_a) mbar_wait(pp.a_full, seg & 1);
 
       // one accumulator tile: warm-up tiles only track column-slot maxima, the others feed the candidate lists.  Two
       // separate loops so that the 32 slot registers are dead while the lists are live.
@@ -639,28 +708,8 @@ __global__ void __launch_bounds__(32 + 128 * kSets, 1)
         const float* sb = kBias ? colbias + gcol0 : nullptr;   // per-column offsets: warp-uniform (broadcast) loads
         unsigned int shared_key = 0;
         if (!kWarm && gslot) shared_key = *reinterpret_cast<volatile unsigned int*>(gslot);
-        // main loop: the stage of k-block kb is released once wgmma_wait<1> in k-block kb+1 has seen its MMAs complete
         WgAcc<kSetCols> acc;
-        uint32_t prev_s = 0;
-        for (int kb = 0; kb < p.num_kb; ++kb, st.next()) {
-          const uint32_t s = st.s;
-          mbar_wait(&b_full[s], st.ph);
-          const uint32_t a_addr = a_base + (stream_a ? s * static_cast<uint32_t>(stage_bytes) : static_cast<uint32_t>(kb) * a_step);
-          const uint32_t b_addr = b_base + s * static_cast<uint32_t>(stage_bytes);
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), (kb | k) != 0);
-          wgmma_commit();
-          wgmma_wait<1>();
-          if (kb > 0 && lane == 0) mbar_arrive(&b_empty[prev_s]);
-          prev_s = s;
-        }
-        wgmma_wait<0>();
-        acc.fence_regs();
-        if (lane == 0) {
-          mbar_arrive(&b_empty[prev_s]);
-          if (!stream_a && last) mbar_arrive(a_empty);
-        }
+        fused_tile_mma(acc, st, pp, a_base, b_base, last, lane);
         if (!kWarm && gslot) {
           if (thr > published) {   // risen since the last publication (compaction): let the other units know
             atomicMax(gslot, thr_key(thr));
@@ -971,6 +1020,60 @@ DCR_DEVICE int group_scan(int v, int& total) {
   }
 }
 
+// How far an approximate score of the fused sweeps can lie from the exact one, for query row qrow.  Whole warp; q is the
+// query row (fp32 in global memory or already widened to fp64 in shared memory: the same values).
+//   eps   bounds |tensor-core score of (bf16 q', bf16 (g-mu)) (+ the column offset nu.(g-mu)) - q.(g-mu)| from the
+//         measured norms (DESIGN.md section 4): bf16 rounding of both operands, fp32 accumulation, fp32 roundings of
+//         q - nu, g - mu, the offset and its addition
+//   qmu   q . mu in fp64: the constant the centred approximate scores are offset by
+//   slack covers the fp64 rounding of an exact score and of q.mu themselves (each a d-term dot of vectors no longer than
+//         (|q'| + |nu|), (|g'| + |mu|)): irrelevant next to eps except when the centred gallery is (nearly) zero -- all
+//         rows identical -- and eps with it
+// So the fp64 score of a pair whose approximate score is a satisfies  s <= a + eps + qmu + slack  and
+// s >= a - eps + qmu - slack.
+struct RowBound {
+  float eps;
+  double qmu, slack;
+};
+template <typename TQ>
+DCR_DEVICE RowBound row_bound(const TQ* __restrict__ q, int d, int d_pad, int qrow, const float* __restrict__ q_norm_hat,
+                              const float* __restrict__ q_norm_res, const float* __restrict__ q_norm_x,
+                              const unsigned int* __restrict__ g_max, const float* __restrict__ mu,
+                              const float* __restrict__ nu, const int* __restrict__ nu_flag, uint32_t lane) {
+  const float g_norm = __uint_as_float(g_max[0]), g_res = __uint_as_float(g_max[1]);
+  const float qh = q_norm_hat[qrow], qr = q_norm_res[qrow], qx = q_norm_x[qrow];
+  float eps = 1.001f * (qh * g_res + qr * g_norm) + d_pad * 2.4e-7f * qh * (g_norm + g_res) + 1e-30f;
+  float nun = 0.f, mun = 0.f;   // |nu|, |mu| (upper bounds)
+  {
+    float acc = 0.f;
+    if (nu && nu_flag && *nu_flag)
+      for (int c = lane; c < d; c += 32) acc += nu[c] * nu[c];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
+    nun = sqrtf(acc) * 1.001f;
+    eps += 3e-7f * (qx + nun) * g_norm;
+  }
+  double qmu = 0.0;
+  {
+    float mu2 = 0.f;
+    for (int c = lane; c < d; c += 32) {
+      qmu = fma(static_cast<double>(q[c]), static_cast<double>(mu[c]), qmu);
+      mu2 = fmaf(mu[c], mu[c], mu2);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      qmu += __shfl_xor_sync(kFull, qmu, o);
+      mu2 += __shfl_xor_sync(kFull, mu2, o);
+    }
+    mun = sqrtf(mu2) * 1.001f;
+  }
+  RowBound rb;
+  rb.eps = eps;
+  rb.qmu = qmu;
+  rb.slack = 4.6e-16 * (d + 8) * static_cast<double>(qx + nun) * static_cast<double>(g_norm + mun);
+  return rb;
+}
+
 template <int kThreads>
 __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const RescoreParams p) {
   constexpr int kWarps = kThreads / 32;
@@ -1064,44 +1167,14 @@ __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const R
   for (int c = 512 + tid; c < d; c += kThreads) qs[c] = static_cast<double>(p.q[static_cast<size_t>(qrow) * d + c]);
   group_sync<kThreads>();
 
-  // eps bounds |tensor-core score of (bf16 q, bf16 (g-mu)) - q.(g-mu)| for this query from the measured norms
-  // (DESIGN.md section 4): bf16 rounding of both operands, fp32 accumulation, fp32 rounding of g - mu.  Every warp of
-  // the group computes eps, ||nu||, ||mu|| and q.mu itself.
-  const float g_norm = __uint_as_float(p.g_max[0]), g_res = __uint_as_float(p.g_max[1]);
-  const float qh = p.q_norm_hat[qrow], qr = p.q_norm_res[qrow], qx = p.q_norm_x[qrow];
-  float eps = 1.001f * (qh * g_res + qr * g_norm) + p.d_pad * 2.4e-7f * qh * (g_norm + g_res) + 1e-30f;
-  float nun = 0.f, mun = 0.f;   // |nu|, |mu| (upper bounds)
-  {
-    // ||nu||: fp32 roundings of q - nu, g - mu, the offset nu.(g - mu) and its addition
-    float acc = 0.f;
-    if (p.nu && p.nu_flag && *p.nu_flag)
-      for (int c = lane; c < d; c += 32) acc += p.nu[c] * p.nu[c];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
-    nun = sqrtf(acc) * 1.001f;
-    eps += 3e-7f * (qx + nun) * g_norm;
-  }
-  double qmu = 0.0;   // q . mu in fp64: the constant the centred approximate scores are offset by
-  {
-    float mu2 = 0.f;
-    for (int c = lane; c < d; c += 32) {
-      qmu = fma(qs[c], static_cast<double>(p.mu[c]), qmu);
-      mu2 = fmaf(p.mu[c], p.mu[c], mu2);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      qmu += __shfl_xor_sync(kFull, qmu, o);
-      mu2 += __shfl_xor_sync(kFull, mu2, o);
-    }
-    mun = sqrtf(mu2) * 1.001f;
-  }
   // certificate: every gallery row that is not a candidate has approximate centred score <= thr, hence exact score
-  // q.g <= thr + eps + q.mu.  `slack` covers the fp64 rounding of kth and q.mu themselves (each a d-term dot of vectors
-  // no longer than (|q'| + |nu|), (|g'| + |mu|)): irrelevant next to eps except when the centred gallery is (nearly)
-  // zero -- all rows identical -- and eps with it
+  // q.g <= thr + eps + q.mu + slack (row_bound)
+  const RowBound rb = row_bound(qs, d, p.d_pad, qrow, p.q_norm_hat, p.q_norm_res, p.q_norm_x, p.g_max, p.mu, p.nu,
+                                p.nu_flag, lane);
+  const float eps = rb.eps;
+  const double qmu = rb.qmu;
   const bool closed = thr > -INFINITY;   // some segment dropped rows
-  const double slack = 4.6e-16 * (d + 8) * static_cast<double>(qx + nun) * static_cast<double>(g_norm + mun);
-  const double bound = static_cast<double>(thr) + static_cast<double>(eps) + qmu + slack;
+  const double bound = static_cast<double>(thr) + static_cast<double>(eps) + qmu + rb.slack;
 
   // ---- prune by approximate score: A_k by rank counting (n is a few dozen: one pass instead of k arg-max rounds) ----
   const int kk = min(k, n);
@@ -1338,6 +1411,287 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// Threshold search (dcr_sim_range): every pair with fp32(exact score) >= tau, in CSR form.
+//   1. range_threshold_kernel  per query row the candidate threshold t_i on the approximate score: no pair whose fp32
+//                              exact score reaches tau has an approximate score below t_i (row_bound)
+//   2. sim_range_kernel<*, 0>  count sweep: candidates per (segment slot, row)
+//   3. range_slot_scan_kernel + exclusive_scan_kernel: per row, the slots' offsets in gallery order; the rows' offsets
+//   4. sim_range_kernel<*, 1>  emit sweep: the same decisions again, each row's candidates written in ascending order
+//   5. range_rescore_kernel    exact scores in pieces of kRangePiece candidates of one row, stable compaction to the
+//                              pairs that reach tau
+//   6. exclusive_scan_kernel over the pieces, range_output_kernel / range_row_offsets_kernel: the CSR arrays
+// Everything is a fixed function of the inputs (no atomics decide an order), so every call returns the same bits.
+constexpr int kRangePiece = 512;   // candidates of one row re-scored by one block
+
+struct RangeParams {
+  int nq, ng;
+  int num_kb, stream_a, n_qtiles, n_gtiles, gchunk, n_chunks, stages;   // as SimParams
+  const int* bias_flag;
+  const float* col_bias;
+  const float* thr;            // [nq] candidate threshold t_i
+  int* seg;                    // [n_slots][128] count sweep: candidates; emit sweep: offset inside the row
+  const long long* row_cand;   // [nq + 1] emit sweep: first candidate of each row
+  int* cand_idx;               // emit sweep: local gallery rows
+};
+
+// Candidate columns of one 32-column chunk of an accumulator row: bit c is set when the approximate score of column
+// col0 + c is not below t (NaN included: the exact score decides) and c < n_valid.  Columns past the gallery are cut by
+// n_valid rather than by mask_tail: at t = -inf their -inf would pass.
+template <bool kBias>
+DCR_DEVICE uint32_t range_hits(const uint32_t (&r)[32], const float* sb, float t, int n_valid) {
+  float v[32];
+#pragma unroll
+  for (int c = 0; c < 32; ++c) v[c] = __uint_as_float(r[c]);
+  if constexpr (kBias) {   // the same fp32 additions as scan_chunk
+#pragma unroll
+    for (int c = 0; c < 32; c += 4) {
+      const float4 b = *reinterpret_cast<const float4*>(sb + c);
+      v[c] += b.x; v[c + 1] += b.y; v[c + 2] += b.z; v[c + 3] += b.w;
+    }
+  }
+  uint32_t m = 0;
+#pragma unroll
+  for (int c = 0; c < 32; ++c) m |= static_cast<uint32_t>(!(v[c] < t)) << c;
+  if (n_valid < 32) m &= n_valid <= 0 ? 0u : (1u << n_valid) - 1u;
+  return m;
+}
+
+// The fused sweep of the threshold search: the work decomposition, pipeline and k-loop of sim_topk_kernel with one
+// consumer warpgroup, an epilogue that compares every accumulator column against its row's threshold, and no warm-up.
+// kEmit = 0 counts the candidates of every (segment slot, row); kEmit = 1 writes them at the offsets the scan derived
+// from those counts.  Both make the same decisions: same tiles, same wgmma sequence, same thresholds.
+template <bool kBias, bool kEmit>
+__global__ void __launch_bounds__(32 + 128, 1)
+    sim_range_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_g,
+                     const RangeParams p) {
+  if (((p.bias_flag != nullptr) && (*p.bias_flag != 0)) != kBias) return;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const FusedPipe pp(smem_raw, p.num_kb, p.stream_a, p.stages, 0);   // then barriers, then 4 transpose buffers
+  const uint32_t warp = threadIdx.x >> 5;
+  const uint32_t lane = threadIdx.x & 31;
+  pp.init(&tmap_q, &tmap_g, p.stages, 4);
+  const long long n_units = gridDim.x;
+  const long long unit = blockIdx.x;
+  SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
+  if (warp == 4) {
+    fused_producer(pp, &tmap_q, &tmap_g, p.stages, w, [](const SegWalker&) { return 0; });
+  } else {
+    const uint32_t row = warp * 32 + lane;   // query row inside the tile
+    const uint32_t xacc = smem_u32(pp.tail) + warp * kAccXposeWarpBytes;
+    const uint32_t a_base = smem_u32(pp.stream_a ? pp.smem_b + kBTileBytes : pp.smem_a);
+    const uint32_t b_base = smem_u32(pp.smem_b);
+    PipeState st(p.stages);
+    uint32_t seg = 0;
+    while (w.next()) {
+      const int qrow = w.qi * kBlockM + static_cast<int>(row);
+      const bool row_ok = qrow < p.nq;
+      const float t = row_ok ? p.thr[qrow] : INFINITY;
+      const size_t sr = static_cast<size_t>(slot_index(w.chunk, static_cast<int>(unit), w.qi, 0, static_cast<int>(n_units),
+                                                       p.n_qtiles, 1)) * kBlockM + row;
+      int cnt = 0;
+      int* out = nullptr;
+      if (kEmit && row_ok) out = p.cand_idx + p.row_cand[qrow] + p.seg[sr];
+      if (!pp.stream_a) mbar_wait(pp.a_full, seg & 1);
+#pragma unroll 1
+      for (int j = 0; j < w.ntiles; ++j) {
+        WgAcc<kBlockN> acc;
+        fused_tile_mma(acc, st, pp, a_base, b_base, j == w.ntiles - 1, lane);
+        const int gcol0 = (w.g_begin + j) * kBlockN;
+#pragma unroll
+        for (int ch = 0; ch < kBlockN / 32; ++ch) {
+          uint32_t r[32];
+          acc.rows32(ch, r, xacc, lane);
+          const int col0 = gcol0 + ch * 32;
+          const uint32_t hits = range_hits<kBias>(r, kBias ? p.col_bias + col0 : nullptr, t, row_ok ? p.ng - col0 : 0);
+          if constexpr (kEmit) {
+            for (uint32_t h = hits; h; h &= h - 1) *out++ = col0 + __ffs(h) - 1;   // ascending columns
+          } else {
+            cnt += __popc(hits);
+          }
+        }
+      }
+      ++seg;
+      if (!kEmit) p.seg[sr] = cnt;
+    }
+  }
+  __syncthreads();
+}
+
+// t_i = tau - q.mu - eps - slack - margin, rounded down at every step.  fp32(s) >= tau needs s >= tau - half an fp32 ulp
+// (margin), hence approximate score >= t_i (row_bound).  A warp per query row.
+__global__ void __launch_bounds__(128)
+    range_threshold_kernel(const float* __restrict__ q, int nq, int d, int d_pad, float tau,
+                           const float* __restrict__ q_norm_hat, const float* __restrict__ q_norm_res,
+                           const float* __restrict__ q_norm_x, const unsigned int* __restrict__ g_max,
+                           const float* __restrict__ mu, const float* __restrict__ nu, const int* __restrict__ nu_flag,
+                           float* __restrict__ thr) {
+  const int row = blockIdx.x * 4 + static_cast<int>(threadIdx.x >> 5);
+  const uint32_t lane = threadIdx.x & 31;
+  if (row >= nq) return;
+  const RowBound rb = row_bound(q + static_cast<size_t>(row) * d, d, d_pad, row, q_norm_hat, q_norm_res, q_norm_x, g_max,
+                                mu, nu, nu_flag, lane);
+  if (lane == 0) {
+    const double margin = isfinite(tau) ? fabs(static_cast<double>(tau)) * 1.2e-7 + 1e-45 : 0.0;
+    double t = __dsub_rd(static_cast<double>(tau), rb.qmu);
+    t = __dsub_rd(t, static_cast<double>(rb.eps));
+    t = __dsub_rd(t, rb.slack);
+    t = __dsub_rd(t, margin);
+    thr[row] = __double2float_rd(t);
+  }
+}
+
+// Per query row (a thread each): walk the row's segment slots in gallery order -- chunk by chunk, and inside a chunk unit
+// by unit (a unit's tiles follow the previous unit's) -- replacing each count by the row's candidates before it.
+__global__ void __launch_bounds__(256)
+    range_slot_scan_kernel(int* __restrict__ seg, int nq, int n_qtiles, int n_gtiles, int gchunk, int n_chunks,
+                           int n_units, long long* __restrict__ row_cnt, long long* __restrict__ row_pieces) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= nq) return;
+  const int qi = row / kBlockM, r = row % kBlockM;
+  int acc = 0;
+  for (int chunk = 0; chunk < n_chunks; ++chunk) {
+    const int ncg = min(gchunk, n_gtiles - chunk * gchunk);
+    const long long T = static_cast<long long>(n_qtiles) * ncg;
+    const int u_lo = static_cast<int>(owner_unit(static_cast<long long>(qi) * ncg, T, n_units));
+    const int u_hi = static_cast<int>(owner_unit(static_cast<long long>(qi + 1) * ncg - 1, T, n_units));
+    for (int u = u_lo; u <= u_hi; ++u) {
+      const size_t sr = static_cast<size_t>(slot_index(chunk, u, qi, 0, n_units, n_qtiles, 1)) * kBlockM + r;
+      const int c = seg[sr];
+      seg[sr] = acc;
+      acc += c;
+    }
+  }
+  row_cnt[row] = acc;
+  row_pieces[row] = (acc + kRangePiece - 1) / kRangePiece;
+}
+
+// out[0..n] = exclusive prefix sums of in[0..n-1] (out[n] = total), one block: thread t sums a contiguous run, the runs'
+// sums are scanned in shared memory, then each thread writes its run.  Fixed association.
+template <typename T>
+__global__ void __launch_bounds__(1024) exclusive_scan_kernel(const T* __restrict__ in, long long n, long long* __restrict__ out) {
+  __shared__ long long part[32];
+  const int tid = threadIdx.x, lane = tid & 31, wp = tid >> 5;
+  const long long per = (n + 1023) / 1024;
+  const long long lo = min(n, tid * per), hi = min(n, lo + per);
+  long long s = 0;
+  for (long long i = lo; i < hi; ++i) s += in[i];
+  long long incl = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const long long v = __shfl_up_sync(kFull, incl, o);
+    if (lane >= o) incl += v;
+  }
+  if (lane == 31) part[wp] = incl;
+  __syncthreads();
+  if (wp == 0) {
+    long long x = part[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const long long v = __shfl_up_sync(kFull, x, o);
+      if (lane >= o) x += v;
+    }
+    part[lane] = x;   // inclusive over warps
+  }
+  __syncthreads();
+  long long run = incl - s + (wp > 0 ? part[wp - 1] : 0);
+  for (long long i = lo; i < hi; ++i) {
+    out[i] = run;
+    run += in[i];
+  }
+  if (tid == 0) out[n] = part[31];
+}
+
+// piece w: row, first candidate and candidate count (row_piece[0] = 0 <= w < row_piece[nq])
+DCR_DEVICE void range_piece(long long w, const long long* __restrict__ row_cand, const long long* __restrict__ row_piece,
+                            int nq, int& row, long long& start, int& n) {
+  int lo = 0, hi = nq;   // row_piece[lo] <= w < row_piece[hi]
+  while (hi - lo > 1) {
+    const int mid = lo + (hi - lo) / 2;
+    if (row_piece[mid] <= w) lo = mid;
+    else hi = mid;
+  }
+  row = lo;
+  start = row_cand[lo] + (w - row_piece[lo]) * kRangePiece;
+  n = static_cast<int>(min(static_cast<long long>(kRangePiece), row_cand[lo + 1] - start));
+}
+
+// Exact scores of one piece (the association of exact_dot_warp: the values dcr_sim_topk reports), then a stable in-place
+// compaction of the pairs with fp32 score >= tau.  piece_kept[w] = pairs kept.
+__global__ void __launch_bounds__(kRescoreThreads)
+    range_rescore_kernel(const float* __restrict__ q, const float* __restrict__ g, int nq, int d, float tau,
+                         const long long* __restrict__ row_cand, const long long* __restrict__ row_piece,
+                         int* __restrict__ cand_idx, float* __restrict__ cand_score, int* __restrict__ piece_kept) {
+  extern __shared__ __align__(16) uint8_t sm[];
+  double* qs = reinterpret_cast<double*>(sm);   // [d] the query row, widened once
+  const int tid = threadIdx.x;
+  const uint32_t lane = threadIdx.x & 31;
+  const int warp = tid >> 5;
+  int row, n;
+  long long start;
+  range_piece(blockIdx.x, row_cand, row_piece, nq, row, start, n);
+  for (int c = tid; c < d; c += kRescoreThreads) qs[c] = static_cast<double>(q[static_cast<size_t>(row) * d + c]);
+  __syncthreads();
+  int* ci = cand_idx + start;
+  float* cs = cand_score + start;
+  for (int c = 2 * warp; c < n; c += 2 * (kRescoreThreads / 32)) {
+    double v0, v1 = 0.0;
+    if (c + 1 < n) exact_dot_warp_qd2(qs, g + static_cast<size_t>(ci[c]) * d, g + static_cast<size_t>(ci[c + 1]) * d, d, lane, v0, v1);
+    else v0 = exact_dot_warp_qd(qs, g + static_cast<size_t>(ci[c]) * d, d, lane);
+    if (lane == 0) {
+      cs[c] = static_cast<float>(v0);
+      if (c + 1 < n) cs[c + 1] = static_cast<float>(v1);
+    }
+  }
+  __syncthreads();
+  // round by round: every read of a round happens before the barrier inside group_scan, every write after it, and a
+  // round writes only below the positions later rounds read
+  int kept = 0;
+  for (int c0 = 0; c0 < n; c0 += kRescoreThreads) {
+    const int c = c0 + tid;
+    int idx = 0;
+    float s = 0.f;
+    bool keep = false;
+    if (c < n) {
+      idx = ci[c];
+      s = cs[c];
+      keep = s >= tau;   // NaN never
+    }
+    int total;
+    const int pos = kept + group_scan<kRescoreThreads>(keep ? 1 : 0, total);
+    if (keep) {
+      ci[pos] = idx;
+      cs[pos] = s;
+    }
+    kept += total;
+  }
+  if (tid == 0) piece_kept[blockIdx.x] = kept;
+}
+
+// piece w's kept pairs -> the output at piece_excl[w] (global gallery indices)
+__global__ void __launch_bounds__(256)
+    range_output_kernel(const long long* __restrict__ row_cand, const long long* __restrict__ row_piece, int nq,
+                        const long long* __restrict__ piece_excl, const int* __restrict__ cand_idx,
+                        const float* __restrict__ cand_score, long long g_index_base, long long g_index_stride,
+                        long long* __restrict__ out_idx, float* __restrict__ out_scores) {
+  int row, n;
+  long long start;
+  range_piece(blockIdx.x, row_cand, row_piece, nq, row, start, n);
+  const long long o = piece_excl[blockIdx.x];
+  const int kept = static_cast<int>(piece_excl[blockIdx.x + 1] - o);
+  for (int j = threadIdx.x; j < kept; j += blockDim.x) {
+    out_idx[o + j] = g_index_base + g_index_stride * cand_idx[start + j];
+    out_scores[o + j] = cand_score[start + j];
+  }
+}
+
+// row i starts at the output position of its first piece (rows without candidates: of the next row's first piece)
+__global__ void range_row_offsets_kernel(const long long* __restrict__ row_piece, const long long* __restrict__ piece_excl,
+                                         int nq, long long* __restrict__ row_offsets) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= nq; i += gridDim.x * blockDim.x)
+    row_offsets[i] = piece_excl[row_piece[i]];
+}
+
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 // launch geometry of one fused pass over nq queries
@@ -1422,19 +1776,12 @@ int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, i
   return 0;
 }
 
-int make_plan(int nq, int ng, int d, int k, int num_sms, size_t max_smem, SimPlan* pl) {
-  DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "sim_topk: empty problem (nq=%d ng=%d d=%d)", nq, ng, d);
-  DCR_REQUIRE(d <= kMaxDim, "sim_topk: descriptor dim %d > %d not supported", d, kMaxDim);
-  DCR_REQUIRE(k >= 1 && k <= 16, "sim_topk: k=%d outside [1,16]", k);
-  DCR_REQUIRE(k <= ng, "sim_topk: k=%d > gallery size %d", k, ng);
+// tiles, padding and gallery chunking of a fused sweep (both entry points)
+void plan_geometry(int ng, int d, SimPlan* pl) {
   pl->d_pad = static_cast<int>(align_up(d, kBlockK));
   pl->num_kb = pl->d_pad / kBlockK;
   pl->stream_a = pl->num_kb > kMaxKB ? 1 : 0;
   pl->rows_per_qtile = kBlockM;
-  // Two consumer warpgroups (two warps per 32-row block, each with its own lists for one column half) when few
-  // candidates are kept (k <= 2: each segment keeps 2 x 4 candidates); with larger k the lists of two sets only fit with
-  // a small capacity.
-  pl->max_sets = k <= 2 ? 2 : 1;
   pl->n_gtiles = (ng + kBlockN - 1) / kBlockN;
   pl->ng_pad = pl->n_gtiles * kBlockN;
   // gallery chunks of ~40 MB of bf16 rows: the units sweep one chunk at a time so that it stays L2 resident
@@ -1446,6 +1793,18 @@ int make_plan(int nq, int ng, int d, int k, int num_sms, size_t max_smem, SimPla
   n_chunks = (pl->n_gtiles + gchunk - 1) / gchunk;
   pl->gchunk = gchunk;
   pl->n_chunks = n_chunks;
+}
+
+int make_plan(int nq, int ng, int d, int k, int num_sms, size_t max_smem, SimPlan* pl) {
+  DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "sim_topk: empty problem (nq=%d ng=%d d=%d)", nq, ng, d);
+  DCR_REQUIRE(d <= kMaxDim, "sim_topk: descriptor dim %d > %d not supported", d, kMaxDim);
+  DCR_REQUIRE(k >= 1 && k <= 16, "sim_topk: k=%d outside [1,16]", k);
+  DCR_REQUIRE(k <= ng, "sim_topk: k=%d > gallery size %d", k, ng);
+  plan_geometry(ng, d, pl);
+  // Two consumer warpgroups (two warps per 32-row block, each with its own lists for one column half) when few
+  // candidates are kept (k <= 2: each segment keeps 2 x 4 candidates); with larger k the lists of two sets only fit with
+  // a small capacity.
+  pl->max_sets = k <= 2 ? 2 : 1;
   // first pass keeps few candidates per (query, segment) -- enough unless many gallery rows sit within the error
   // bound of the k-th score; such queries get a second chance with 32 candidates before the brute-force path
   // k in 6..10 keeps 12 (two spare candidates per segment keep the second-chance pass rare)
@@ -1540,6 +1899,120 @@ int launch_fused(const SimPlan& pl, const PassPlan& pp, const __nv_bfloat16* qb,
   return launch(sim_topk_kernel<true, 1>);
 }
 
+// Stage 1 of both entry points: the centres, the decision whether to centre the queries, and the bf16 operands with the
+// norms their error bound needs.
+struct Operands {
+  __nv_bfloat16 *qb, *gb;   // [nq_pad, d_pad], [ng_pad, d_pad]
+  float *qnh, *qnr, *qnx;   // per query row, see to_bf16_rows_kernel
+  unsigned int* gmax;       // [2]
+  double* colsum;           // [2 d] scratch
+  float *mu, *nu, *bias;    // gallery centre, query centre, per-gallery-row offset nu.(g - mu)
+  int* qflag;               // device flag: query centring on / off
+};
+
+int prepare_operands(const float* q, int nq, int nq_pad, const float* g, int ng, int d, const SimPlan& pl,
+                     const DeviceInfo* di, const Operands& o, cudaStream_t stream) {
+  DCR_CUDA_CHECK(cudaMemsetAsync(o.gmax, 0, 16, stream));
+  const int conv_blocks = di->num_sms * 8;
+  auto sampled_mean = [&](const float* x, int n, float* out, bool decide) -> int {
+    // any fixed vector works as a centre, so a strided sample of <= 8192 rows is enough
+    DCR_CUDA_CHECK(cudaMemsetAsync(o.colsum, 0, static_cast<size_t>(d) * 16, stream));
+    const int row_stride = std::max(1, n / 8192);
+    const int n_sample = (n + row_stride - 1) / row_stride;
+    col_sum_kernel<<<std::max(1, std::min((n_sample + 63) / 64, di->num_sms)), kColSumThreads, 0, stream>>>(
+        x, n_sample, row_stride, d, o.colsum, decide ? o.colsum + d : nullptr);
+    count_launch();
+    col_mean_finish_kernel<<<(d + 255) / 256, 256, 0, stream>>>(o.colsum, n_sample, d, out);
+    count_launch();
+    if (decide) {
+      centre_decision_kernel<<<1, 256, 0, stream>>>(o.colsum, o.colsum + d, n_sample, d, o.qflag);
+      count_launch();
+    }
+    return 0;
+  };
+  if (int rc = sampled_mean(g, ng, o.mu, false)) return rc;    // gallery centre mu (always used)
+  if (int rc = sampled_mean(q, nq, o.nu, true)) return rc;     // query centre nu + the decision whether to use it
+  // q' = q - nu, g' = g - mu:  q.g = q'.g' + nu.g' + q.mu  -- the tensor cores see only the centred parts, nu.g' is a
+  // per-gallery-row offset added to the accumulator columns, q.mu a per-query constant that cannot change the ranking
+  // d_pad <= 256: 2 loads per lane cover the row; otherwise 4 per round (512 dims = one round)
+  auto convert = (pl.d_pad <= 256) ? to_bf16_rows_kernel<2> : to_bf16_rows_kernel<4>;
+  convert<<<conv_blocks, 256, 0, stream>>>(q, nq, d, nq_pad, pl.d_pad, o.nu, o.qb, o.qnh, o.qnr, o.qnx, nullptr,
+                                           nullptr, nullptr, o.qflag, nullptr);
+  count_launch();
+  convert<<<conv_blocks, 256, 0, stream>>>(g, ng, d, pl.ng_pad, pl.d_pad, o.mu, o.gb, nullptr, nullptr, nullptr,
+                                           o.gmax, o.nu, o.bias, nullptr, o.qflag);
+  count_launch();
+  DCR_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+constexpr long long kMaxRangePairs = 1ll << 40;   // capacity accepted by the planner (keeps the byte counts in range)
+
+struct RangePlan {
+  SimPlan geo;   // plan_geometry fields only
+  int nq_pad, n_qtiles, n_units, n_slots, stages;
+  size_t smem_bytes;
+  long long max_pieces;   // pieces of kRangePiece candidates when max_pairs candidates fill the rows worst
+  size_t off_qb, off_gb, off_qnh, off_qnr, off_qnx, off_gmax, off_colsum, off_mu, off_nu, off_bias, off_flag, off_thr,
+      off_seg, off_row_cnt, off_row_cand, off_row_pcnt, off_row_piece, off_cand_idx, off_cand_score, off_piece_kept,
+      off_piece_excl;
+  size_t total;
+};
+
+int make_range_plan(int nq, int ng, int d, long long max_pairs, int num_sms, size_t max_smem, RangePlan* rp) {
+  DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "sim_range: empty problem (nq=%d ng=%d d=%d)", nq, ng, d);
+  DCR_REQUIRE(d <= kMaxDim, "sim_range: descriptor dim %d > %d not supported", d, kMaxDim);
+  DCR_REQUIRE(d % 4 == 0, "sim_range: descriptor dim %d is not a multiple of 4", d);
+  DCR_REQUIRE(max_pairs >= 0 && max_pairs <= kMaxRangePairs, "sim_range: max_pairs=%lld outside [0, 2^40]", max_pairs);
+  plan_geometry(ng, d, &rp->geo);
+  const SimPlan& g = rp->geo;
+  rp->n_qtiles = (nq + kBlockM - 1) / kBlockM;
+  rp->nq_pad = rp->n_qtiles * kBlockM;
+  // shared memory: resident query tile + stages x gallery stage + barriers + the transpose buffers of 4 warps
+  const size_t a_bytes = g.stream_a ? 0 : static_cast<size_t>(g.num_kb) * kATileBytes;
+  const size_t b_tile = static_cast<size_t>(kBTileBytes) + (g.stream_a ? kATileBytes : 0);
+  const size_t fixed = 1024 /*align slack*/ + 256 /*barriers*/ + 4 * kAccXposeWarpBytes;
+  int stages = 2;
+  DCR_REQUIRE(max_smem >= fixed + a_bytes + stages * b_tile, "sim_range: not enough shared memory (%zu B) for d=%d", max_smem, d);
+  while (stages < 8 && max_smem >= fixed + a_bytes + (stages + 1) * b_tile) ++stages;
+  rp->stages = stages;
+  rp->smem_bytes = fixed + a_bytes + stages * b_tile;
+  // every unit owns at least one tile of every chunk (the last chunk is the smallest): every slot the scan walks is written
+  const int last = g.n_gtiles - (g.n_chunks - 1) * g.gchunk;
+  rp->n_units = static_cast<int>(std::min<long long>(num_sms, static_cast<long long>(rp->n_qtiles) * last));
+  rp->n_slots = g.n_chunks * (rp->n_units + rp->n_qtiles);
+  rp->max_pieces = max_pairs / kRangePiece + nq;
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    size_t o = off;
+    off = align_up(off + bytes, 256);
+    return o;
+  };
+  rp->off_qb = take(static_cast<size_t>(rp->nq_pad) * g.d_pad * 2);
+  rp->off_gb = take(static_cast<size_t>(g.ng_pad) * g.d_pad * 2);
+  rp->off_qnh = take(static_cast<size_t>(rp->nq_pad) * 4);
+  rp->off_qnr = take(static_cast<size_t>(rp->nq_pad) * 4);
+  rp->off_qnx = take(static_cast<size_t>(rp->nq_pad) * 4);
+  rp->off_gmax = take(16);
+  rp->off_colsum = take(static_cast<size_t>(d) * 16);
+  rp->off_mu = take(static_cast<size_t>(d) * 4);
+  rp->off_nu = take(static_cast<size_t>(d) * 4);
+  rp->off_bias = take(static_cast<size_t>(g.ng_pad) * 4);
+  rp->off_flag = take(16);
+  rp->off_thr = take(static_cast<size_t>(nq) * 4);
+  rp->off_seg = take(static_cast<size_t>(rp->n_slots) * kBlockM * 4);
+  rp->off_row_cnt = take(static_cast<size_t>(nq) * 8);
+  rp->off_row_cand = take((static_cast<size_t>(nq) + 1) * 8);
+  rp->off_row_pcnt = take(static_cast<size_t>(nq) * 8);
+  rp->off_row_piece = take((static_cast<size_t>(nq) + 1) * 8);
+  rp->off_cand_idx = take(static_cast<size_t>(max_pairs) * 4);
+  rp->off_cand_score = take(static_cast<size_t>(max_pairs) * 4);
+  rp->off_piece_kept = take(static_cast<size_t>(rp->max_pieces) * 4);
+  rp->off_piece_excl = take((static_cast<size_t>(rp->max_pieces) + 1) * 8);
+  rp->total = off;
+  return 0;
+}
+
 }  // namespace
 
 int split_rescore(const float* q, const float* g, int nq, int d, int n_chunks, int cross, const long long* cand, int n_cand,
@@ -1602,39 +2075,10 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
   auto* clk = reinterpret_cast<unsigned long long*>(w + pl.off_clk);
   auto* gthr = reinterpret_cast<unsigned int*>(w + pl.off_gthr);
 
-  DCR_CUDA_CHECK(cudaMemsetAsync(gmax, 0, 16, stream));
   DCR_CUDA_CHECK(cudaMemsetAsync(counts, 0, 16, stream));   // [0],[1] flagged counts, [2] query-centring flag
-  const int conv_blocks = di->num_sms * 8;
   int* qflag = counts + 2;   // device flag: query centring on/off
-  auto sampled_mean = [&](const float* x, int n, float* out, bool decide) -> int {
-    // any fixed vector works as a centre, so a strided sample of <= 8192 rows is enough
-    DCR_CUDA_CHECK(cudaMemsetAsync(colsum, 0, static_cast<size_t>(d) * 16, stream));
-    const int row_stride = std::max(1, n / 8192);
-    const int n_sample = (n + row_stride - 1) / row_stride;
-    col_sum_kernel<<<std::max(1, std::min((n_sample + 63) / 64, di->num_sms)), kColSumThreads, 0, stream>>>(
-        x, n_sample, row_stride, d, colsum, decide ? colsum + d : nullptr);
-    count_launch();
-    col_mean_finish_kernel<<<(d + 255) / 256, 256, 0, stream>>>(colsum, n_sample, d, out);
-    count_launch();
-    if (decide) {
-      centre_decision_kernel<<<1, 256, 0, stream>>>(colsum, colsum + d, n_sample, d, qflag);
-      count_launch();
-    }
-    return 0;
-  };
-  if (int rc = sampled_mean(g, ng, mu, false)) return rc;    // gallery centre mu (always used)
-  if (int rc = sampled_mean(q, nq, nu, true)) return rc;     // query centre nu + the decision whether to use it
-  // q' = q - nu, g' = g - mu:  q.g = q'.g' + nu.g' + q.mu  -- the tensor cores see only the centred parts, nu.g' is a
-  // per-gallery-row offset added to the accumulator columns, q.mu a per-query constant that cannot change the ranking
-  // d_pad <= 256: 2 loads per lane cover the row; otherwise 4 per round (512 dims = one round)
-  auto convert = (pl.d_pad <= 256) ? to_bf16_rows_kernel<2> : to_bf16_rows_kernel<4>;
-  convert<<<conv_blocks, 256, 0, stream>>>(q, nq, d, pl.p0.nq_pad, pl.d_pad, nu, qb, qnh, qnr, qnx, nullptr,
-                                           nullptr, nullptr, qflag, nullptr);
-  count_launch();
-  convert<<<conv_blocks, 256, 0, stream>>>(g, ng, d, pl.ng_pad, pl.d_pad, mu, gb, nullptr, nullptr, nullptr,
-                                           gmax, nu, bias, nullptr, qflag);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
+  const Operands ops = {qb, gb, qnh, qnr, qnx, gmax, colsum, mu, nu, bias, qflag};
+  if (int rc = prepare_operands(q, nq, pl.p0.nq_pad, g, ng, d, pl, di, ops, stream)) return rc;
 
   // CUDA events around the first fused pass only (thread-local, created once): bench.py's roofline numerator
   // (events belong to the device that was current when they were created: one pair per device)
@@ -1736,6 +2180,131 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     stats->n_second = n_second;
     stats->d_pad = pl.d_pad;
   }
+  return 0;
+}
+
+size_t sim_range_workspace_size(int nq, int ng, int d, long long max_pairs) {
+  const DeviceInfo* di = device_info();
+  RangePlan rp;
+  if (make_range_plan(nq, ng, d, max_pairs, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &rp) != 0) return 0;
+  return rp.total;
+}
+
+int sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, long long g_index_base,
+              long long g_index_stride, long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,
+              long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  const DeviceInfo* di = device_info();
+  if (!di) return -2;
+  DCR_REQUIRE(di->cc_major == 9 && di->cc_minor == 0, "sim_range: this build targets sm_90a; device reports sm_%d%d", di->cc_major,
+              di->cc_minor);
+  DCR_REQUIRE(!std::isnan(threshold), "sim_range: threshold is NaN");
+  DCR_REQUIRE(g_index_stride >= 1, "sim_range: g_index_stride=%lld < 1", g_index_stride);
+  RangePlan rp;
+  if (int rc = make_range_plan(nq, ng, d, max_pairs, di->num_sms, di->max_smem_optin, &rp)) return rc;
+  DCR_REQUIRE(ws != nullptr && ws_bytes >= rp.total, "sim_range: workspace too small (%zu < %zu)", ws_bytes, rp.total);
+  DCR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "sim_range: workspace must be 256-byte aligned");
+  DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0,
+              "sim_range: q/g must be 16-byte aligned");
+  const SimPlan& geo = rp.geo;
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  auto* qb = reinterpret_cast<__nv_bfloat16*>(w + rp.off_qb);
+  auto* gb = reinterpret_cast<__nv_bfloat16*>(w + rp.off_gb);
+  auto* qnh = reinterpret_cast<float*>(w + rp.off_qnh);
+  auto* qnr = reinterpret_cast<float*>(w + rp.off_qnr);
+  auto* qnx = reinterpret_cast<float*>(w + rp.off_qnx);
+  auto* gmax = reinterpret_cast<unsigned int*>(w + rp.off_gmax);
+  auto* mu = reinterpret_cast<float*>(w + rp.off_mu);
+  auto* nu = reinterpret_cast<float*>(w + rp.off_nu);
+  auto* bias = reinterpret_cast<float*>(w + rp.off_bias);
+  auto* qflag = reinterpret_cast<int*>(w + rp.off_flag);
+  auto* thr = reinterpret_cast<float*>(w + rp.off_thr);
+  auto* seg = reinterpret_cast<int*>(w + rp.off_seg);
+  auto* row_cnt = reinterpret_cast<long long*>(w + rp.off_row_cnt);
+  auto* row_cand = reinterpret_cast<long long*>(w + rp.off_row_cand);
+  auto* row_pcnt = reinterpret_cast<long long*>(w + rp.off_row_pcnt);
+  auto* row_piece = reinterpret_cast<long long*>(w + rp.off_row_piece);
+  auto* cand_idx = reinterpret_cast<int*>(w + rp.off_cand_idx);
+  auto* cand_score = reinterpret_cast<float*>(w + rp.off_cand_score);
+  auto* piece_kept = reinterpret_cast<int*>(w + rp.off_piece_kept);
+  auto* piece_excl = reinterpret_cast<long long*>(w + rp.off_piece_excl);
+
+  const Operands ops = {qb, gb, qnh, qnr, qnx, gmax, reinterpret_cast<double*>(w + rp.off_colsum), mu, nu, bias, qflag};
+  if (int rc = prepare_operands(q, nq, rp.nq_pad, g, ng, d, geo, di, ops, stream)) return rc;
+  range_threshold_kernel<<<(nq + 3) / 4, 128, 0, stream>>>(q, nq, d, geo.d_pad, threshold, qnh, qnr, qnx, gmax, mu, nu,
+                                                           qflag, thr);
+  count_launch();
+
+  CUtensorMap tq, tg;
+  if (int rc = make_tmap_2d_bf16(&tq, qb, rp.nq_pad, geo.d_pad, geo.d_pad, kBlockM, kBlockK)) return rc;
+  if (int rc = make_tmap_2d_bf16(&tg, gb, geo.ng_pad, geo.d_pad, geo.d_pad, kBlockN, kBlockK)) return rc;
+  RangeParams p;
+  p.nq = nq;
+  p.ng = ng;
+  p.num_kb = geo.num_kb;
+  p.stream_a = geo.stream_a;
+  p.n_qtiles = rp.n_qtiles;
+  p.n_gtiles = geo.n_gtiles;
+  p.gchunk = geo.gchunk;
+  p.n_chunks = geo.n_chunks;
+  p.stages = rp.stages;
+  p.bias_flag = qflag;
+  p.col_bias = bias;
+  p.thr = thr;
+  p.seg = seg;
+  p.row_cand = row_cand;
+  p.cand_idx = cand_idx;
+  auto launch = [&](auto kern) -> int {
+    DCR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(rp.smem_bytes)));
+    kern<<<rp.n_units, 32 + 128, rp.smem_bytes, stream>>>(tq, tg, p);
+    count_launch();
+    DCR_CUDA_CHECK(cudaGetLastError());
+    return 0;
+  };
+  // both centring variants are launched; the one that does not match the device flag returns at once
+  if (int rc = launch(sim_range_kernel<false, false>)) return rc;
+  if (int rc = launch(sim_range_kernel<true, false>)) return rc;
+  range_slot_scan_kernel<<<(nq + 255) / 256, 256, 0, stream>>>(seg, nq, rp.n_qtiles, geo.n_gtiles, geo.gchunk,
+                                                                geo.n_chunks, rp.n_units, row_cnt, row_pcnt);
+  count_launch();
+  exclusive_scan_kernel<long long><<<1, 1024, 0, stream>>>(row_cnt, nq, row_cand);
+  count_launch();
+  exclusive_scan_kernel<long long><<<1, 1024, 0, stream>>>(row_pcnt, nq, row_piece);
+  count_launch();
+  long long h_tot[2] = {0, 0};   // candidates, pieces
+  DCR_CUDA_CHECK(cudaMemcpyAsync(h_tot, row_cand + nq, 8, cudaMemcpyDeviceToHost, stream));
+  DCR_CUDA_CHECK(cudaMemcpyAsync(h_tot + 1, row_piece + nq, 8, cudaMemcpyDeviceToHost, stream));
+  DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
+  const long long n_cand = h_tot[0], n_pieces = h_tot[1];
+  counts[0] = 0;
+  counts[1] = n_cand;
+  if (n_cand > max_pairs)
+    return set_error(DCR_ERR_CAPACITY, "sim_range: %lld candidate pairs exceed max_pairs=%lld (call again with that capacity)",
+                     n_cand, max_pairs);
+
+  if (n_pieces > 0) {
+    if (int rc = launch(sim_range_kernel<false, true>)) return rc;
+    if (int rc = launch(sim_range_kernel<true, true>)) return rc;
+    const size_t smem = static_cast<size_t>(d) * 8;
+    DCR_CUDA_CHECK(cudaFuncSetAttribute(range_rescore_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    range_rescore_kernel<<<static_cast<unsigned>(n_pieces), kRescoreThreads, smem, stream>>>(
+        q, g, nq, d, threshold, row_cand, row_piece, cand_idx, cand_score, piece_kept);
+    count_launch();
+  }
+  exclusive_scan_kernel<int><<<1, 1024, 0, stream>>>(piece_kept, n_pieces, piece_excl);
+  count_launch();
+  if (n_pieces > 0) {
+    range_output_kernel<<<static_cast<unsigned>(n_pieces), 256, 0, stream>>>(row_cand, row_piece, nq, piece_excl, cand_idx,
+                                                                             cand_score, g_index_base, g_index_stride,
+                                                                             out_idx, out_scores);
+    count_launch();
+  }
+  range_row_offsets_kernel<<<grid_for(nq + 1, 256, di->num_sms), 256, 0, stream>>>(row_piece, piece_excl, nq, row_offsets);
+  count_launch();
+  DCR_CUDA_CHECK(cudaGetLastError());
+  long long h_pairs = 0;
+  DCR_CUDA_CHECK(cudaMemcpyAsync(&h_pairs, piece_excl + n_pieces, 8, cudaMemcpyDeviceToHost, stream));
+  DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
+  counts[0] = h_pairs;
   return 0;
 }
 

@@ -19,7 +19,7 @@ import torch
 
 from . import _lib
 from .nets import DcrNet
-from .similarity import l2_normalize_, sim_topk, sim_topk_split
+from .similarity import l2_normalize_, sim_range, sim_topk, sim_topk_split
 
 
 @torch.no_grad()
@@ -144,9 +144,14 @@ def retrieval_stats(main_v: torch.Tensor, bg_v: Optional[torch.Tensor] = None) -
 
 def run_retrieval(net: DcrNet, query_images: torch.Tensor, gallery_images: torch.Tensor, k: int = 1,
                   with_background: bool = False, batch_size: Optional[int] = None,
-                  num_loss_chunks: int = 1, cross: bool = False) -> Dict[str, object]:
-    """Embed both image sets and match them (the rank-0 block of diff_retrieval.py:386-419)."""
-    if isinstance(net, (list, tuple)):                                        # multiscale=args.multiscale (:386-387)
+                  num_loss_chunks: int = 1, cross: bool = False, threshold: Optional[float] = None) -> Dict[str, object]:
+    """Embed both image sets and match them (the rank-0 block of diff_retrieval.py:386-419).  With a threshold, also
+    every pair scoring at least that much (sim_range, CSR): out["matches"] (query x gallery, the entries of the
+    reference's similarity.pth, :402, :414) and, with the background, out["bg_matches"] (the gallery self-join, diagonal
+    included, as similarity_wtrain.pth, :403, :415).  Dot-product metric only."""
+    if threshold is not None and num_loss_chunks > 1:
+        raise NotImplementedError("a similarity threshold is implemented for the dot-product metric only")
+    if isinstance(net, (list, tuple)):                                      # multiscale=args.multiscale (:386-387)
         values_features = extract_features_multiscale(net, gallery_images, batch_size)
         query_features = extract_features_multiscale(net, query_images, batch_size)
     else:
@@ -165,5 +170,9 @@ def run_retrieval(net: DcrNet, query_images: torch.Tensor, gallery_images: torch
         bg, _ = sim_topk(values_features, values_features, 2)                 # :403, :418
         bg_v = bg[:, -1]                                                      # :419
         out["bg_values"] = bg_v
+    if threshold is not None:
+        out["matches"] = sim_range(query_features, values_features, threshold)
+        if with_background:
+            out["bg_matches"] = sim_range(values_features, values_features, threshold)
     out["stats"] = retrieval_stats(main_v[:, 0], bg_v)
     return out

@@ -117,6 +117,31 @@ int dcr_sim_topk_sharded(const float* q, int nq, const float* g, int ng_local, i
 int dcr_split_rescore(const float* q, const float* g, int nq, int d, int n_chunks, int cross, const int64_t* cand,
                       int n_cand, int k, float* out_scores, int64_t* out_idx, void* stream);
 
+/* ---- threshold search ----------------------------------------------------------------------------------------- */
+#define DCR_ERR_CAPACITY (-3) /* more result candidates than the caller's max_pairs; counts[1] says how many */
+
+/* Bytes of device workspace dcr_sim_range needs (host-only planning; 0 on invalid arguments, see last error).  It grows
+ * with nq, ng, d and max_pairs, never with nq * ng. */
+size_t dcr_sim_range_workspace_size(int nq, int ng, int d, int64_t max_pairs);
+
+/* For every query row i, every gallery row j whose score s_ij >= threshold.  s_ij is the score dcr_sim_topk reports for
+ * the same pair, bit for bit: the fp64 sum of the fp32 products (the association of its exact re-score) rounded to
+ * fp32.  A NaN score is never reported; threshold = -inf reports all nq * ng pairs; a NaN threshold is an error.
+ * The answer is exact (no qualifying pair is missed, no other pair reported) and the same bits on every call.
+ * q[nq,d], g[ng,d]: as dcr_sim_topk (device, fp32, 16-byte aligned, d % 4 == 0, d <= 8192).  Output, CSR (device):
+ *   row_offsets[nq + 1]  int64, row i's pairs are entries row_offsets[i] .. row_offsets[i + 1] - 1
+ *   out_idx[max_pairs]   int64, g_index_base + g_index_stride * j, ascending j within a row (g_index_stride >= 1)
+ *   out_scores[max_pairs] fp32
+ * counts (HOST [2]): [0] pairs returned, [1] candidate pairs examined = the capacity this call needs.  When the
+ * candidates exceed max_pairs the call returns DCR_ERR_CAPACITY after the counting pass, with counts[1] set and the
+ * outputs undefined; the same call with max_pairs = counts[1] then succeeds.  Synchronises `stream` before returning.
+ * Replaces   sim = torch.mm(values, query.T); sim2 = mm(values, values.T)    diff_retrieval.py:402-403
+ *            torch.save(sim / sim2, 'similarity*.pth')                       diff_retrieval.py:414-415
+ *            the fraction of scores above 0.5 (sim_gt_05pc)                  diff_retrieval.py:454 */
+int dcr_sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, int64_t g_index_base,
+                  int64_t g_index_stride, int64_t* row_offsets, int64_t* out_idx, float* out_scores, int64_t max_pairs,
+                  int64_t* counts, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- dense contraction of the descriptor networks ------------------------------------------------------------- */
 /* y = act(scale[n] * conv2d(x, w)[.., n] + bias[n] (+ residual)) as a wgmma implicit GEMM.
  *   x        NHWC bf16, `x_planes` planes of B*H*W*C elements each (plane p at x + p*x_plane_stride elements);
