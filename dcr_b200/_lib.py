@@ -14,7 +14,7 @@ class DcrError(RuntimeError):
     pass
 
 
-ERR_CAPACITY = -3   # DCR_ERR_CAPACITY: dcr_sim_range found more candidate pairs than its max_pairs
+ERR_CAPACITY = -3   # DCR_ERR_CAPACITY: dcr_sim_range(_sharded) found more candidate pairs than its capacities
 
 
 # name -> (restype, argtypes); mirrors include/dcr_b200.h one to one (tests check the header against this table)
@@ -35,6 +35,11 @@ SIGNATURES = {
     "dcr_sim_range": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int64, C.c_int64,
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p,
                                 C.c_size_t, C.c_void_p]),
+    "dcr_sim_range_sharded_workspace_size": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64]),
+    "dcr_sim_range_sharded": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int64,
+                                        C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_int64, C.c_int64, C.POINTER(C.c_int64), C.c_void_p, C.c_size_t,
+                                        C.c_void_p]),
     "dcr_sim_topk_last_stats": (C.c_int, [C.POINTER(C.c_int)]),
     "dcr_sim_topk_last_kernel_ms": (C.c_float, []),
     "dcr_sim_topk_last_sm_mhz": (C.c_float, []),
@@ -71,7 +76,7 @@ SIGNATURES = {
                                  C.c_void_p]),
 }
 
-# the all-gather callback of dcr_sim_topk_sharded: int (*)(const void* send, void* recv, size_t bytes_per_rank, void* ctx, void* stream)
+# the all-gather callback of dcr_sim_topk_sharded / dcr_sim_range_sharded: int (*)(const void* send, void* recv, size_t bytes_per_rank, void* ctx, void* stream)
 ALLGATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p)
 
 _lib = None

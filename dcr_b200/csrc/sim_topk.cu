@@ -2308,4 +2308,11 @@ int sim_range(const float* q, int nq, const float* g, int ng, int d, float thres
   return 0;
 }
 
+int exclusive_scan_i64(const long long* in, long long n, long long* out, cudaStream_t stream) {
+  exclusive_scan_kernel<long long><<<1, 1024, 0, stream>>>(in, n, out);
+  count_launch();
+  DCR_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace dcr

@@ -15,6 +15,10 @@ and one all-gather of the [Q,k] (score, index) pairs + a merge gives every rank 
 There is no data-path collective inside the kernels: the exchange is two small all-gathers per run (message sizes
 are KBs..MBs, latency bound), so NCCL is the right tool.  The functions take the local scorer / merger as arguments
 so the sharding logic is testable on CPU with the oracle under the gloo backend (tests/test_dist_cpu.py).
+
+The threshold search has the same shape (`sharded_range`, C entry `dcr_sim_range_sharded`): each rank searches all
+queries against its shard, a fixed-size header per rank is all-gathered first so that every rank reaches the same
+outcome, then the CSR pieces, padded to the largest, and a device merge places them into the CSR of the whole gallery.
 """
 from __future__ import annotations
 
@@ -121,26 +125,7 @@ def sharded_topk_c(query_all: torch.Tensor, gallery_local: torch.Tensor, k: int,
         world = dist.get_world_size() if dist.is_initialized() else 1
     nq, d = q.shape
     ng = g.shape[0]
-    holders = []
-
-    def default_allgather(send, recv, nbytes, stream):
-        # zero-copy uint8 views of the library's device buffers
-        sv = device_bytes(send, nbytes, q.device)
-        rv = device_bytes(recv, nbytes * world, q.device)
-        holders.extend([sv, rv])
-        dist.all_gather_into_tensor(rv, sv)
-        return 0
-
-    fn = allgather or default_allgather
-
-    def trampoline(send, recv, nbytes, ctx, stream):
-        try:
-            return int(fn(send, recv, nbytes, stream))
-        except Exception as e:                      # never unwind through the C frame
-            print(f"dcr_b200.dist.sharded_topk_c: all-gather callback raised {e!r}")
-            return 1
-
-    cb = _lib.ALLGATHER_FN(trampoline)
+    cb = _allgather_callback(allgather, world, q.device, "sharded_topk_c")
     with torch.cuda.device(q.device):
         nbytes = lib.dcr_sim_topk_sharded_workspace_size(nq, ng, d, k, world)
         if nbytes == 0:
@@ -154,6 +139,89 @@ def sharded_topk_c(query_all: torch.Tensor, gallery_local: torch.Tensor, k: int,
         _lib.check(rc, "dcr_sim_topk_sharded")
         torch.cuda.current_stream().synchronize()    # the workspace and the views above die with this frame
     return out_s, out_i
+
+
+def _allgather_callback(allgather: Optional[Callable], world: int, device: torch.device, what: str):
+    """The C callback (_lib.ALLGATHER_FN) the sharded entries call: `allgather(send_ptr, recv_ptr, bytes_per_rank,
+    stream_ptr) -> int`, by default torch.distributed.all_gather_into_tensor over zero-copy uint8 views of the library's
+    device buffers.  An exception becomes a non-zero return: it never unwinds through the C frame.  Keep the returned
+    object alive for the duration of the call."""
+    holders = []
+
+    def default_allgather(send, recv, nbytes, stream):
+        sv = device_bytes(send, nbytes, device)
+        rv = device_bytes(recv, nbytes * world, device)
+        holders.extend([sv, rv])
+        dist.all_gather_into_tensor(rv, sv)
+        return 0
+
+    fn = allgather or default_allgather
+
+    def trampoline(send, recv, nbytes, ctx, stream):
+        try:
+            return int(fn(send, recv, nbytes, stream))
+        except Exception as e:                      # never unwind through the C frame
+            print(f"dcr_b200.dist.{what}: all-gather callback raised {e!r}")
+            return 1
+
+    from . import _lib
+    return _lib.ALLGATHER_FN(trampoline)
+
+
+def sharded_range(query_all: torch.Tensor, gallery_local: torch.Tensor, threshold: float, gallery_base: int, *,
+                  allgather: Optional[Callable] = None, world: Optional[int] = None, index_stride: int = 1
+                  ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Threshold search over a gallery sharded across ranks, through the C entry `dcr_sim_range_sharded`
+    (include/dcr_b200.h): every rank searches ALL queries against its shard (global index of local row j =
+    gallery_base + index_stride * j), the CSR pieces are exchanged and merged on the device, and every rank returns
+    (offsets i64[Q+1], indices i64[P], scores f32[P]) -- bit for bit what similarity.sim_range returns for the union of
+    the shards.  `query_all`: every query descriptor (a query-sharded caller all-gathers them first with
+    all_gather_rows).  `gallery_local` may have 0 rows; that rank still takes part in the exchanges.  `allgather` as in
+    sharded_topk_c (default: torch.distributed.all_gather_into_tensor).  The capacities start where sim_range's do; when
+    some rank needs more, every rank gets DCR_ERR_CAPACITY with the needs and retries once, together."""
+    import ctypes as C
+    from . import _lib
+    from .similarity import _aligned_ptr, _check_cuda_f32
+    lib = _lib.load()
+    q = _check_cuda_f32("query_all", query_all)
+    g = _check_cuda_f32("gallery_local", gallery_local)
+    if world is None:
+        world = dist.get_world_size() if dist.is_initialized() else 1
+    nq, d = q.shape
+    ng = g.shape[0]
+    # a gallery of another dim or device is this rank's failure: it goes to the library as a missing gallery, so that
+    # every rank returns the error instead of this one leaving its peers in the exchange
+    g_ok = g.shape[1] == d and g.device == q.device
+    g_ptr = (g.data_ptr() if ng > 0 else None) if g_ok else None
+    cb = _allgather_callback(allgather, world, q.device, "sharded_range")
+    counts = (C.c_int64 * 3)()
+    local_cap = out_cap = max(1 << 20, 16 * nq)   # sim_range's start; the exact needs come back with ERR_CAPACITY
+    with torch.cuda.device(q.device):
+        offsets = torch.empty(nq + 1, dtype=torch.int64, device=q.device)
+        for attempt in range(2):
+            # 0 (invalid arguments) is passed on: the library reports the reason on every rank
+            nbytes = lib.dcr_sim_range_sharded_workspace_size(nq, ng if g_ok else 1, d, world, local_cap)
+            ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=q.device) if nbytes else None
+            out_i = torch.empty(out_cap, dtype=torch.int64, device=q.device)
+            out_s = torch.empty(out_cap, dtype=torch.float32, device=q.device)
+            st = torch.cuda.current_stream().cuda_stream
+            rc = lib.dcr_sim_range_sharded(q.data_ptr(), nq, g_ptr, ng if g_ok else 1, d, float(threshold),
+                                           gallery_base, index_stride, world, C.cast(cb, C.c_void_p), None,
+                                           offsets.data_ptr(), out_i.data_ptr() or None, out_s.data_ptr() or None,
+                                           out_cap, local_cap, counts, _aligned_ptr(ws) if ws is not None else None,
+                                           nbytes, st)
+            if rc == _lib.ERR_CAPACITY and attempt == 0:
+                local_cap, out_cap = int(counts[1]), int(counts[2])   # agreed by every rank: all retry together
+                continue
+            if rc != 0 and not g_ok:
+                raise _lib.DcrError(f"dcr_sim_range_sharded: gallery_local {tuple(g.shape)} on {g.device} does not "
+                                    f"match query_all {tuple(q.shape)} on {q.device} ({_lib.last_error()})")
+            _lib.check(rc, "dcr_sim_range_sharded")
+            break
+    n = int(counts[0])
+    if n < out_cap:   # do not keep the whole capacity alive behind the result
+        out_i, out_s = out_i[:n].clone(), out_s[:n].clone()
+    return offsets, out_i, out_s
 
 
 def device_bytes(ptr: int, nbytes: int, device: torch.device) -> torch.Tensor:

@@ -142,6 +142,49 @@ int dcr_sim_range(const float* q, int nq, const float* g, int ng, int d, float t
                   int64_t g_index_stride, int64_t* row_offsets, int64_t* out_idx, float* out_scores, int64_t max_pairs,
                   int64_t* counts, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Gallery-sharded form: this rank searches ALL queries q[nq,d] against ITS gallery shard g[ng_local,d] (global index of
+ * local row j = g_index_base + g_index_stride * j; contiguous shards or interleaved ones with stride = world), the per-rank
+ * CSR pieces are exchanged through the caller's all-gather (dcr_allgather_fn, as dcr_sim_topk_sharded) and merged on the
+ * device.  On success every rank holds the CSR dcr_sim_range returns for the same queries against the union of the shards,
+ * bit for bit: offsets, indices (ascending within a row) and scores.  ng_local = 0 is allowed (g may then be NULL): the
+ * rank contributes nothing but takes part in both exchanges.  world = 1 never calls the callback.
+ *
+ * Agreement.  Only world < 1 (or > 65535) and a missing callback with world > 1 return before the first exchange.  Every
+ * other outcome is decided from a header that every rank all-gathers first (the callback's first call, 80 bytes per rank,
+ * int64 words):
+ *     [0] 0x31474E52524344 ("DCRRNG1" in memory)   [1] status: 0, DCR_ERR_CAPACITY or the code of a local failure
+ *     [2] local pairs   [3] local candidates (the max_local_pairs its search needs)   [4] max_local_pairs   [5] max_pairs
+ *     [6] nq   [7] d   [8] the threshold's fp32 bits   [9] 0
+ * so every rank returns the same code:
+ *   - a local failure on any rank (bad argument, workspace too small, CUDA error): that rank's code on every rank
+ *   - headers that disagree on nq, d or the threshold: -1
+ *   - a local search over its candidate capacity, a largest local pair count above some rank's max_local_pairs, or a
+ *     global pair total above some rank's max_pairs: DCR_ERR_CAPACITY with counts[1] = the largest local candidate count
+ *     and counts[2] = the global total (when a search did not finish, a bound: its candidates stand for its pairs).  The
+ *     call repeated on every rank with max_local_pairs = counts[1] and max_pairs = counts[2] succeeds.
+ *   - two ranks reporting the same global index (overlapping shards), or a malformed message: -1, nothing written.
+ * The second call of the callback exchanges the messages, each padded to the largest (bytes_per_rank = the message size
+ * for the largest pair count in the headers).  Message of a rank with P pairs, 8-byte aligned:
+ *     int64 offsets[nq + 1]   its CSR row offsets (offsets[0] = 0, offsets[nq] = P)
+ *     int64 idx[P]            global gallery indices, ascending within a row
+ *     fp32  scores[P]
+ *     padding to bytes_per_rank = (8 * (nq + 1) + 12 * P_max) rounded up to a multiple of 16
+ * The merge: row i of the result holds sum over ranks (in rank order) of the ranks' row-i counts entries, placed by the
+ * fixed-association scan of dcr_sim_range; each entry's place in its row is its place in its own piece plus, for every
+ * other rank, the number of that rank's row-i entries with a smaller index (binary search).  No atomic decides an order.
+ * Outputs and counts (HOST [3]: [0] pairs returned, [1] / [2] as above) as dcr_sim_range, with out_idx / out_scores
+ * holding max_pairs entries.  Synchronises `stream` before returning.
+ * workspace: dcr_sim_range_sharded_workspace_size(nq, ng_local, d, world, max_local_pairs) bytes: the local search's
+ * workspace, a send buffer and a receive buffer of world x the message size for max_local_pairs pairs (which bounds every
+ * message the call accepts), and nq int64 counts.  It grows with nq, ng_local, d, world and max_local_pairs, never with
+ * nq * ng.  The header buffers sit at the head of the workspace; a rank whose workspace cannot hold even them (NULL, say)
+ * allocates them on `stream` (stream-ordered), so that it still takes part in the header exchange. */
+size_t dcr_sim_range_sharded_workspace_size(int nq, int ng_local, int d, int world, int64_t max_local_pairs);
+int dcr_sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int d, float threshold,
+                          int64_t g_index_base, int64_t g_index_stride, int world, dcr_allgather_fn allgather,
+                          void* allgather_ctx, int64_t* row_offsets, int64_t* out_idx, float* out_scores, int64_t max_pairs,
+                          int64_t max_local_pairs, int64_t* counts, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- dense contraction of the descriptor networks ------------------------------------------------------------- */
 /* y = act(scale[n] * conv2d(x, w)[.., n] + bias[n] (+ residual)) as a wgmma implicit GEMM.
  *   x        NHWC bf16, `x_planes` planes of B*H*W*C elements each (plane p at x + p*x_plane_stride elements);
