@@ -26,11 +26,14 @@ SENTINEL = -7.75                # output planes the op must not touch
 
 # ---- micro-network plumbing ---------------------------------------------------------------------------------------
 class Micro:
-    """A DcrNet with direct access to its activation tensors."""
+    """A DcrNet with direct access to its activation tensors.  precision: a name of nets.PRECISION_PLANES, or a plane
+    count (1: "fast", 3: "fp32")."""
 
-    def __init__(self, max_batch: int, planes: int):
-        self.net = nets.DcrNet(max_batch, "fast" if planes == 1 else "fp32")
-        self.lib, self.mb, self.planes = self.net.lib, max_batch, planes
+    def __init__(self, max_batch: int, precision):
+        if not isinstance(precision, str):
+            precision = "fast" if precision == 1 else "fp32"
+        self.net = nets.DcrNet(max_batch, precision)
+        self.lib, self.mb, self.planes = self.net.lib, max_batch, self.net.planes
         self.shapes = {}
 
     def tensor(self, rows: int, ch: int) -> int:
