@@ -11,13 +11,17 @@ What changes underneath:
     them are nearest-neighbour questions, answered by the fused similarity + top-k kernel on augmented vectors:
         -d(x,y)^2 / 2 + ||x||^2 / 2 = x.y - ||y||^2 / 2            = [x, 1] . [y, -||y||^2 / 2]              (k-th NN radius)
         (r_j^2 - d(y_j, x)^2) / 2 + ||x||^2 / 2 = x.y_j + (r_j^2 - ||y_j||^2) / 2                          (inside any ball?)
-    The kernel ranks by the float64 dot product of the float32 vectors (features are centred first so that the rounding of
-    the augmented component is small against the gaps between neighbours); a few spare candidates are kept and the final
-    distances / comparisons are re-evaluated in float64 with the reference's own formula on the ORIGINAL features, so radii
-    and the precision / recall counts agree with the reference to float64 rounding.
+    Features are float32 (what the VGG-16 network produces), used uncentred, so the vector part of both operands is exact.
+    The float64 norm term, divided by a power of two s, is carried as an error-free split into three float32 columns
+    (hi + mid + lo == the float64 value) against s, s, s on the query side (_operands).  The kernel ranks by the float64
+    dot product of its float32 operands, so its ranking is the float64 ranking of the features themselves: a few spare
+    candidates absorb float64-level ties, and the final distances / comparisons are re-evaluated in float64 with the
+    reference's own formula, so radii and the precision / recall counts agree with the reference to float64 rounding --
+    also for sets of exact and near copies.
 """
 from __future__ import annotations
 
+import math
 import os
 from collections import namedtuple
 from glob import glob
@@ -34,16 +38,52 @@ from .similarity import sim_topk
 Manifold = namedtuple("Manifold", ["features", "radii"])
 PrecisionAndRecall = namedtuple("PrecisinoAndRecall", ["precision", "recall"])     # (sic) metrics/ipr.py:31
 
-_SPARE = 3          # candidates kept beyond what the exact answer needs
+_SPARE = 3          # candidates kept beyond what the exact answer needs (float64-level ties)
+_MAX_CANDIDATES = 16  # sim_topk keeps at most 16 rows per query
 
 
-def _augmented(feats64: torch.Tensor, centre: torch.Tensor, last: torch.Tensor) -> torch.Tensor:
-    """[feats - centre | last | 0 0 0] as float32 (descriptor dim must be a multiple of 4 for the kernel)."""
-    n, d = feats64.shape
-    out = torch.zeros((n, d + 4), dtype=torch.float32, device=feats64.device)
-    out[:, :d] = (feats64 - centre).float()
-    out[:, d] = last.float()
+def _split3(a: torch.Tensor) -> torch.Tensor:
+    """float64 [n] -> float32 [n, 3] (hi, mid, lo) with hi + mid + lo == a exactly (each step's remainder is exact)."""
+    hi = a.float()
+    r = a - hi.double()
+    mid = r.float()
+    lo = (r - mid.double()).float()
+    return torch.stack([hi, mid, lo], dim=1)
+
+
+def _augmented(x32: torch.Tensor, tail: torch.Tensor) -> torch.Tensor:
+    """[x | tail | 0 ...] as float32, the width padded to a multiple of 4 (sim_topk's requirement)."""
+    n, d = x32.shape
+    out = torch.zeros((n, (d + 6) // 4 * 4), dtype=torch.float32, device=x32.device)
+    out[:, :d] = x32
+    out[:, d:d + 3] = tail
     return out
+
+
+def _operands(queries: torch.Tensor, rows: torch.Tensor, term: torch.Tensor):
+    """sim_topk operands whose float64 score is queries_i . rows_j + term_j with no rounding of either operand: the
+    features as float32 (exact for float32 features), and term / s split over three columns against s, s, s.
+    s is a power of two (the products are the same), 4x the largest feature norm rounded up: the constant query columns
+    then dominate the queries' mean square, so sim_topk centres the queries, and term / s varies no more than the features
+    do.  Both keep the kernel's bf16 error bound as tight as for centred features, so few queries need its float64
+    brute-force path (with s = 1 every query of 4096-d VGG features does)."""
+    q32, r32 = queries.float(), rows.float()
+    top = max((q32.double() ** 2).sum(-1).max().item(), (r32.double() ** 2).sum(-1).max().item()) ** 0.5
+    s = 2.0 ** (math.ceil(math.log2(max(top, 2.0 ** -60))) + 2)
+    cols = torch.full((q32.shape[0], 3), s, dtype=torch.float32, device=q32.device)
+    return _augmented(q32, cols), _augmented(r32, _split3(term / s))
+
+
+def _knn_operands(x: torch.Tensor):
+    """Score x_i . x_j - ||x_j||^2 / 2 = (||x_i||^2 - d(x_i, x_j)^2) / 2: nearest rows first."""
+    x32 = x.float()
+    return _operands(x32, x32, -0.5 * (x32.double() ** 2).sum(-1))
+
+
+def _ball_operands(ref: torch.Tensor, radii: torch.Tensor, subjects: torch.Tensor):
+    """Score s_i . r_j + (rad_j^2 - ||r_j||^2) / 2 = (rad_j^2 - d(s_i, r_j)^2 + ||s_i||^2) / 2: deepest ball first."""
+    r32 = ref.float()
+    return _operands(subjects, r32, 0.5 * (radii * radii - (r32.double() ** 2).sum(-1)))
 
 
 def _sq_dists(a64: torch.Tensor, b64: torch.Tensor) -> torch.Tensor:
@@ -55,15 +95,17 @@ def _sq_dists(a64: torch.Tensor, b64: torch.Tensor) -> torch.Tensor:
 def kth_nn_radii(features, k: int = 3) -> np.ndarray:
     """distances2radii(compute_pairwise_distances(features), k) (metrics/ipr.py:119-121, 220-233): per row the distance to
     its k-th nearest OTHER row -- the (k+1)-th smallest entry of its distance row, the smallest being the row itself."""
-    x = torch.as_tensor(np.asarray(features), dtype=torch.float64).cuda()
-    n = x.shape[0]
-    kk = min(k + 1 + _SPARE, n, 16)
-    if k + 1 > n:
-        raise ValueError(f"k = {k} needs at least {k + 1} samples (np.argpartition would fail in the reference, too)")
-    centre = x.mean(dim=0, keepdim=True)
-    xc = (x - centre)
-    q = _augmented(x, centre, torch.ones(n, dtype=torch.float64, device=x.device))
-    g = _augmented(x, centre, -0.5 * (xc.float().double() ** 2).sum(-1))
+    if k + 1 + _SPARE > _MAX_CANDIDATES:
+        raise _lib.DcrError(f"k = {k}: at most k = {_MAX_CANDIDATES - 1 - _SPARE} (k + 1 + {_SPARE} spare candidates per "
+                            f"row, sim_topk keeps at most {_MAX_CANDIDATES})")
+    features = np.asarray(features)
+    n = features.shape[0]
+    if k < 0 or n < k + 2:
+        raise ValueError(f"k = {k} needs k >= 0 and at least {k + 2} samples, got {n} "
+                         f"(np.argpartition(row, k + 1) fails in the reference, too)")
+    x = torch.as_tensor(features, dtype=torch.float64).cuda()
+    kk = min(k + 1 + _SPARE, n)
+    q, g = _knn_operands(x)
     _, idx = sim_topk(q, g, kk)                                            # nearest rows first (self among them)
     cand = x[idx.reshape(-1)].reshape(n, kk, -1)
     d = torch.sqrt(_sq_dists(x[:, None, :].expand_as(cand), cand))        # [n, kk] float64
@@ -77,11 +119,8 @@ def compute_metric(manifold_ref: Manifold, feats_subject, desc: str = "") -> flo
     rad = torch.as_tensor(np.asarray(manifold_ref.radii), dtype=torch.float64).cuda()
     sub = torch.as_tensor(np.asarray(feats_subject), dtype=torch.float64).cuda()
     ns, nr = sub.shape[0], ref.shape[0]
-    kk = min(1 + 2 * _SPARE, nr, 16)
-    centre = ref.mean(dim=0, keepdim=True)
-    rc = ref - centre
-    g = _augmented(ref, centre, 0.5 * (rad * rad - (rc.float().double() ** 2).sum(-1)))
-    q = _augmented(sub, centre, torch.ones(ns, dtype=torch.float64, device=sub.device))
+    kk = min(1 + 2 * _SPARE, nr)
+    q, g = _ball_operands(ref, rad, sub)
     _, idx = sim_topk(q, g, kk)                                            # balls the subject is deepest inside, first
     cand = ref[idx.reshape(-1)].reshape(ns, kk, -1)
     d = torch.sqrt(_sq_dists(cand, sub[:, None, :].expand_as(cand)))      # dist[j, i] of the reference, selected pairs
