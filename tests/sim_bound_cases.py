@@ -1,0 +1,273 @@
+"""Operands that drive the bf16 error of the fused similarity sweep to its bound (test infrastructure only).
+
+dcr_sim_topk and dcr_sim_range both rank on a bf16 tensor-core score and trust one number per query, the `eps` of
+row_bound (dcr_b200/csrc/sim_topk.cu), to bound |approximate score - exact centred score|.  Random descriptors keep that
+error far below the bound.  The instances built here reach it, and they are built so that a CPU restatement of stage 1
+reproduces the kernel's operands bit for bit:
+
+- Few significant bits.  Gallery elements are 1 + x*2^-11 for a small integer x, or +-1; query elements are small
+  multiples of 1/2.  Every fp32 partial sum of col_sum_kernel and of the tensor-core accumulation, and every fp64 dot
+  product, is then exact: the centres, the approximate scores and the exact scores are known without rounding, and
+  equal exact scores are real ties.
+- Known centres.  The gallery comes in exact +- pairs, so its centre mu is 0.  The queries come in pairs c + w, c - w:
+  with c = 0 the query centre is 0 and centring stays off; with c = 8 p (p = +1 on the first half of the dimensions,
+  -1 on the second) the centre is exactly c, q - nu = +-w, and centre_decision_kernel switches centring on.
+- The target A (every element 1 + 7*2^-11, just below the rounding midpoint 1 + 2^-8, so it rounds down to 1) loses
+  ||w|| ||A - bf16(A)|| of its score to bf16 rounding: the Cauchy-Schwarz bound that eps is written for, attained.  It
+  is the gallery's largest-residual row.
+- The competitors B have a elements per half at 1 + 9*2^-11 (rounds up to 1 + 2^-7) and the rest at 1 - 3*2^-11 (rounds
+  up to 1).  With 24 a < 10 d their exact score lies below A's, by as little as a few 2^-11 quanta, while their bf16
+  score lies up to almost 2 eps above A's.  B rows (or the tie twin) are the gallery's largest-norm rows.
+- Fillers are +-1 rows that score far below A for both queries.
+
+For the query c - w the rows -A and -B play the roles of A and B, so both queries of a pair meet the same instance.
+"""
+from __future__ import annotations
+
+from dataclasses import dataclass, field
+
+import numpy as np
+import torch
+
+U = 2.0 ** -11          # the gallery's quantum
+SEG = 64                # the target and its competitors sit in the first 64 columns of a 128-row tile: one segment
+                        # whether the fused sweep runs one epilogue set (128 columns) or two (64 each)
+KP0 = {1: 4, 2: 4, 10: 12, 16: 32}   # candidates the first pass keeps per segment, by k (make_plan)
+KP1 = 32                             # candidates of the second-chance pass
+
+
+def bf16(x: np.ndarray) -> np.ndarray:
+    """Round-to-nearest-even fp32 -> bf16, back in fp32 (torch's conversion is RNE, as __float2bfloat16_rn)."""
+    return torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).to(torch.bfloat16).float().numpy()
+
+
+def _levels(d: int):
+    """Counts a of 1 + 9*2^-11 elements per half of a B row: exact score below A's (24 a < 10 d), bf16 score above A's
+    fp32 score (32 a > 7 d).  Highest first (the closest to A, the largest bf16 lead)."""
+    a_max = -(-10 * d // 24) - 1
+    a_min = 7 * d // 32 + 1
+    return list(range(a_max, a_min - 1, -1))
+
+
+def _b_row(d: int, a: int, rng, bump: int = 0) -> np.ndarray:
+    """x offsets of a B row: per half a entries 9, the rest -3; `bump` (even, < 24) is added to each half by raising
+    -3 entries to 0 (+3) and one to -2 or -1, which still round up to 1."""
+    x = np.empty(d, dtype=np.int64)
+    h = d // 2
+    for lo in (0, h):
+        part = np.full(h, -3, dtype=np.int64)
+        part[rng.permutation(h)[:a]] = 9
+        rest = np.nonzero(part == -3)[0]
+        b, j = bump, 0
+        while b > 0:
+            step = min(3, b)
+            part[rest[j]] += step
+            b -= step
+            j += 1
+        x[lo:lo + h] = part
+    return x
+
+
+def _filler(d: int, rng) -> np.ndarray:
+    """+-1 row with d/4 + u_h ones in each half (u_h in -1..1, |u_1 - u_2| <= 1): sum 2(u_1 + u_2), p-sum 2(u_1 - u_2)."""
+    h = d // 2
+    u1 = int(rng.integers(-1, 2))
+    u2 = int(np.clip(u1 + rng.integers(-1, 2), -1, 1))
+    f = np.empty(d, dtype=np.float32)
+    for lo, u in ((0, u1), (h, u2)):
+        part = -np.ones(h, dtype=np.float32)
+        part[rng.permutation(h)[:h // 2 + u]] = 1.0
+        f[lo:lo + h] = part
+    return f
+
+
+@dataclass
+class Case:
+    """One instance.  Query i's target is target[i], its competitors comps[i], its tie twin twin[i] (-1: none)."""
+    q: np.ndarray
+    g: np.ndarray
+    centred: bool
+    target: np.ndarray
+    comps: list
+    twin: np.ndarray
+    info: dict = field(default_factory=dict)
+
+
+def build(d: int, n_b: int, *, centred: bool, shared: bool = False, tie: bool = False, tiles: int = 2,
+          scales=(1.0,), seed: int = 0) -> Case:
+    """The gallery X ++ (-X), X of 128 * tiles rows.  A sits in tile 0 (position 2 when it has competitors before it);
+    the n_b competitors fill the rest of tile 0's first 64 rows, or of tile 1's when `shared` (A alone in its
+    segment).  With `tie`, a twin row right after A has A's exact score and a bf16 score like the best B's.  Queries:
+    for every scale s, the pair c + s w, c - s w."""
+    assert d % 4 == 0 and d >= 64
+    rng = np.random.default_rng(seed + 7919 * d + 31 * n_b + 3 * int(centred) + 5 * int(shared) + 11 * int(tie))
+    n_x = 128 * tiles
+    X = np.stack([_filler(d, rng) for _ in range(n_x)])
+    lv = _levels(d)
+    a_row = 1.0 + 7 * U
+    b_rows = [(1.0 + _b_row(d, lv[j % len(lv)], rng) * U) for j in range(n_b)]
+    pos_a = 0 if shared else min(2, n_b)
+    X[pos_a] = a_row
+    if shared:
+        assert tiles >= 2 and n_b <= SEG
+        b_pos = list(range(128, 128 + n_b))
+    else:
+        free = [p for p in range(SEG) if p != pos_a and not (tie and p == pos_a + 1)]
+        assert n_b <= len(free)
+        b_pos = free[:n_b]
+    for p, r in zip(b_pos, b_rows):
+        X[p] = r
+    twin = -1
+    if tie:
+        a = lv[0]
+        bump = 5 * d - 12 * a                       # per half: reach A's half sum 3.5 d exactly
+        assert 0 < bump < 24 and bump % 2 == 0
+        twin = pos_a + 1
+        X[twin] = 1.0 + _b_row(d, a, rng, bump) * U
+    X = X.astype(np.float32)
+    g = np.concatenate([X, -X]).astype(np.float32)
+    w = np.ones(d, dtype=np.float32)
+    p = np.concatenate([np.ones(d // 2), -np.ones(d // 2)]).astype(np.float32)
+    c = 8.0 * p if centred else np.zeros(d, dtype=np.float32)
+    qs, target, comps, twins = [], [], [], []
+    for s in scales:
+        for sign in (1, -1):
+            qs.append(c + sign * s * w)
+            off = 0 if sign > 0 else n_x
+            target.append(off + pos_a)
+            comps.append(np.array(b_pos, dtype=np.int64) + off)
+            twins.append(off + twin if tie else -1)
+    q = np.stack(qs).astype(np.float32)
+    return Case(q=q, g=g, centred=centred, target=np.array(target, dtype=np.int64), comps=comps,
+                twin=np.array(twins, dtype=np.int64), info=dict(d=d, n_b=n_b, shared=shared, tie=tie))
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# CPU restatement of stage 1 and of row_bound
+
+
+def centre(x: np.ndarray):
+    """col_sum_kernel + col_mean_finish_kernel (every partial sum exact here, so the order does not matter) and
+    centre_decision_kernel: (mean as fp32, centring flag)."""
+    x64 = x.astype(np.float64)
+    n = x.shape[0]
+    sums, sq = x64.sum(axis=0), (x64 * x64).sum(axis=0)
+    m2 = float(np.sum(sq / n))
+    nu2 = float(np.sum((sums / n) ** 2))
+    return (sums / n).astype(np.float32), (m2 - nu2 < m2 / 16.0)
+
+
+@dataclass
+class Operands:
+    mu: np.ndarray
+    nu: np.ndarray          # the query centre in use (zeros when centring is off)
+    flag: bool
+    qh: np.ndarray          # bf16(q - nu), fp32 values
+    gh: np.ndarray          # bf16(g - mu)
+    qv: np.ndarray          # fp32(q - nu)
+    gv: np.ndarray          # fp32(g - mu)
+    qnh: np.ndarray         # to_bf16_rows_kernel's norms of the query rows
+    qnr: np.ndarray
+    qnx: np.ndarray
+    g_norm: np.float32      # gmax[0], gmax[1]
+    g_res: np.float32
+    bias: np.ndarray        # fp32 nu.(g - mu) per gallery row (zeros when centring is off)
+
+
+def _norm(v: np.ndarray) -> np.ndarray:
+    """sqrtf of the row's sum of squares times 1.0001f, as to_bf16_rows_kernel stores it (the kernel's fp32 summation
+    order is not restated: the sums agree to an ulp or two)."""
+    s = np.sum(v.astype(np.float64) ** 2, axis=1).astype(np.float32)
+    return (np.sqrt(s) * np.float32(1.0001)).astype(np.float32)
+
+
+def operands(q: np.ndarray, g: np.ndarray) -> Operands:
+    mu, _ = centre(g)
+    nu, flag = centre(q)
+    if not flag:
+        nu = np.zeros_like(nu)
+    qv = (q - nu[None, :]).astype(np.float32)
+    gv = (g - mu[None, :]).astype(np.float32)
+    qh, gh = bf16(qv), bf16(gv)
+    bias = (gv.astype(np.float64) @ nu.astype(np.float64)).astype(np.float32) if flag else np.zeros(g.shape[0], np.float32)
+    return Operands(mu=mu, nu=nu, flag=flag, qh=qh, gh=gh, qv=qv, gv=gv, qnh=_norm(qh), qnr=_norm(qv - qh),
+                    qnx=_norm(qv), g_norm=_norm(gv).max(), g_res=_norm(gv - gh).max(), bias=bias)
+
+
+def d_pad(d: int) -> int:
+    return -(-d // 64) * 64
+
+
+def eps(op: Operands, d: int) -> np.ndarray:
+    """row_bound's eps per query row, in the kernel's fp32 order of operations."""
+    f = np.float32
+    qh, qr, qx = op.qnh, op.qnr, op.qnx
+    e = f(1.001) * (qh * op.g_res + qr * op.g_norm) + f(d_pad(d)) * f(2.4e-7) * qh * (op.g_norm + op.g_res) + f(1e-30)
+    nun = f(np.sqrt(np.float32(np.sum(op.nu.astype(np.float64) ** 2))) * f(1.001)) if op.flag else f(0)
+    return (e + f(3e-7) * (qx + nun) * op.g_norm).astype(np.float32)
+
+
+def bf16_terms(op: Operands) -> np.ndarray:
+    """The bf16 part of eps, qh g_res + qr g_norm: what a row's bf16 rounding alone can cost."""
+    return (op.qnh * op.g_res + op.qnr * op.g_norm).astype(np.float32)
+
+
+def approx(op: Operands) -> np.ndarray:
+    """The fused sweep's score: the tensor-core product of the bf16 operands (exact here) plus the column offset, one
+    fp32 addition."""
+    acc = (op.qh.astype(np.float64) @ op.gh.astype(np.float64).T).astype(np.float32)
+    return (acc + op.bias[None, :]).astype(np.float32)
+
+
+def exact(q: np.ndarray, g: np.ndarray) -> np.ndarray:
+    return q.astype(np.float64) @ g.astype(np.float64).T
+
+
+def realized(case: Case, op: Operands) -> np.ndarray:
+    """Per query: how far the target's approximate score lies below its exact centred score q.(g - mu)."""
+    ex_c = case.q.astype(np.float64) @ op.gv.astype(np.float64).T
+    a = approx(op).astype(np.float64)
+    rows = np.arange(case.q.shape[0])
+    return ex_c[rows, case.target] - a[rows, case.target]
+
+
+def as_integers(x: np.ndarray, quantum: float) -> np.ndarray:
+    """x / quantum as int64, asserting that every entry is an integer multiple of the quantum."""
+    y = x.astype(np.float64) / quantum
+    assert np.array_equal(y, np.round(y)), "entries off the quantum grid"
+    return y.astype(np.int64)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# The instances the tests run
+
+DIMS = (64, 512, 516, 1024, 4096)   # resident query tile, padded d_pad, streamed query tile
+
+# (name, k, competitors, competitors in another segment, tie twin, stage that must decide both queries)
+#   first:  fewer than kp - 1 competitors share A's segment: A is a candidate of the first pass and the re-score puts it
+#           above the competitors the bf16 scores rank first
+#   second: at least kp of them (or, shared, in another segment whose threshold reaches A's unit): the first pass drops
+#           A, the certificate fails, the second-chance pass keeps 32 per segment and finds it
+#   brute:  more than 32: the brute-force path (k = 16 has no second pass)
+TOPK_CASES = [
+    ("k1_first", 1, 2, False, False, "first"),
+    ("k2_first", 2, 2, False, False, "first"),
+    ("k10_first", 10, 10, False, False, "first"),
+    ("k16_first", 16, 20, False, False, "first"),
+    ("k1_second", 1, 8, False, False, "second"),
+    ("k2_second", 2, 30, False, False, "second"),
+    ("k10_second", 10, 20, False, False, "second"),
+    ("k1_brute", 1, 40, False, False, "brute"),
+    ("k10_brute", 10, 40, False, False, "brute"),
+    ("k16_brute", 16, 40, False, False, "brute"),
+    ("k1_shared", 1, 8, True, False, "second"),
+    ("k10_shared", 10, 20, True, False, "second"),
+    ("k1_tie", 1, 1, False, True, "first"),
+    ("k2_tie", 2, 1, False, True, "first"),
+    ("k10_tie", 10, 9, False, True, "first"),
+]
+
+
+def topk_case(name: str, d: int, centred: bool) -> Case:
+    _, k, n_b, shared, tie, _ = next(c for c in TOPK_CASES if c[0] == name)
+    return build(d, n_b, centred=centred, shared=shared, tie=tie)
