@@ -17,6 +17,12 @@
 // Weights are streamed per (tap, channel block) exactly as in the generic kernel (all SMs read the same tiles; that
 // traffic is served at several times the rate of per-SM-unique data).  Fast (single-plane bf16) mode only, no residual:
 // what the 3x3 convolutions of the ResNet / ResNeXt bottlenecks need.
+//
+// Ping-pong schedule (as in conv_gemm.cu): the CTA's tiles are dealt alternately to the two consumer
+// warpgroups, each accumulates whole 128 x BN tiles, and a warpgroup starts its k-loop only once the other one has issued
+// its last wgmma, so one tile's epilogue runs under the next tile's k-loop.  The halo ring and the weight ring (or the
+// resident taps) are shared in tile order; each warpgroup has its own output staging box, which its epilogue fills
+// straight from the accumulator layout (no transpose buffers: that shared memory keeps a third halo buffer at W = 56).
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -33,7 +39,10 @@ namespace {
 constexpr int kHM = 128;                    // MMA rows (padded-raster positions) per tile
 constexpr int kHK = 64;                     // channels per block = one 128-byte swizzled row
 constexpr int kSlabBytes = kHM * 128;       // one 64-channel slab of the output staging tile
-constexpr int kHThreads = 288;              // warps 0-7 two consumer warpgroups (MMA + epilogue), warp 8 producer
+// warps 0-7 two consumer warpgroups (MMA + epilogue), warp 8 producer, warps 9-11 idle: the producer warpgroup's
+// registers go to the consumers (8 x 224 + 4 x 56 per lane = the 384 x 168 the CTA is launched with)
+constexpr int kHThreads = 384;
+constexpr int kHConsumerRegs = 224, kHProducerRegs = 56;
 
 struct HaloMaps {
   CUtensorMap a;     // input  [B][H][W][C]   box 64 x (W+2) x (R+2) x 1
@@ -68,17 +77,17 @@ __global__ void __launch_bounds__(kHThreads, 1)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int kWStage = BN * 128;
-  constexpr int kChunksPerWarp = BN / 64;
+  constexpr int kStageBytes = (BN / 64) * kSlabBytes;                       // one output staging box
   uint8_t* a_ring = smem;
   uint8_t* w_ring = a_ring + p.a_bufs * p.a_buf_bytes;                // kRW: 9 * cblocks resident tiles, tap-major
-  uint8_t* out_stage = w_ring + (kRW ? 9 * p.cblocks : p.w_stages) * kWStage;                 // BN/64 slabs
-  uint8_t* acc_xpose = out_stage + (BN / 64) * kSlabBytes;                  // [8 warps] accumulator transposes
-  float* sb = reinterpret_cast<float*>(acc_xpose + 8 * kAccXposeWarpBytes);   // [scale | bias][BN]
+  uint8_t* out_stage = w_ring + (kRW ? 9 * p.cblocks : p.w_stages) * kWStage;   // [2 warpgroups] BN/64 slabs
+  float* sb = reinterpret_cast<float*>(out_stage + 2 * kStageBytes);      // [scale | bias][BN]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sb + 2 * BN);
   uint64_t* a_full = bars;          // [4]
   uint64_t* a_empty = bars + 4;     // [4]
   uint64_t* w_full = bars + 8;      // [8]
   uint64_t* w_empty = bars + 16;    // [8]
+  uint64_t* turn = bars + 24;       // [2] turn[g] completes when warpgroup g may start its k-loop
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
@@ -89,20 +98,22 @@ __global__ void __launch_bounds__(kHThreads, 1)
   if (warp == 0 && lane == 0) {
     for (int s = 0; s < p.a_bufs; ++s) {
       mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], 8);   // one arrive per consumer warp
+      mbar_init(&a_empty[s], 4);   // one arrive per warp of the warpgroup that consumes it
     }
     for (int s = 0; s < (kRW ? 1 : p.w_stages); ++s) {
       mbar_init(&w_full[s], 1);
-      mbar_init(&w_empty[s], 8);
+      mbar_init(&w_empty[s], 4);
     }
+    for (int g = 0; g < 2; ++g) mbar_init(&turn[g], 4);   // the other warpgroup's four warps
     fence_mbar_init();
   }
   __syncthreads();
 
-  if (warp == 8) {
+  if (warp >= 8) {
     // ===================================== TMA producer =====================================
     // (whole warp walks the loop, one elected lane issues: see conv_gemm.cu)
-    {
+    wg_regs_dec<kHProducerRegs>();
+    if (warp == 8) {
       PipeState as(p.a_bufs), ws(kRW ? 1 : p.w_stages);
       if constexpr (kRW) {   // every filter tap once
         if (elect_one()) {
@@ -139,33 +150,51 @@ __global__ void __launch_bounds__(kHThreads, 1)
     }
   } else {
     // ===================================== consumer warpgroups =====================================
-    const uint32_t ewarp = warp;
+    wg_regs_inc<kHConsumerRegs>();
     const uint32_t quad = warp & 3;
-    const uint32_t half = ewarp >> 2;                    // column half of the tile (= warpgroup)
-    const uint32_t m = quad * 32 + lane;                 // padded-raster position of this thread's accumulator row
-    const uint32_t etid = ewarp * 32 + lane;
-    const uint32_t xacc = smem_u32(acc_xpose) + warp * kAccXposeWarpBytes;
+    const uint32_t wg = warp >> 2;
+    const uint32_t gtid = (warp & 3) * 32 + lane;       // 0..127 within the warpgroup
     const uint32_t a_base = smem_u32(a_ring);
-    const uint32_t w_base = smem_u32(w_ring) + half * (BN / 2) * 128;
+    const uint32_t w_base = smem_u32(w_ring);
     const uint32_t row_bytes = static_cast<uint32_t>(p.Wp) * 128u;   // one padded image row (128 B per pixel)
+    const int k_groups = 9 * p.cblocks;                 // one wgmma group (4 x k16) per (channel block, tap)
     PipeState as(p.a_bufs), ws(kRW ? 1 : p.w_stages);
     if constexpr (kRW) mbar_wait(&w_full[0], 0);
-    const int pl = static_cast<int>(m) / p.Wp, ql = static_cast<int>(m) - pl * p.Wp;
-    const bool valid = ql < p.W && pl < p.R;
-    const uint32_t srow = static_cast<uint32_t>(pl * p.W + ql);          // row of the compact [R x W] staging box
-    const uint32_t sb_addr = smem_u32(sb), stage_addr = smem_u32(out_stage);
-    for (int c = etid; c < BN; c += 256) {
-      st_shared_f32(sb_addr + c * 4, (p.scale && c < p.N) ? p.scale[c] : 1.f);
-      st_shared_f32(sb_addr + (BN + c) * 4, (p.bias && c < p.N) ? p.bias[c] : 0.f);
+    // this thread's accumulator rows (WgAcc layout: rows r0 + 8 g of its warp's 32-row block, g = 0..3) -> rows of the
+    // compact [R x W] staging box; junk positions (the two pad columns per padded row, rows past R) are dropped
+    const uint32_t r0 = lane >> 2, c0 = 2 * (lane & 3);
+    uint32_t srow[4];
+    bool valid[4];
+#pragma unroll
+    for (int g = 0; g < 4; ++g) {
+      const int m = static_cast<int>(quad * 32 + r0 + 8 * g);   // padded-raster position
+      const int pl = m / p.Wp, ql = m - pl * p.Wp;
+      valid[g] = ql < p.W && pl < p.R;
+      srow[g] = static_cast<uint32_t>(pl * p.W + ql);
     }
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const uint32_t sb_addr = smem_u32(sb), stage_addr = smem_u32(out_stage) + wg * kStageBytes;
+    uint8_t* ostage = out_stage + wg * kStageBytes;
+    for (int c = warp * 32 + lane; c < BN; c += 256) {
+      st_shared_f32(sb_addr + c * 4, p.scale ? p.scale[c] : 1.f);
+      st_shared_f32(sb_addr + (BN + c) * 4, p.bias ? p.bias[c] : 0.f);
+    }
+    named_bar_sync(5, 256);
+    if (wg == 1) {                                      // the CTA's first tile is warpgroup 0's
+      as.skip(p.cblocks);
+      if constexpr (!kRW) ws.skip(k_groups);
+    }
+    uint32_t tc = 0;
+    for (int tile = blockIdx.x + wg * gridDim.x; tile < p.num_tiles; tile += 2 * gridDim.x, ++tc) {
       const int b = tile / p.tiles_per_img;
       const int p0 = (tile - b * p.tiles_per_img) * p.R;
-      if (etid == 0) tma_store_wait_read_();     // the previous tile's store has finished reading the staging box
-      asm volatile("bar.sync 1, 256;" ::: "memory");   // (also orders the scale/bias staging before its first use)
-      // main loop: per channel block one halo box, nine taps = nine start addresses into it
-      WgAcc<BN / 2> acc;
-      uint32_t accumulate = 0;
+      if (gtid == 0) tma_store_wait_read_();     // this warpgroup's previous store has finished reading its staging box
+      named_bar_sync(1 + 2 * wg, 128);
+      if (wg == 1 || tc > 0) mbar_wait(&turn[wg], (wg == 1 ? tc : tc - 1) & 1);
+      // main loop: per channel block one halo box, nine taps = nine start addresses into it.  Group (cb, tap)'s operands
+      // are released once wgmma_wait<1> after the next group has seen it complete.
+      WgAcc<BN> acc;
+      uint32_t prev_w = 0, prev_a = 0;
+      bool prev_a_last = false;
       for (int cb = 0; cb < p.cblocks; ++cb, as.next()) {
         const uint32_t sa = as.s;
         mbar_wait(&a_full[sa], as.ph);
@@ -185,68 +214,60 @@ __global__ void __launch_bounds__(kHThreads, 1)
           const uint32_t b_addr = w_base + sw * kWStage;
           wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kHK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), accumulate | k);
+          for (int k = 0; k < kHK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), (cb | tap | k) != 0);
           wgmma_commit();
-          wgmma_wait<0>();
-          accumulate = 1;
-          if constexpr (!kRW) {
-            if (lane == 0) mbar_arrive(&w_empty[sw]);
-            ws.next();
+          const bool last = cb == p.cblocks - 1 && tap == 8;
+          if (last && lane == 0) mbar_arrive(&turn[wg ^ 1]);   // hand the tensor core over
+          wgmma_wait<1>();
+          if ((cb | tap) != 0 && lane == 0) {
+            if constexpr (!kRW) mbar_arrive(&w_empty[prev_w]);
+            if (prev_a_last) mbar_arrive(&a_empty[prev_a]);
           }
+          prev_w = sw;
+          prev_a = sa;
+          prev_a_last = tap == 8;
+          if constexpr (!kRW) ws.next();
         }
-        if (lane == 0) mbar_arrive(&a_empty[sa]);
       }
+      wgmma_wait<0>();
       acc.fence_regs();
-#pragma unroll
-      for (int ci = 0; ci < kChunksPerWarp; ++ci) {
-        const int ch = half * kChunksPerWarp + ci;
-        uint32_t r[32];
-        acc.rows32(ci, r, xacc, lane);
-        if (ch * 32 >= p.N) continue;   // warp-uniform
-        float y[32];
-#pragma unroll
-        for (int c = 0; c < 32; c += 4) {
-          const float4 sc = ld_shared_f4(sb_addr + (ch * 32 + c) * 4);
-          const float4 bi = ld_shared_f4(sb_addr + (BN + ch * 32 + c) * 4);
-          y[c + 0] = fmaf(__uint_as_float(r[c + 0]), sc.x, bi.x);
-          y[c + 1] = fmaf(__uint_as_float(r[c + 1]), sc.y, bi.y);
-          y[c + 2] = fmaf(__uint_as_float(r[c + 2]), sc.z, bi.z);
-          y[c + 3] = fmaf(__uint_as_float(r[c + 3]), sc.w, bi.w);
-        }
-        if (p.act == 1) {
-#pragma unroll
-          for (int c = 0; c < 32; ++c) y[c] = fmaxf(y[c], 0.f);
-        }
-        const uint32_t dst = stage_addr + (ch >> 1) * kSlabBytes + srow * 128;
-        const uint32_t sw = srow & 7;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          uint4 v;
-          v.x = pack_bf16_(y[j * 8 + 0], y[j * 8 + 1]);
-          v.y = pack_bf16_(y[j * 8 + 2], y[j * 8 + 3]);
-          v.z = pack_bf16_(y[j * 8 + 4], y[j * 8 + 5]);
-          v.w = pack_bf16_(y[j * 8 + 6], y[j * 8 + 7]);
-          if (valid) st_shared_v4(dst + ((((ch & 1) * 4 + j) ^ sw) << 4), v);   // junk positions are dropped here
-        }
-        __syncwarp();
+      if (lane == 0) {
+        if constexpr (!kRW) mbar_arrive(&w_empty[prev_w]);
+        mbar_arrive(&a_empty[prev_a]);
       }
+      as.skip(p.cblocks);                                // the other warpgroup's next tile
+      if constexpr (!kRW) ws.skip(k_groups);
+      // epilogue: straight from the accumulator layout into the 128B-swizzled staging box, one bf16 pair per store (a
+      // warp's 8 rows x 16 B per store land in 8 different 16-byte bank groups)
+      acc.for_each_pair(lane, [&](uint32_t row, uint32_t col, float v0, float v1) {
+        const uint32_t g = (row - r0) >> 3;
+        const float2 sc = ld_shared_f2(sb_addr + col * 4);
+        const float2 bi = ld_shared_f2(sb_addr + (BN + col) * 4);
+        float y0 = fmaf(v0, sc.x, bi.x), y1 = fmaf(v1, sc.y, bi.y);
+        if (p.act == 1) {
+          y0 = fmaxf(y0, 0.f);
+          y1 = fmaxf(y1, 0.f);
+        }
+        const uint32_t chunk = (col & 63) >> 3;
+        if (valid[g])
+          st_shared_u32(stage_addr + (col >> 6) * kSlabBytes + srow[g] * 128 + ((chunk ^ (srow[g] & 7)) << 4) + c0 * 2,
+                        pack_bf16_(y0, y1));
+      });
       fence_proxy_async();
-      asm volatile("bar.sync 2, 256;" ::: "memory");
-      if (etid == 0) {
-        for (int sl = 0; sl < BN / 64; ++sl)
-          if (sl * 64 < p.N) tma_store_4d(&maps.out, out_stage + sl * kSlabBytes, p.out_col_off + sl * 64, 0, p0, b);
+      named_bar_sync(2 + 2 * wg, 128);
+      if (gtid == 0) {
+        for (int sl = 0; sl < BN / 64; ++sl) tma_store_4d(&maps.out, ostage + sl * kSlabBytes, p.out_col_off + sl * 64, 0, p0, b);
         tma_store_commit_();
       }
     }
-    if (etid == 0) tma_store_wait_all_();
+    if (gtid == 0) tma_store_wait_all_();
   }
-
 }
 
 template <int BN, bool kRW>
 int launch_halo(const HaloMaps& maps, HaloParams& p, int num_sms, size_t max_smem, cudaStream_t stream) {
   constexpr size_t kWStage = static_cast<size_t>(BN) * 128;
-  const size_t fixed = 1024 + static_cast<size_t>(BN / 64) * kSlabBytes + 8 * kAccXposeWarpBytes + 2 * BN * 4 + 256;
+  const size_t fixed = 1024 + static_cast<size_t>(2) * (BN / 64) * kSlabBytes + 2 * BN * 4 + 256;   // 2 staging boxes
   const size_t abuf = p.a_buf_bytes;
   size_t smem = 0;
   if constexpr (kRW) {

@@ -15,11 +15,14 @@
 // accumulates the listed cross terms into the same register accumulator, which reproduces fp32 arithmetic on the
 // tensor cores (DESIGN.md section 5).
 //
-// Structure per CTA (288 threads, persistent over output tiles of 128 x BN):
-//   warps 0-7 : two consumer warpgroups; warpgroup h issues the wgmma for columns [h BN/2, (h+1) BN/2) of the tile
-//               (two m64 x BN/2 x k16 per k16 step, fp32 accumulators in registers) and runs the epilogue of those
-//               columns (scale/bias/residual/activation -> bf16 planes / fp32 -> global)
-//   warp 8    : TMA producer (A tile 128x64, W tile BNx64 per stage, 128B swizzle)
+// Structure per CTA (384 threads, persistent over output tiles of 128 x BN, BN = 64 or 128):
+//   warps 0-7 : two consumer warpgroups in a ping-pong schedule.  The CTA's tiles are dealt alternately to warpgroup 0
+//               and 1; each owns whole tiles (two m64 x BN x k16 wgmma per k16 step, fp32 accumulators in registers)
+//               and runs their epilogue (scale/bias/residual/activation -> bf16 planes / fp32 -> global).  A warpgroup
+//               starts its k-loop only once the other one has issued its last k-block, so the tensor core sees
+//               back-to-back k-loops and each epilogue runs under the other warpgroup's k-loop.
+//   warp 8    : TMA producer (A tile 128x64, W tile BNx64 per stage, 128B swizzle), one stage ring in tile order
+//   warps 9-11: idle (they complete the producer warpgroup for the register reallocation)
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -35,7 +38,13 @@ namespace {
 
 constexpr int kBM = 128;
 constexpr int kBK = 64;
-constexpr int kThreads = 288;   // warps 0-7 MMA + epilogue (two warpgroups), warp 8 TMA
+// warps 0-7 MMA + epilogue (two warpgroups), warp 8 TMA; warps 9-11 only complete the producer warpgroup, whose
+// registers (setmaxnreg) go to the consumers: 8 x 224 + 4 x 56 per lane = the 384 x 168 the CTA is launched with.  The
+// direct epilogue (run-time activation, up to three output planes, fp32 output) needs more: 8 x 240 + 4 x 24.  These
+// are the splits at which ptxas reports no spills for any instantiation (DESIGN.md section 6).
+constexpr int kThreads = 384;
+constexpr int consumer_regs(int epi) { return epi == 0 ? 240 : 224; }
+constexpr int producer_regs(int epi) { return epi == 0 ? 24 : 56; }
 constexpr int kAccXposeBytes = 8 * kAccXposeWarpBytes;
 constexpr int kAStage = kBM * kBK * 2;   // 16 KB
 // direct epilogue: per epilogue warp a [32 rows][64 B + 16 B pad] buffer through which the bf16 planes are transposed, so that
@@ -70,8 +79,6 @@ struct GemmParams {
   int ld_out_f32;
   int act;                    // 0 none, 1 relu, 2 gelu (erf)
   int tma_epi;                // 1: stage the bf16 output tile in shared memory and write it with TMA stores
-  int n_out_bufs;             // 1 or 2 output staging tiles (2: the TMA store of tile i drains during tile i+1)
-  int n_res_bufs;             // 0 or 2 residual staging tiles (the residual of tile i+1 is prefetched during tile i)
   int fast_gelu;              // 1: single-plane bf16 mode: act 2 is the tanh-form GELU (gelu_tanh_fast); 0: erf form
   int n_fastest;              // 1: consecutive tiles are the column blocks of one m-tile (round robin over the CTAs: the CTAs that
                               //    share an m-tile's A rows read them at the same time, one HBM read + L2 hits).  Default order is
@@ -136,8 +143,7 @@ DCR_DEVICE void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;
 
 // kEpi: 0 = direct epilogue (any number of planes, optional fp32 output, runtime activation; parity mode and final
 //           layers), 1/2/3/4 = TMA-store epilogue with compile-time activation none / ReLU / GELU / QuickGELU (fast mode hot path).
-// Eight MMA + epilogue warps: warps w and w+4 own the same 32 rows and split the tile's columns, so every SM
-// sub-partition has two warps to switch between (the epilogue is latency bound, not issue bound).
+// Eight MMA + epilogue warps: warp w of a warpgroup owns rows 32w .. 32w+31 of the warpgroup's accumulator tile.
 template <int BN, bool kIm2col, int kEpi>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm_bf16_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
@@ -147,7 +153,10 @@ __global__ void __launch_bounds__(kThreads, 1)
   constexpr int kBStage = BN * kBK * 2;
   constexpr int kStageBytes = kAStage + kBStage;
   constexpr int kStagingBytes = (BN / 64) * kBM * 128;   // BN/64 slabs of [128 rows x 64 bf16], 128B swizzle
-  constexpr int kChunksPerWarp = BN / 64;                // 32-column chunks each epilogue warp handles per tile
+  constexpr int kChunksPerWarp = BN / 32;                // 32-column chunks each epilogue warp handles per tile
+  // wgmma groups (k-iterations) a warpgroup keeps in flight before it waits: one k-block of a 64-column tile is half the
+  // tensor-core work of a 128-column one, too little to cover the wgmma latency with a single group behind it
+  constexpr int kPend = BN <= 64 ? 2 : 1;
   const int stages = p.stages;
   const int k_iters = p.n_terms * p.taps * p.cblocks;
   // A-resident mode (wide 1x1 convolutions / Linear layers with small K): [k_iters x 16 KB A rows of the current m-tile]
@@ -157,16 +166,25 @@ __global__ void __launch_bounds__(kThreads, 1)
   const int num_n_tiles = p.num_n_tiles;
   uint8_t* smem_ares = smem;
   uint8_t* smem_ab = smem + (a_res ? k_iters * kAStage : 0);
-  uint8_t* out_stage = smem_ab + stages * stage_bytes;                      // n_out_bufs tiles, 1024-aligned
-  // direct epilogue (kEpi == 0): no staging tiles; one 32-row x 64-byte transpose buffer per epilogue warp instead
-  uint8_t* res_stage = out_stage + (kTma ? p.n_out_bufs * kStagingBytes : kXposeBytes);   // n_res_bufs tiles
-  uint8_t* acc_xpose = res_stage + p.n_res_bufs * kStagingBytes;   // [8 warps] accumulator transpose buffers
-  float* sb = reinterpret_cast<float*>(acc_xpose + kAccXposeBytes);   // [2 bufs][2 (scale,bias)][BN] | a_res: [2][n_tiles*BN]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sb + (a_res ? 2 * num_n_tiles * BN : 4 * BN));
+  uint8_t* out_stage = smem_ab + stages * stage_bytes;                      // 1024-aligned
+  // TMA-store epilogue: one staging tile per warpgroup (the residual lands in it by TMA and is overwritten in place by
+  // the output); direct epilogue: a 32-row transpose buffer per warp instead
+  uint8_t* acc_xpose = out_stage + (kTma ? 2 * kStagingBytes : kXposeBytes);   // [8 warps] accumulator transposes
+  // [2 warpgroups][2 bufs][2 (scale,bias)][BN] | a_res: [2][n_tiles*BN]
+  float* sb = reinterpret_cast<float*>(acc_xpose + kAccXposeBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sb + (a_res ? 2 * num_n_tiles * BN : 8 * BN));
   uint64_t* full = bars;          // [stages] (<= 12)
   uint64_t* empty = bars + 12;    // [stages]
-  uint64_t* res_full = bars + 28;   // [2]
-  uint64_t* a_full = bars + 10;    // A-resident mode (stages <= 8, so full[10..11] are free)
+  uint64_t* res_full = bars + 28;   // [2]  one per warpgroup
+  uint64_t* turn = bars + 30;       // [2]  ping-pong hand-off: turn[g] completes when warpgroup g may start its k-loop
+  // A-resident mode (stages <= 8, so full[9..11] are free): a_full[j & 1] completes when the rows of the CTA's j-th
+  // m-tile have landed.  Two barriers, because a ping-pong warpgroup may have no tile in the CTA's first m-tile and then
+  // waits for the second one: on a single barrier that parity would also match the not-yet-completed first phase.  Only
+  // the first and the last m-tile of the CTA can lack a tile of one warpgroup: the CTA's tiles are a contiguous range of
+  // the n-fastest order and A-resident layers have num_n_tiles >= 2, so every other m-tile contributes two or more
+  // consecutive tiles, which the alternation deals to both warpgroups.  A warpgroup therefore never waits on a barrier
+  // more than one phase ahead of the last phase it has seen complete, or could have seen (the CTA's first m-tile).
+  uint64_t* a_full = bars + 9;     // [2]
   uint64_t* a_empty = bars + 11;
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -196,19 +214,24 @@ __global__ void __launch_bounds__(kThreads, 1)
   if (warp == 0 && lane == 0) {
     for (int s = 0; s < stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 8);         // one arrive per consumer warp once its wgmma on the stage have completed
+      mbar_init(&empty[s], 4);           // one arrive per warp of the consuming warpgroup once its wgmma on the stage completed
     }
-    for (int b = 0; b < 2; ++b) mbar_init(&res_full[b], 1);
-    mbar_init(a_full, 1);
-    mbar_init(a_empty, 8);
+    for (int b = 0; b < 2; ++b) {
+      mbar_init(&res_full[b], 1);
+      mbar_init(&turn[b], 4);            // the four warps of the other warpgroup, after their last k-block's wgmma
+    }
+    mbar_init(&a_full[0], 1);
+    mbar_init(&a_full[1], 1);
+    mbar_init(a_empty, 8);               // 8 warp arrivals per m-tile (see the release below)
     fence_mbar_init();
   }
   __syncthreads();
 
   // Producer: the WHOLE warp walks the loops (so that every value is provably warp-uniform and lives in uniform
   // registers) and one elected lane issues the TMA instructions.
-  if (warp == 8) {
-    {
+  if (warp >= 8) {
+    wg_regs_dec<producer_regs(kEpi)>();
+    if (warp == 8) {
       const int n_terms = p.n_terms, taps = p.taps, kw = p.kw, cblocks = p.cblocks;
       PipeState st(stages);
       int res_m = -1;
@@ -221,9 +244,9 @@ __global__ void __launch_bounds__(kThreads, 1)
             res_m = m0;
             mbar_wait(a_empty, (a_seg & 1) ^ 1);
             if (elect_one()) {
-              mbar_arrive_expect_tx(a_full, k_iters * kAStage);
+              mbar_arrive_expect_tx(&a_full[a_seg & 1], k_iters * kAStage);
               for (int ki = 0; ki < k_iters; ++ki)
-                tma_load_2d(smem_ares + ki * kAStage, &maps.a[p.term_a[0]], a_full, ki * kBK, m0, kEvictFirst);
+                tma_load_2d(smem_ares + ki * kAStage, &maps.a[p.term_a[0]], &a_full[a_seg & 1], ki * kBK, m0, kEvictFirst);
             }
             __syncwarp();
             ++a_seg;
@@ -273,34 +296,33 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
     }
   } else {
+    wg_regs_inc<consumer_regs(kEpi)>();
     const uint32_t ewarp = warp;                   // 0..7
     const uint32_t quad = warp & 3;                // rows quad*32 .. +31 of the tile
-    const uint32_t half = ewarp >> 2;              // which half of the tile's columns (= warpgroup)
+    const uint32_t wg = ewarp >> 2;                // consumer warpgroup
     const uint32_t row = quad * 32 + lane;
     const uint32_t etid = ewarp * 32 + lane;       // 0..255 among the consumer threads
+    const uint32_t gtid = etid & 127;              // 0..127 within the warpgroup
+    const uint32_t bar_top = 1 + 2 * wg, bar_end = bar_top + 1;   // the warpgroup's named barriers
     const uint32_t xacc = smem_u32(acc_xpose) + warp * kAccXposeWarpBytes;
     const int act = p.act;
-    uint32_t tc = 0;
+    uint32_t tc = 0;                               // tiles this thread's warpgroup has run
     PipeState st(stages);
     const uint32_t a_base = smem_u32(a_res ? smem_ares : smem_ab);
-    const uint32_t b_base = smem_u32(a_res ? smem_ab : smem_ab + kAStage) + half * (BN / 2) * 128;
+    const uint32_t b_base = smem_u32(a_res ? smem_ab : smem_ab + kAStage);
     int res_m_c = -1;
-    uint32_t a_seg = 0;
-    auto load_residual = [&](int tile_idx, uint32_t rbuf) {   // one thread: residual tile -> res_stage[rbuf]
+    const int m_first = t_first < t_end ? tile_m(t_first) : 0;
+    auto load_residual = [&](int tile_idx, uint8_t* dst, uint64_t* bar) {   // one thread: residual tile -> dst
       const int rm0 = tile_m(tile_idx) * kBM;
       const int rn0 = tile_n(tile_idx) * BN;
       int slabs = 0;
       for (int sl = 0; sl < BN / 64; ++sl)
         if (rn0 + sl * 64 < N) ++slabs;
-      mbar_arrive_expect_tx(&res_full[rbuf], slabs * kBM * 128);
+      mbar_arrive_expect_tx(bar, slabs * kBM * 128);
       for (int sl = 0; sl < BN / 64; ++sl)
-        if (rn0 + sl * 64 < N)
-          tma_load_2d(res_stage + rbuf * kStagingBytes + sl * kBM * 128, &maps.res, &res_full[rbuf], rn0 + sl * 64, rm0,
-                         kEvictFirst);
+        if (rn0 + sl * 64 < N) tma_load_2d(dst + sl * kBM * 128, &maps.res, bar, rn0 + sl * 64, rm0, kEvictFirst);
     };
-    if (kTma && has_res && etid == 0 && t_first < t_end) load_residual(t_first, 0);
-    const bool two_out = p.n_out_bufs == 2;
-    const uint32_t sb_addr = smem_u32(sb), out_addr = smem_u32(out_stage), res_addr = smem_u32(res_stage);
+    const uint32_t sb_addr = smem_u32(sb) + (a_res ? 0 : wg * 4 * BN * 4);
     int staged_n0 = -1;
     uint32_t sbsel = 1;
     if (a_res) {   // per-channel affine of every column block, once
@@ -309,53 +331,60 @@ __global__ void __launch_bounds__(kThreads, 1)
         st_shared_f32(sb_addr + c * 4, (p.scale && c < N) ? p.scale[c] : 1.f);
         st_shared_f32(sb_addr + (npad + c) * 4, (p.bias && c < N) ? p.bias[c] : 0.f);
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
+      named_bar_sync(5, 256);
     }
-    for (int tile = t_first; tile < t_end; tile += t_step, ++tc) {
+    if (wg == 1) st.skip(k_iters);                 // the CTA's first tile is warpgroup 0's
+    for (int tile = t_first + static_cast<int>(wg) * t_step; tile < t_end; tile += 2 * t_step, ++tc) {
       const int m0 = tile_m(tile) * kBM;
       const int n0 = tile_n(tile) * BN;
-      uint8_t* ostage = out_stage + (two_out ? (tc & 1) : 0) * kStagingBytes;
-      const uint32_t ostage_addr = out_addr + (two_out ? (tc & 1) : 0) * kStagingBytes;
-      const uint32_t rstage_addr = res_addr + (tc & 1) * kStagingBytes;
-      if constexpr (kTma) {
-        if (etid == 0) {
-          // single output staging tile: it is free once the store of the previous tile has finished READING it (with
-          // two tiles that wait sits before the end-of-tile barrier, see below)
-          if (!two_out) tma_store_wait_read();
-          // prefetch the NEXT tile's residual; its buffer was last read in tile tc-1 (all warps passed that barrier)
-          if (has_res && tile + t_step < t_end) load_residual(tile + t_step, (tc & 1) ^ 1);
-        }
+      uint8_t* ostage = out_stage + wg * kStagingBytes;
+      const uint32_t ostage_addr = smem_u32(ostage);
+      if (kTma && gtid == 0) {
+        // the warpgroup's staging tile is free once its previous store has finished READING it; the residual then lands
+        // in it (the other warpgroup's k-loop hides the load)
+        tma_store_wait_read();
+        if (has_res) load_residual(tile, ostage, &res_full[wg]);
       }
       // Per-channel affine: staged only when the column block changes (tiles are walked m-fastest, so a CTA keeps its
-      // column block for many tiles) into the buffer the previous block did not use -- warps still finishing the
-      // previous tile read the other one.  The barrier is also what orders a single output staging tile's reuse.
+      // column block for many tiles) into the warpgroup's buffer the previous block did not use -- warps still finishing
+      // the previous tile read the other one.  The barrier also orders the staging tile's reuse after the wait above.
       const bool restage = !a_res && n0 != staged_n0;
       if (restage) {
         sbsel ^= 1;
         staged_n0 = n0;
-        for (int c = etid; c < BN; c += 256) {
+        for (int c = gtid; c < BN; c += 128) {
           const int n = n0 + c;
           st_shared_f32(sb_addr + (sbsel * 2 * BN + c) * 4, (p.scale && n < N) ? p.scale[n] : 1.f);
           st_shared_f32(sb_addr + (sbsel * 2 * BN + BN + c) * 4, (p.bias && n < N) ? p.bias[n] : 0.f);
         }
       }
-      if (restage || (kTma && !two_out)) asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (restage || kTma) named_bar_sync(bar_top, 128);
       const uint32_t s_scale = a_res ? sb_addr + n0 * 4 : sb_addr + sbsel * 2 * BN * 4;
       const uint32_t s_bias = s_scale + (a_res ? num_n_tiles * BN : BN) * 4;
-      // ---- main loop: this warpgroup's 128 x BN/2 accumulator over all k-iterations.  The stage of k-iteration i is
+      // ---- main loop: this warpgroup's 128 x BN accumulator over all k-iterations.  The stage of k-iteration i is
       // released once wgmma_wait<1> in iteration i+1 has seen its MMAs complete.
-      bool last_of_m = false;
+      bool a_release = false;
+      uint32_t a_release_cnt = 1;
       if (a_res) {
         const int mt = tile_m(tile);
         if (mt != res_m_c) {
           res_m_c = mt;
-          mbar_wait(a_full, a_seg & 1);
-          ++a_seg;
+          const int seg = mt - m_first;             // the CTA's seg-th m-tile
+          mbar_wait(&a_full[seg & 1], (seg >> 1) & 1);
         }
-        last_of_m = (tile + t_step >= t_end) || tile_m(tile + t_step) != mt;
+        // The resident rows are released by the last MMAs on them: 8 warp arrivals per m-tile, each warpgroup's 4
+        // warps after its own last tile of the m-tile, or 2 each when the m-tile has no tile of the other warpgroup
+        // (tiles are a contiguous range, so the other warpgroup's tiles of this m-tile include a neighbour).
+        const int next = tile + 2 * t_step;
+        a_release = next >= t_end || tile_m(next) != mt;
+        const bool alone = (tile - t_step < t_first || tile_m(tile - t_step) != mt) &&
+                           (tile + t_step >= t_end || tile_m(tile + t_step) != mt);
+        a_release_cnt = alone ? 2 : 1;
       }
-      WgAcc<BN / 2> acc;
-      uint32_t prev_s = 0;
+      if (wg == 1 || tc > 0) mbar_wait(&turn[wg], (wg == 1 ? tc : tc - 1) & 1);
+      WgAcc<BN> acc;
+      // pend[]: the stages of the last kPend k-iterations, oldest first (their wgmma groups may still be in flight)
+      uint32_t pend[kPend] = {};
       for (int ki = 0; ki < k_iters; ++ki, st.next()) {
         const uint32_t s = st.s;
         mbar_wait(&full[s], st.ph);
@@ -365,22 +394,28 @@ __global__ void __launch_bounds__(kThreads, 1)
 #pragma unroll
         for (int k = 0; k < kBK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), (ki | k) != 0);
         wgmma_commit();
-        wgmma_wait<1>();
-        if (ki > 0 && lane == 0) mbar_arrive(&empty[prev_s]);
-        prev_s = s;
+        if (ki == k_iters - 1 && lane == 0) mbar_arrive(&turn[wg ^ 1]);   // hand the tensor core over
+        wgmma_wait<kPend>();
+        if (ki >= kPend && lane == 0) mbar_arrive(&empty[pend[0]]);
+#pragma unroll
+        for (int j = 0; j + 1 < kPend; ++j) pend[j] = pend[j + 1];
+        pend[kPend - 1] = s;
       }
       wgmma_wait<0>();
       acc.fence_regs();
       if (lane == 0) {
-        mbar_arrive(&empty[prev_s]);
-        if (last_of_m) mbar_arrive(a_empty);
+#pragma unroll
+        for (int j = 0; j < kPend; ++j)
+          if (k_iters - kPend + j >= 0) mbar_arrive(&empty[pend[j]]);
+        if (a_release) mbar_arrive_cnt(a_empty, a_release_cnt);
       }
-      if (kTma && has_res) mbar_wait(&res_full[tc & 1], (tc >> 1) & 1);
+      st.skip(k_iters);                            // the other warpgroup's next tile
+      if (kTma && has_res) mbar_wait(&res_full[wg], tc & 1);
       const int m = m0 + static_cast<int>(row);
       const bool row_ok = m < M;
 #pragma unroll
       for (int ci = 0; ci < kChunksPerWarp; ++ci) {
-        const int ch = half * kChunksPerWarp + ci;
+        const int ch = ci;
         uint32_t r[32];
         acc.rows32(ci, r, xacc, lane);
         const int nc = n0 + ch * 32;
@@ -398,12 +433,11 @@ __global__ void __launch_bounds__(kThreads, 1)
         if constexpr (kTma) {
           // this thread's 32 columns live in slab ch/2 at 16-byte chunks (ch&1)*4 .. +3 of row `row` (128B swizzle)
           const uint32_t srow = ostage_addr + (ch >> 1) * kBM * 128 + row * 128;
-          const uint32_t rrow = rstage_addr + (ch >> 1) * kBM * 128 + row * 128;
           const uint32_t sw = row & 7;
           if (has_res) {
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-              const uint4 rv = ld_shared_v4(rrow + ((((ch & 1) * 4 + j) ^ sw) << 4));
+              const uint4 rv = ld_shared_v4(srow + ((((ch & 1) * 4 + j) ^ sw) << 4));   // residual, then output in place
               const uint32_t w[4] = {rv.x, rv.y, rv.z, rv.w};
 #pragma unroll
               for (int e = 0; e < 4; ++e) {
@@ -514,11 +548,8 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
       if constexpr (kTma) {
         fence_proxy_async();   // generic-proxy writes -> visible to the TMA (async proxy)
-        // two output staging tiles: the NEXT tile writes the tile the PREVIOUS store (committed a whole tile ago) reads
-        // from; that read must be over before anyone passes this barrier
-        if (two_out && etid == 0) tma_store_wait_read();
-        asm volatile("bar.sync 2, 256;" ::: "memory");
-        if (etid == 0) {
+        named_bar_sync(bar_end, 128);
+        if (gtid == 0) {
           for (int sl = 0; sl < BN / 64; ++sl)
             if (n0 + sl * 64 < N && m0 < M) tma_store_2d(&maps.out, ostage + sl * kBM * 128, p.out_col_off + n0 + sl * 64, m0);
           tma_store_commit();
@@ -527,7 +558,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
   }
 
-  if (kTma && warp == 0 && lane == 0) tma_store_wait_all();   // etid 0 issued the stores
+  if (kTma && (warp == 0 || warp == 4) && lane == 0) tma_store_wait_all();   // gtid 0 of each warpgroup issued stores
 }
 
 // A-resident mode: plain (non-im2col) single-term GEMMs with several column blocks and K <= 256 -- the wide 1x1
@@ -542,9 +573,9 @@ bool wants_a_resident(const GemmParams& p, int BN, bool im2col, size_t max_smem)
     return false;
   // the resident rows, the all-blocks affine table and the staging tiles must leave at least three W stages; otherwise
   // the layer runs with the default schedule
-  const size_t staging = static_cast<size_t>(BN / 64) * kBM * 128;
+  const size_t staging = static_cast<size_t>(BN / 64) * kBM * 128;   // one per warpgroup
   const size_t need = 1024 + static_cast<size_t>(2) * p.num_n_tiles * BN * 4 + static_cast<size_t>(k_iters_h) * kAStage + 256 +
-                      static_cast<size_t>(1 + (p.res ? 2 : 0)) * staging + kAccXposeBytes + 3 * static_cast<size_t>(BN) * kBK * 2;
+                      2 * staging + kAccXposeBytes + 3 * static_cast<size_t>(BN) * kBK * 2;
   return need <= max_smem;
 }
 
@@ -552,22 +583,14 @@ template <int BN, bool kIm2col, int kEpi>
 int launch(const GemmMaps& maps, GemmParams& p, int num_sms, size_t max_smem, cudaStream_t stream) {
   constexpr int kStageBytes = kAStage + BN * kBK * 2;
   constexpr size_t kStagingBytes = static_cast<size_t>(BN / 64) * kBM * 128;
-  // staging tiles: residual layers get 2 residual + 2 output tiles (prefetch / drain a full tile ahead) when they still
-  // leave >= 3 pipeline stages, otherwise one output tile (plus two residual tiles if needed)
-  p.n_res_bufs = (p.tma_epi && p.res) ? 2 : 0;
-  p.n_out_bufs = p.tma_epi ? 2 : 0;
   const int k_iters_h = p.n_terms * p.taps * p.cblocks;
   p.a_resident = (kEpi != 0 && wants_a_resident(p, BN, kIm2col, max_smem)) ? 1 : 0;
-  const size_t sb_bytes = p.a_resident ? static_cast<size_t>(2) * p.num_n_tiles * BN * 4 : static_cast<size_t>(4) * BN * 4;
+  const size_t sb_bytes = p.a_resident ? static_cast<size_t>(2) * p.num_n_tiles * BN * 4 : static_cast<size_t>(8) * BN * 4;
   const size_t ares_bytes = p.a_resident ? static_cast<size_t>(k_iters_h) * kAStage : 0;
-  auto fixed_for = [&](int nout, int nres) {
-    return 1024 + sb_bytes + ares_bytes + 256 + static_cast<size_t>(nout + nres) * kStagingBytes + (p.tma_epi ? 0 : kXposeBytes) +
-           kAccXposeBytes;
-  };
+  // one output staging tile per warpgroup (TMA-store epilogue) or the per-warp transpose buffers (direct epilogue)
+  const size_t fixed = 1024 + sb_bytes + ares_bytes + 256 + (p.tma_epi ? 2 * kStagingBytes : kXposeBytes) + kAccXposeBytes;
   const size_t stage_bytes = p.a_resident ? static_cast<size_t>(BN) * kBK * 2 : static_cast<size_t>(kStageBytes);
-  if (p.tma_epi && (fixed_for(p.n_out_bufs, p.n_res_bufs) + 3 * stage_bytes > max_smem)) p.n_out_bufs = 1;
-  const size_t fixed = fixed_for(p.n_out_bufs, p.n_res_bufs);
-  DCR_REQUIRE(max_smem > fixed + 2 * stage_bytes, "gemm: not enough shared memory");
+  DCR_REQUIRE(max_smem > fixed + 3 * stage_bytes, "gemm: not enough shared memory");   // kPend + 1 stages at least
   int stages = static_cast<int>((max_smem - fixed) / stage_bytes);
   stages = std::min(stages, 8);
   p.stages = stages;
@@ -621,15 +644,17 @@ int conv_gemm(const ConvGemmDesc& d, cudaStream_t stream) {
     w_planes = std::max(w_planes, d.term_w[t] + 1);
   }
   DCR_REQUIRE(a_planes <= 3 && w_planes <= 3, "conv_gemm: at most 3 planes");
-  int BN = d.N <= 64 ? 64 : (d.N <= 128 ? 128 : 256);
-  // memory-bound shapes (residual epilogue, or little K per output) favour 128-wide tiles: their staging tiles can be
-  // double buffered; compute-bound shapes keep 256 (fewer re-reads of A)
-  const bool single_plane = d.out && d.out_planes <= 1 && !d.out_f32 && (!d.res || d.res_planes <= 1);
-  if (BN == 256 && single_plane && (d.res != nullptr || static_cast<long long>(d.kh) * d.kw * d.C <= 256)) BN = 128;
-  // (256-wide tiles for the long-K residual layers -- ResNet layer4 expansions, K = 512 -- were tried in round 2: the output
-  // and residual staging tiles of a 128 x 256 tile do not fit beside three pipeline stages)
-  // few output tiles and a long K (the SSCD head: 256 x 512 x 2048 is four 128 x 256 tiles, each CTA streaming 1.5 MB through
-  // one SM's L2 port: 22 us): narrower tiles put more CTAs -- more L2 ports -- on the same K stream
+  // at most 128 columns: a warpgroup holds a whole 128 x 128 tile (128 accumulator registers per thread).  Two 128-wide
+  // ping-pong tiles beat one 128 x 256 tile split over both warpgroups on every 256-wide shape of SSCD ResNet-50 and DINO
+  // ViT-S (ResNet layer3/4 3x3 and reduces, ViT qkv / fc1; DESIGN.md section 2): the epilogue no longer stalls the tensor
+  // core, which outweighs reading A twice as often
+  int BN = d.N <= 64 ? 64 : 128;
+  // QuickGELU divides by 1 + exp(-1.702 y) in IEEE single precision, whose rare-operand path is a subroutine call: with
+  // a 128-column accumulator live across 32 such calls per chunk ptxas spills, so QuickGELU layers (CLIP) take 64-column
+  // tiles
+  if (d.act == 3) BN = 64;
+  // few output tiles and a long K (the SSCD head: 384 x 512 x 2048 is twelve 128 x 128 tiles, each CTA streaming its K
+  // through one SM's L2 port): narrower tiles put more CTAs -- more L2 ports -- on the same K stream
   {
     const long long m_tiles = (M + kBM - 1) / kBM;
     while (BN > 64 && ktot >= 1024 && m_tiles * ((d.N + BN - 1) / BN) * 4 <= di->num_sms) BN /= 2;
@@ -715,11 +740,10 @@ int conv_gemm(const ConvGemmDesc& d, cudaStream_t stream) {
           : launch<BNv, false, E>(maps, p, di->num_sms, di->max_smem_optin, stream))
 #define DCR_LAUNCH(BNv)                                                                          \
   (epi == 0 ? DCR_LAUNCH_E(BNv, 0)                                                                \
-            : (epi == 1 ? DCR_LAUNCH_E(BNv, 1) : (epi == 2 ? DCR_LAUNCH_E(BNv, 2) : (epi == 3 ? DCR_LAUNCH_E(BNv, 3) : DCR_LAUNCH_E(BNv, 4)))))
+            : (epi == 1 ? DCR_LAUNCH_E(BNv, 1) : (epi == 2 ? DCR_LAUNCH_E(BNv, 2) : (epi == 3 ? DCR_LAUNCH_E(BNv, 3) : DCR_LAUNCH_E(64, 4)))))
   switch (BN) {
     case 64: return DCR_LAUNCH(64);
     case 128: return DCR_LAUNCH(128);
-    case 256: return DCR_LAUNCH(256);
     default: return set_error(-1, "conv_gemm: unsupported BN %d", BN);
   }
 #undef DCR_LAUNCH_E

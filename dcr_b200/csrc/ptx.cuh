@@ -31,6 +31,9 @@ DCR_DEVICE void fence_proxy_async() { asm volatile("fence.proxy.async.shared::ct
 DCR_DEVICE void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+DCR_DEVICE void mbar_arrive_cnt(uint64_t* bar, uint32_t count) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
 DCR_DEVICE void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -68,7 +71,23 @@ struct PipeState {
       ph ^= 1;
     }
   }
+  // past the k ring positions another consumer takes (ping-pong schedules: the other warpgroup's tile)
+  DCR_DEVICE void skip(int k) {
+    for (int i = 0; i < k; ++i) next();
+  }
 };
+
+// Register reallocation between warpgroups (executed by all warps of a warpgroup): the producer warpgroup gives registers
+// back so that the consumer warpgroups can hold a 128 x 128 fp32 accumulator and its epilogue without spilling.
+template <int kRegs>
+DCR_DEVICE void wg_regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <int kRegs>
+DCR_DEVICE void wg_regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+
+// named barrier among `threads` threads (a warpgroup: 128, both consumer warpgroups: 256)
+DCR_DEVICE void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 // ----------------------------------------------------------------------------------------------
 // TMA
