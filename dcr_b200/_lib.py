@@ -74,6 +74,11 @@ SIGNATURES = {
                                     C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dcr_topk_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                  C.c_void_p]),
+    "dcr_image_stats": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dcr_jpeg_workspace_size": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "dcr_jpeg_max_bytes": (C.c_int64, [C.c_int, C.c_int]),
+    "dcr_jpeg_encode": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_size_t, C.c_void_p]),
 }
 
 # the all-gather callback of dcr_sim_topk_sharded / dcr_sim_range_sharded: int (*)(const void* send, void* recv, size_t bytes_per_rank, void* ctx, void* stream)

@@ -5,8 +5,9 @@
 
 What it does is the `if args.rank == 0:` block diff_retrieval.py:375-483 restricted to the hot path: embed both folders,
 L2-normalise, top-1 (and top-`num_matches`... the reference hard-codes top-10 for its galleries, :621) matches, background
-top-2, the printed statistics dictionary, and optionally FID (:597-600).  Plots, CLIP score, complexity statistics and
-wandb are out of scope (DESIGN.md section 9).  Flags that the reference parses but never reads are accepted and ignored.
+top-2, the printed statistics dictionary, optionally FID (:597-600) and, with --complexity, the match-complexity
+statistics (:497-540).  Plots, CLIP score and wandb are out of scope (DESIGN.md section 1).  Flags that the reference
+parses but never reads are accepted and ignored.
 """
 from __future__ import annotations
 
@@ -70,6 +71,10 @@ def build_parser() -> argparse.ArgumentParser:
                         "gallery self-join): sparse CSR in place of the reference's similarity*.pth matrices; "
                         "--sim_threshold=-inf gives every pair.  Dot-product metric, one process")
     p.add_argument("--fid_weights", default="", type=str, help="pt_inception-2015-12-05 state_dict; enables FID")
+    p.add_argument("--complexity", action="store_true",
+                   help="entropy, quality-90 JPEG size and total variation of every top-1 training match: writes "
+                        "entropies.pth, totvar.pth, compressions.pth and dbsims.pth and adds their Pearson correlations "
+                        "with the top-1 similarity (cc_* / pval_*) to stats.json")
     return p
 
 
@@ -248,6 +253,16 @@ def main_worker(gpu, ngpus_per_node, args) -> int:
                 fid_val = fid.fid_from_images(inc, fid.load_resized(args.val_dir), fid.load_resized(args.query_dir))   # :597-600
             print({"fid": fid_val})
             out["stats"]["fid"] = fid_val
+        if args.complexity:                                                                   # :497-540
+            from . import complexity
+            cx = complexity.top1_complexity(v_files, out["indices"][:, 0].cpu().numpy(),
+                                            out["values"][:, 0].cpu().numpy(), workers=args.workers)
+            for key, name in (("entropies", "entropies.pth"), ("totvar", "totvar.pth"),
+                              ("compressions", "compressions.pth"), ("dbsims", "dbsims.pth")):
+                torch.save(cx[key], os.path.join(save, name))
+            corr = {k: cx[k] for k in complexity.CORRELATION_KEYS}
+            print(corr)
+            out["stats"].update(corr)
         with open(os.path.join(save, "stats.json"), "w") as f:
             json.dump(out["stats"], f)
     if args.distributed:

@@ -310,4 +310,15 @@ int dcr_fid_merge(dcr_fid* st, const void* packed, int count, void* stream) {
   return dcr::fid_merge(reinterpret_cast<dcr::FidState*>(st), packed, count, as_stream(stream));
 }
 
+int dcr_image_stats(const uint8_t* images, int n, int h, int w, double* out_entropy, int64_t* out_tv, void* stream) {
+  return dcr::image_stats(images, n, h, w, out_entropy, reinterpret_cast<long long*>(out_tv), as_stream(stream));
+}
+size_t dcr_jpeg_workspace_size(int n, int h, int w) { return dcr::jpeg_workspace_size(n, h, w); }
+int64_t dcr_jpeg_max_bytes(int h, int w) { return dcr::jpeg_max_bytes(h, w); }
+int dcr_jpeg_encode(const uint8_t* images, int n, int h, int w, int quality, int64_t* out_sizes, uint8_t* out_bytes,
+                    void* workspace, size_t workspace_bytes, void* stream) {
+  return dcr::jpeg_encode(images, n, h, w, quality, reinterpret_cast<long long*>(out_sizes), out_bytes, workspace,
+                          workspace_bytes, as_stream(stream));
+}
+
 }  // extern "C"

@@ -53,6 +53,14 @@ int pad_topk_lists(const float* s_in, const long long* i_in, int nq, int k_in, i
 int topk_merge(const float* scores, const long long* idx, int nq, int nlists, int k_in, int k_out, float* out_scores,
                long long* out_idx, cudaStream_t stream);
 
+// complexity.cu: grey-level entropy, total variation and baseline-JPEG size of uint8 HWC images
+int image_stats(const unsigned char* images, int n, int h, int w, double* out_entropy, long long* out_tv,
+                cudaStream_t stream);
+size_t jpeg_workspace_size(int n, int h, int w);
+long long jpeg_max_bytes(int h, int w);
+int jpeg_encode(const unsigned char* images, int n, int h, int w, int quality, long long* out_sizes,
+                unsigned char* out_bytes, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+
 
 // ---- wgmma GEMM / implicit-GEMM convolution (conv_gemm.cu) ---------------------------------------------------
 constexpr int kMaxGemmTerms = 6;

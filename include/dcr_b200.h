@@ -304,6 +304,32 @@ size_t dcr_fid_packed_size(int d);
 int dcr_fid_export(const dcr_fid* st, void* packed, void* stream);
 int dcr_fid_merge(dcr_fid* st, const void* packed, int count, void* stream);
 
+/* ---- match complexity ------------------------------------------------------------------------------------------- */
+/* images: DEVICE uint8 [n, h, w, 3] (HWC), the array the reference hands to skimage and cv2.  n = 0 is a no-op.
+ * Replaces   entropy(img_as_ubyte(color.rgb2gray(rgbImg)))          diff_retrieval.py:508
+ *            tv_loss(torchim)                                         diff_retrieval.py:113-122, 516
+ * out_entropy[n] (DEVICE fp64): sklearn's entropy of the grey levels, u = rint(((c0/255)*0.2125 + (c1/255)*0.7154)
+ *   + (c2/255)*0.0721) * 255) in fp64, each operation rounded on its own (DESIGN.md, "Match complexity").
+ * out_tv[n][2] (DEVICE int64): h = sum |img[y+1,x,c] - img[y,x,c]|, w = sum |img[y,x+1,c] - img[y,x,c]|; the
+ *   reference's value is 1e-4 * (h + w).  1 <= h * w <= 2^26. */
+int dcr_image_stats(const uint8_t* images, int n, int h, int w, double* out_entropy, int64_t* out_tv, void* stream);
+
+/* Baseline JPEG, byte for byte what cv2.imencode('.jpg', a, [IMWRITE_JPEG_QUALITY, quality]) (libjpeg-turbo) writes
+ * for the array a as given -- which cv2 reads as BGR, so channel 2 is red:
+ *   4:2:0, islow DCT, Annex K Huffman tables, JFIF APP0, no restart interval; a 623-byte header at every quality.
+ * Replaces   cv2.imencode('.jpg', rgbImg, encode_param); len(encimg)   diff_retrieval.py:513-515
+ * h and w: multiples of 16 in 16..4096 (other sizes need libjpeg's edge replication and are refused); quality 1..100.
+ * dcr_jpeg_max_bytes(h, w): a bound on the file size (header, every scan byte stuffed, EOI; a multiple of 16), the
+ *   stride of out_bytes.  < 0 on a refused size.
+ * dcr_jpeg_workspace_size(n, h, w): DEVICE workspace bytes for n images per call (per-block DC and bit offsets and a
+ *   bit buffer per image; no coefficient array).  0 on a refused size.
+ * dcr_jpeg_encode: out_sizes[n] (DEVICE int64) the file sizes; out_bytes (DEVICE [n][dcr_jpeg_max_bytes], or NULL for
+ *   sizes only) the files.  Deterministic: the same bytes on every call and for every split of a batch into calls. */
+size_t dcr_jpeg_workspace_size(int n, int h, int w);
+int64_t dcr_jpeg_max_bytes(int h, int w);
+int dcr_jpeg_encode(const uint8_t* images, int n, int h, int w, int quality, int64_t* out_sizes, uint8_t* out_bytes,
+                    void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
