@@ -223,11 +223,6 @@ DCR_DEVICE float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-DCR_DEVICE uint32_t pack_bf16x2(float lo, float hi) {
-  uint32_t w;
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(w) : "f"(hi), "f"(lo));   // upper half <- first source
-  return w;
-}
 // running maximum over one 32-column chunk of a score row; columns >= lim are not part of the row
 DCR_DEVICE float chunk_max(const uint32_t (&r)[32], int c0, int lim, float mx) {
   if (c0 + 32 <= lim) {
@@ -244,7 +239,7 @@ DCR_DEVICE float chunk_max(const uint32_t (&r)[32], int c0, int lim, float mx) {
 __global__ void __launch_bounds__(kAttnTcThreads, 1)
     attention_tc_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnTcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   uint8_t* s_q = smem;                 // [128 x 64] bf16
   uint8_t* s_k = s_q + 16384;          // [256 x 64]
   uint8_t* s_v = s_k + 32768;          // [256 x 64]
@@ -398,33 +393,20 @@ int attention(const __nv_bfloat16* qkv, long long qkv_plane_stride, __nv_bfloat1
     AttnTcParams tp;
     tp.out = out; tp.B = B; tp.T = T; tp.heads = heads; tp.causal = causal;
     tp.scale_log2e = scale * 1.4426950408889634f;
-    DCR_CUDA_CHECK(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(kAttnTcSmem)));
-    attention_tc_kernel<<<B * heads * ((T + 127) / 128), kAttnTcThreads, kAttnTcSmem, stream>>>(tm, tp);
-    count_launch();
-    DCR_CUDA_CHECK(cudaGetLastError());
-    return 0;
+    return launch(attention_tc_kernel, B * heads * ((T + 127) / 128), kAttnTcThreads, kAttnTcSmem, stream, "attention",
+                  tm, tp);
   }
   AttnParams p;
   p.qkv = qkv; p.qkv_plane_stride = qkv_plane_stride; p.out = out; p.out_plane_stride = out_plane_stride;
   p.planes = planes; p.B = B; p.T = T; p.heads = heads; p.dh = dh; p.scale = scale; p.causal = causal;
   if (T > 256) {   // K / V streamed in tiles, online softmax (patch-8 ViTs)
     const size_t smem_s = (static_cast<size_t>(kStreamK) * 65 + kStreamK * 64 + kStreamQ * 64 + 8 * kStreamK) * 4;
-    DCR_CUDA_CHECK(cudaFuncSetAttribute(attention_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(smem_s)));
-    attention_stream_kernel<<<dim3(B * heads, (T + kStreamQ - 1) / kStreamQ), 256, smem_s, stream>>>(p);
-    count_launch();
-    DCR_CUDA_CHECK(cudaGetLastError());
-    return 0;
+    return launch(attention_stream_kernel, dim3(B * heads, (T + kStreamQ - 1) / kStreamQ), 256, smem_s, stream, "attention",
+                  p);
   }
   const int Tpad = (T + 31) / 32 * 32;
   const size_t smem = (static_cast<size_t>(T) * 65 + static_cast<size_t>(T) * 64 + 8 * 64 + 8 * Tpad) * 4;
-  DCR_CUDA_CHECK(cudaFuncSetAttribute(attention_fp32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      static_cast<int>(smem)));
-  attention_fp32_kernel<<<B * heads, 256, smem, stream>>>(p);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(attention_fp32_kernel, B * heads, 256, smem, stream, "attention", p);
 }
 
 }  // namespace dcr

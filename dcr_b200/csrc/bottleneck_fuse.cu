@@ -63,20 +63,6 @@ struct FuseParams {
   const float* bias1;
 };
 
-DCR_DEVICE uint32_t pack2(float a, float b) {
-  __nv_bfloat162 p = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&p);
-}
-DCR_DEVICE void store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-DCR_DEVICE void store_wait_read_1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
-DCR_DEVICE void store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-DCR_DEVICE void tma_store_2d_(const void* tmap, uint32_t src_smem, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tmap)),
-               "r"(src_smem), "r"(c0), "r"(c1)
-               : "memory");
-}
-
 // N2 = 0: expansion only (no following reduce convolution to fuse with) -- the same in-place residual / three rotating
 // tile pipeline for the 1x1 expansions whose separate staging tiles do not fit beside the resident A rows in conv_gemm.cu
 // (K = 256: layer3 of the ResNet-50, where that kernel has to serialise on a single output staging tile).
@@ -85,7 +71,7 @@ __global__ void __launch_bounds__(kFThreads, 1) expand_reduce_kernel(const __gri
   static_assert(N2 == 0 || N2 == 64 || N2 == 128, "second GEMM width");
   constexpr bool kSecond = N2 != 0;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   const int k_iters1 = p.k_iters1, nb = p.nb;
   const int a_buf_bytes = k_iters1 * kSlab;
   uint8_t* smem_a = smem;                                           // a_bufs x k_iters1 slabs
@@ -213,7 +199,7 @@ __global__ void __launch_bounds__(kFThreads, 1) expand_reduce_kernel(const __gri
           const bool has_next = (j + 1 < nb) || (tile + static_cast<int>(gridDim.x) < num_m_tiles);
           if (has_next) {
             const uint32_t xn = (xb + 1 == kXBufs) ? 0 : xb + 1;
-            if (g >= 2) store_wait_read_1();
+            if (g >= 2) tma_store_wait_read<1>();
             const int nm0 = (j + 1 < nb) ? m0 : (tile + static_cast<int>(gridDim.x)) * kFM;
             const int nn0 = (j + 1 < nb) ? (j + 1) * kFN : 0;
             mbar_arrive_expect_tx(&r_full[xn], kXTile);
@@ -239,14 +225,14 @@ __global__ void __launch_bounds__(kFThreads, 1) expand_reduce_kernel(const __gri
           float y0 = fmaf(v0, sc.x, bi.x), y1 = fmaf(v1, sc.y, bi.y);
           y0 += __uint_as_float(w << 16);
           y1 += __uint_as_float(w & 0xffff0000u);
-          st_shared_u32(addr, pack2(fmaxf(y0, 0.f), fmaxf(y1, 0.f)));
+          st_shared_u32(addr, pack_bf16x2(fmaxf(y0, 0.f), fmaxf(y1, 0.f)));
         });
         fence_proxy_async();   // generic-proxy writes -> visible to the TMA store and to wgmma (async proxy)
         asm volatile("bar.sync 2, 256;" ::: "memory");
         if (etid == 0) {
           for (int sl = 0; sl < 2; ++sl)
-            tma_store_2d_(&maps.out, x_addr + xb * kXTile + sl * kSlab, j * kFN + sl * kFK, m0);
-          store_commit();
+            tma_store_2d(&maps.out, x_addr + xb * kXTile + sl * kSlab, j * kFN + sl * kFK, m0);
+          tma_store_commit();
         }
         if constexpr (kSecond) {   // second GEMM: acc2 += Y block j (in place in X buffer xb) x W1 slabs
           for (int sl = 0; sl < 2; ++sl)
@@ -255,7 +241,7 @@ __global__ void __launch_bounds__(kFThreads, 1) expand_reduce_kernel(const __gri
       }
       if constexpr (!kSecond) continue;
       // ---- T1 tile of this m-tile: acc2 -> BN + ReLU -> bf16 -> staging -> TMA store ----
-      if (etid == 0) store_wait_read_1();   // the previous m-tile's T1 store has finished reading the staging slabs
+      if (etid == 0) tma_store_wait_read<1>();   // the previous m-tile's T1 store has finished reading the staging slabs
       asm volatile("bar.sync 1, 256;" ::: "memory");
       {
         const uint32_t s_scale2 = sb_addr + 2 * N1 * 4;
@@ -264,17 +250,17 @@ __global__ void __launch_bounds__(kFThreads, 1) expand_reduce_kernel(const __gri
           const uint32_t rr = quad * 32 + r, c = half * (N2 / 2) + cl;
           const float2 sc = ld_shared_f2(s_scale2 + c * 4), bi = ld_shared_f2(s_bias2 + c * 4);
           const uint32_t addr = o2_addr + (c >> 6) * kSlab + rr * 128 + ((((c & 63) >> 3) ^ (rr & 7)) << 4) + (c & 7) * 2;
-          st_shared_u32(addr, pack2(fmaxf(fmaf(v0, sc.x, bi.x), 0.f), fmaxf(fmaf(v1, sc.y, bi.y), 0.f)));
+          st_shared_u32(addr, pack_bf16x2(fmaxf(fmaf(v0, sc.x, bi.x), 0.f), fmaxf(fmaf(v1, sc.y, bi.y), 0.f)));
         });
       }
       fence_proxy_async();
       asm volatile("bar.sync 2, 256;" ::: "memory");
       if (etid == 0) {
-        for (int sl = 0; sl < N2 / 64; ++sl) tma_store_2d_(&maps.out2, o2_addr + sl * kSlab, sl * kFK, m0);
-        store_commit();
+        for (int sl = 0; sl < N2 / 64; ++sl) tma_store_2d(&maps.out2, o2_addr + sl * kSlab, sl * kFK, m0);
+        tma_store_commit();
       }
     }
-    if (etid == 0) store_wait_all();
+    if (etid == 0) tma_store_wait_all();
   }
 
 }
@@ -311,28 +297,11 @@ bool expand_reduce_eligible(const ConvGemmDesc& a, const ConvGemmDesc& b, size_t
   return need <= max_smem;
 }
 
-namespace {
-template <int N2>
-int launch_fused(const FuseMaps& maps, const FuseParams& p, int grid, size_t smem, const DeviceInfo* di, cudaStream_t stream) {
-  static bool attr_set[64] = {};
-  if (!attr_set[di->device & 63]) {
-    DCR_CUDA_CHECK(cudaFuncSetAttribute(expand_reduce_kernel<N2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(di->max_smem_optin)));
-    attr_set[di->device & 63] = true;
-  }
-  expand_reduce_kernel<N2><<<grid, kFThreads, smem, stream>>>(maps, p);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
-}  // namespace
-
 // b == nullptr: expansion only
 static int expand_reduce_impl(const ConvGemmDesc& a, const ConvGemmDesc* b, cudaStream_t stream) {
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  DCR_REQUIRE(di->cc_major == 9 && di->cc_minor == 0, "expand_reduce: this build targets sm_90a; device reports sm_%d%d", di->cc_major,
-              di->cc_minor);
+  if (int rc = require_sm90a(di, "expand_reduce")) return rc;
   const long long M = static_cast<long long>(a.B) * a.H * a.W;
   DCR_REQUIRE(M > 0 && M < (1ll << 31), "expand_reduce: M out of range");
   const int n2 = b ? b->N : 0;
@@ -367,9 +336,9 @@ static int expand_reduce_impl(const ConvGemmDesc& a, const ConvGemmDesc* b, cuda
   DCR_REQUIRE(p.w_stages >= 3, "expand_reduce: not enough shared memory");
   const size_t smem = fixed + p.a_bufs * a_buf + static_cast<size_t>(p.w_stages) * kWStage;
   const int grid = std::min(p.num_m_tiles, di->num_sms);
-  if (n2 == 0) return launch_fused<0>(maps, p, grid, smem, di, stream);
-  if (n2 == 64) return launch_fused<64>(maps, p, grid, smem, di, stream);
-  return launch_fused<128>(maps, p, grid, smem, di, stream);
+  if (n2 == 0) return launch(expand_reduce_kernel<0>, grid, kFThreads, smem, stream, "expand_reduce", maps, p);
+  if (n2 == 64) return launch(expand_reduce_kernel<64>, grid, kFThreads, smem, stream, "expand_reduce", maps, p);
+  return launch(expand_reduce_kernel<128>, grid, kFThreads, smem, stream, "expand_reduce", maps, p);
 }
 
 int expand_reduce(const ConvGemmDesc& a, const ConvGemmDesc& b, cudaStream_t stream) {

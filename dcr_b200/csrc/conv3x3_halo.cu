@@ -61,21 +61,13 @@ struct HaloParams {
   int act, out_col_off;
 };
 
-DCR_DEVICE void tma_store_commit_() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-DCR_DEVICE void tma_store_wait_read_() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-DCR_DEVICE void tma_store_wait_all_() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-DCR_DEVICE uint32_t pack_bf16_(float a, float b) {
-  __nv_bfloat162 p = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&p);
-}
-
 // kRW: ALL filter taps stay resident in shared memory (9 * cblocks tiles of [BN x 64]; fits for the 64 -> 64 convolutions of
 // ResNet layer1: 72 KB): no weight ring, the producer only streams halo boxes.
 template <int BN, bool kRW>
 __global__ void __launch_bounds__(kHThreads, 1)
     conv3x3_halo_kernel(const __grid_constant__ HaloMaps maps, const HaloParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   constexpr int kWStage = BN * 128;
   constexpr int kStageBytes = (BN / 64) * kSlabBytes;                       // one output staging box
   uint8_t* a_ring = smem;
@@ -87,7 +79,7 @@ __global__ void __launch_bounds__(kHThreads, 1)
   uint64_t* a_empty = bars + 4;     // [4]
   uint64_t* w_full = bars + 8;      // [8]
   uint64_t* w_empty = bars + 16;    // [8]
-  uint64_t* turn = bars + 24;       // [2] turn[g] completes when warpgroup g may start its k-loop
+  uint64_t* turn = bars + 24;       // [2] PingPong::turn
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
@@ -183,13 +175,14 @@ __global__ void __launch_bounds__(kHThreads, 1)
       as.skip(p.cblocks);
       if constexpr (!kRW) ws.skip(k_groups);
     }
+    const PingPong pingpong{turn};
     uint32_t tc = 0;
     for (int tile = blockIdx.x + wg * gridDim.x; tile < p.num_tiles; tile += 2 * gridDim.x, ++tc) {
       const int b = tile / p.tiles_per_img;
       const int p0 = (tile - b * p.tiles_per_img) * p.R;
-      if (gtid == 0) tma_store_wait_read_();     // this warpgroup's previous store has finished reading its staging box
+      if (gtid == 0) tma_store_wait_read<0>();     // this warpgroup's previous store has finished reading its staging box
       named_bar_sync(1 + 2 * wg, 128);
-      if (wg == 1 || tc > 0) mbar_wait(&turn[wg], (wg == 1 ? tc : tc - 1) & 1);
+      pingpong.wait(wg, tc);
       // main loop: per channel block one halo box, nine taps = nine start addresses into it.  Group (cb, tap)'s operands
       // are released once wgmma_wait<1> after the next group has seen it complete.
       WgAcc<BN> acc;
@@ -217,7 +210,7 @@ __global__ void __launch_bounds__(kHThreads, 1)
           for (int k = 0; k < kHK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), (cb | tap | k) != 0);
           wgmma_commit();
           const bool last = cb == p.cblocks - 1 && tap == 8;
-          if (last && lane == 0) mbar_arrive(&turn[wg ^ 1]);   // hand the tensor core over
+          if (last && lane == 0) pingpong.hand_over(wg);
           wgmma_wait<1>();
           if ((cb | tap) != 0 && lane == 0) {
             if constexpr (!kRW) mbar_arrive(&w_empty[prev_w]);
@@ -251,16 +244,16 @@ __global__ void __launch_bounds__(kHThreads, 1)
         const uint32_t chunk = (col & 63) >> 3;
         if (valid[g])
           st_shared_u32(stage_addr + (col >> 6) * kSlabBytes + srow[g] * 128 + ((chunk ^ (srow[g] & 7)) << 4) + c0 * 2,
-                        pack_bf16_(y0, y1));
+                        pack_bf16x2(y0, y1));
       });
       fence_proxy_async();
       named_bar_sync(2 + 2 * wg, 128);
       if (gtid == 0) {
-        for (int sl = 0; sl < BN / 64; ++sl) tma_store_4d(&maps.out, ostage + sl * kSlabBytes, p.out_col_off + sl * 64, 0, p0, b);
-        tma_store_commit_();
+        for (int sl = 0; sl < BN / 64; ++sl) tma_store_4d(&maps.out, smem_u32(ostage + sl * kSlabBytes), p.out_col_off + sl * 64, 0, p0, b);
+        tma_store_commit();
       }
     }
-    if (gtid == 0) tma_store_wait_all_();
+    if (gtid == 0) tma_store_wait_all();
   }
 }
 
@@ -287,19 +280,8 @@ int launch_halo(const HaloMaps& maps, HaloParams& p, int num_sms, size_t max_sme
     }
     smem = fixed + static_cast<size_t>(p.a_bufs) * abuf + static_cast<size_t>(p.w_stages) * kWStage;
   }
-  auto kern = conv3x3_halo_kernel<BN, kRW>;
-  static bool attr_set_dev[64] = {};   // per template instantiation and device (the attribute is per device)
-  int cur_dev = 0;
-  DCR_CUDA_CHECK(cudaGetDevice(&cur_dev));
-  bool& attr_set = attr_set_dev[cur_dev & 63];
-  if (!attr_set) {
-    DCR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(max_smem)));
-    attr_set = true;
-  }
-  kern<<<std::min(p.num_tiles, num_sms), kHThreads, smem, stream>>>(maps, p);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(conv3x3_halo_kernel<BN, kRW>, std::min(p.num_tiles, num_sms), kHThreads, smem, stream, "conv3x3_halo",
+                maps, p);
 }
 
 }  // namespace

@@ -126,21 +126,6 @@ DCR_DEVICE float apply_act(float y, int act) {
   return y;
 }
 
-DCR_DEVICE uint32_t pack_bf16(float a, float b) {
-  __nv_bfloat162 p = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&p);
-}
-
-DCR_DEVICE void tma_store_2d(const void* tmap, const void* src_smem, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tmap)),
-               "r"(smem_u32(src_smem)), "r"(c0), "r"(c1)
-               : "memory");
-}
-DCR_DEVICE void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-DCR_DEVICE void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-DCR_DEVICE void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
 // kEpi: 0 = direct epilogue (any number of planes, optional fp32 output, runtime activation; parity mode and final
 //           layers), 1/2/3/4 = TMA-store epilogue with compile-time activation none / ReLU / GELU / QuickGELU (fast mode hot path).
 // Eight MMA + epilogue warps: warp w of a warpgroup owns rows 32w .. 32w+31 of the warpgroup's accumulator tile.
@@ -148,7 +133,7 @@ template <int BN, bool kIm2col, int kEpi>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm_bf16_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   constexpr bool kTma = kEpi != 0;
   constexpr int kBStage = BN * kBK * 2;
   constexpr int kStageBytes = kAStage + kBStage;
@@ -176,7 +161,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   uint64_t* full = bars;          // [stages] (<= 12)
   uint64_t* empty = bars + 12;    // [stages]
   uint64_t* res_full = bars + 28;   // [2]  one per warpgroup
-  uint64_t* turn = bars + 30;       // [2]  ping-pong hand-off: turn[g] completes when warpgroup g may start its k-loop
+  uint64_t* turn = bars + 30;       // [2]  PingPong::turn
   // A-resident mode (stages <= 8, so full[9..11] are free): a_full[j & 1] completes when the rows of the CTA's j-th
   // m-tile have landed.  Two barriers, because a ping-pong warpgroup may have no tile in the CTA's first m-tile and then
   // waits for the second one: on a single barrier that parity would also match the not-yet-completed first phase.  Only
@@ -307,6 +292,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     const uint32_t xacc = smem_u32(acc_xpose) + warp * kAccXposeWarpBytes;
     const int act = p.act;
     uint32_t tc = 0;                               // tiles this thread's warpgroup has run
+    const PingPong pingpong{turn};
     PipeState st(stages);
     const uint32_t a_base = smem_u32(a_res ? smem_ares : smem_ab);
     const uint32_t b_base = smem_u32(a_res ? smem_ab : smem_ab + kAStage);
@@ -342,7 +328,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       if (kTma && gtid == 0) {
         // the warpgroup's staging tile is free once its previous store has finished READING it; the residual then lands
         // in it (the other warpgroup's k-loop hides the load)
-        tma_store_wait_read();
+        tma_store_wait_read<0>();
         if (has_res) load_residual(tile, ostage, &res_full[wg]);
       }
       // Per-channel affine: staged only when the column block changes (tiles are walked m-fastest, so a CTA keeps its
@@ -381,7 +367,7 @@ __global__ void __launch_bounds__(kThreads, 1)
                            (tile + t_step >= t_end || tile_m(tile + t_step) != mt);
         a_release_cnt = alone ? 2 : 1;
       }
-      if (wg == 1 || tc > 0) mbar_wait(&turn[wg], (wg == 1 ? tc : tc - 1) & 1);
+      pingpong.wait(wg, tc);
       WgAcc<BN> acc;
       // pend[]: the stages of the last kPend k-iterations, oldest first (their wgmma groups may still be in flight)
       uint32_t pend[kPend] = {};
@@ -394,7 +380,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 #pragma unroll
         for (int k = 0; k < kBK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), (ki | k) != 0);
         wgmma_commit();
-        if (ki == k_iters - 1 && lane == 0) mbar_arrive(&turn[wg ^ 1]);   // hand the tensor core over
+        if (ki == k_iters - 1 && lane == 0) pingpong.hand_over(wg);
         wgmma_wait<kPend>();
         if (ki >= kPend && lane == 0) mbar_arrive(&empty[pend[0]]);
 #pragma unroll
@@ -451,10 +437,10 @@ __global__ void __launch_bounds__(kThreads, 1)
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             uint4 v;
-            v.x = pack_bf16(y[j * 8 + 0], y[j * 8 + 1]);
-            v.y = pack_bf16(y[j * 8 + 2], y[j * 8 + 3]);
-            v.z = pack_bf16(y[j * 8 + 4], y[j * 8 + 5]);
-            v.w = pack_bf16(y[j * 8 + 6], y[j * 8 + 7]);
+            v.x = pack_bf16x2(y[j * 8 + 0], y[j * 8 + 1]);
+            v.y = pack_bf16x2(y[j * 8 + 2], y[j * 8 + 3]);
+            v.z = pack_bf16x2(y[j * 8 + 4], y[j * 8 + 5]);
+            v.w = pack_bf16x2(y[j * 8 + 6], y[j * 8 + 7]);
             st_shared_v4(srow + ((((ch & 1) * 4 + j) ^ sw) << 4), v);
           }
         } else {
@@ -523,10 +509,10 @@ __global__ void __launch_bounds__(kThreads, 1)
 #pragma unroll
               for (int j = 0; j < 4; ++j) {
                 uint4 v;
-                v.x = pack_bf16(y[j * 8 + 0], y[j * 8 + 1]);
-                v.y = pack_bf16(y[j * 8 + 2], y[j * 8 + 3]);
-                v.z = pack_bf16(y[j * 8 + 4], y[j * 8 + 5]);
-                v.w = pack_bf16(y[j * 8 + 6], y[j * 8 + 7]);
+                v.x = pack_bf16x2(y[j * 8 + 0], y[j * 8 + 1]);
+                v.y = pack_bf16x2(y[j * 8 + 2], y[j * 8 + 3]);
+                v.z = pack_bf16x2(y[j * 8 + 4], y[j * 8 + 5]);
+                v.w = pack_bf16x2(y[j * 8 + 6], y[j * 8 + 7]);
                 st_shared_v4(x_own + j * 16, v);
               }
               __syncwarp();
@@ -551,7 +537,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         named_bar_sync(bar_end, 128);
         if (gtid == 0) {
           for (int sl = 0; sl < BN / 64; ++sl)
-            if (n0 + sl * 64 < N && m0 < M) tma_store_2d(&maps.out, ostage + sl * kBM * 128, p.out_col_off + n0 + sl * 64, m0);
+            if (n0 + sl * 64 < N && m0 < M) tma_store_2d(&maps.out, smem_u32(ostage + sl * kBM * 128), p.out_col_off + n0 + sl * 64, m0);
           tma_store_commit();
         }
       }
@@ -580,7 +566,7 @@ bool wants_a_resident(const GemmParams& p, int BN, bool im2col, size_t max_smem)
 }
 
 template <int BN, bool kIm2col, int kEpi>
-int launch(const GemmMaps& maps, GemmParams& p, int num_sms, size_t max_smem, cudaStream_t stream) {
+int launch_gemm(const GemmMaps& maps, GemmParams& p, int num_sms, size_t max_smem, cudaStream_t stream) {
   constexpr int kStageBytes = kAStage + BN * kBK * 2;
   constexpr size_t kStagingBytes = static_cast<size_t>(BN / 64) * kBM * 128;
   const int k_iters_h = p.n_terms * p.taps * p.cblocks;
@@ -595,23 +581,8 @@ int launch(const GemmMaps& maps, GemmParams& p, int num_sms, size_t max_smem, cu
   stages = std::min(stages, 8);
   p.stages = stages;
   const size_t smem = fixed + static_cast<size_t>(stages) * stage_bytes;
-  auto kern = gemm_bf16_kernel<BN, kIm2col, kEpi>;
-  static bool attr_set_dev[64] = {};   // per template instantiation and device (the attribute is per device)
-  int cur_dev = 0;
-  DCR_CUDA_CHECK(cudaGetDevice(&cur_dev));
-  bool& attr_set = attr_set_dev[cur_dev & 63];
-  if (!attr_set) {
-    DCR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(max_smem)));
-    attr_set = true;
-  }
-  {
-    const int tiles = p.num_m_tiles * p.num_n_tiles;
-    const int grid = std::min(tiles, num_sms);
-    kern<<<grid, kThreads, smem, stream>>>(maps, p);
-  }
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  const int grid = std::min(p.num_m_tiles * p.num_n_tiles, num_sms);
+  return launch(gemm_bf16_kernel<BN, kIm2col, kEpi>, grid, kThreads, smem, stream, "conv_gemm", maps, p);
 }
 
 }  // namespace
@@ -619,8 +590,7 @@ int launch(const GemmMaps& maps, GemmParams& p, int num_sms, size_t max_smem, cu
 int conv_gemm(const ConvGemmDesc& d, cudaStream_t stream) {
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  DCR_REQUIRE(di->cc_major == 9 && di->cc_minor == 0, "conv_gemm: this build targets sm_90a; device reports sm_%d%d", di->cc_major,
-              di->cc_minor);
+  if (int rc = require_sm90a(di, "conv_gemm")) return rc;
   DCR_REQUIRE(d.n_terms >= 1 && d.n_terms <= kMaxGemmTerms, "conv_gemm: bad n_terms %d", d.n_terms);
   DCR_REQUIRE(d.C % 8 == 0 && d.N % 8 == 0, "conv_gemm: C (%d) and N (%d) must be multiples of 8", d.C, d.N);
   DCR_REQUIRE(d.kh >= 1 && d.kw >= 1 && d.stride >= 1, "conv_gemm: bad filter geometry");
@@ -736,8 +706,8 @@ int conv_gemm(const ConvGemmDesc& d, cudaStream_t stream) {
   const int epi = p.tma_epi ? 1 + p.act : 0;   // compile-time activation on the TMA-store path
 
 #define DCR_LAUNCH_E(BNv, E)                                                                      \
-  (im2col ? launch<BNv, true, E>(maps, p, di->num_sms, di->max_smem_optin, stream)              \
-          : launch<BNv, false, E>(maps, p, di->num_sms, di->max_smem_optin, stream))
+  (im2col ? launch_gemm<BNv, true, E>(maps, p, di->num_sms, di->max_smem_optin, stream)         \
+          : launch_gemm<BNv, false, E>(maps, p, di->num_sms, di->max_smem_optin, stream))
 #define DCR_LAUNCH(BNv)                                                                          \
   (epi == 0 ? DCR_LAUNCH_E(BNv, 0)                                                                \
             : (epi == 1 ? DCR_LAUNCH_E(BNv, 1) : (epi == 2 ? DCR_LAUNCH_E(BNv, 2) : (epi == 3 ? DCR_LAUNCH_E(BNv, 3) : DCR_LAUNCH_E(64, 4)))))

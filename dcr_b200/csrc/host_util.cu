@@ -4,6 +4,8 @@
 #include <cstring>
 #include <atomic>
 #include <mutex>
+#include <map>
+#include <utility>
 
 namespace dcr {
 
@@ -60,6 +62,33 @@ const DeviceInfo* device_info() {
     d.max_smem_optin = prop.sharedMemPerBlockOptin;
   }
   return &d;
+}
+
+int require_sm90a(const DeviceInfo* di, const char* who) {
+  DCR_REQUIRE(di->cc_major == 9 && di->cc_minor == 0, "%s: this build targets sm_90a; device reports sm_%d%d", who,
+              di->cc_major, di->cc_minor);
+  return 0;
+}
+
+int allow_dynamic_smem(const void* func, size_t bytes, const char* who) {
+  if (bytes <= 48 * 1024) return 0;
+  const DeviceInfo* di = device_info();
+  if (!di) return -2;
+  static std::map<std::pair<const void*, int>, size_t> limits;   // (kernel, device) -> dynamic shared memory allowed
+  static std::mutex mu;
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = limits.find({func, di->device});
+  if (it == limits.end()) {
+    // the kernel's static shared memory counts against the device's opt-in maximum too
+    cudaFuncAttributes fa;
+    DCR_CUDA_CHECK(cudaFuncGetAttributes(&fa, func));
+    const size_t limit = di->max_smem_optin - fa.sharedSizeBytes;
+    DCR_CUDA_CHECK(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(limit)));
+    it = limits.emplace(std::make_pair(func, di->device), limit).first;
+  }
+  DCR_REQUIRE(bytes <= it->second, "%s: %zu bytes of dynamic shared memory exceed the %zu the device allows this kernel", who,
+              bytes, it->second);
+  return 0;
 }
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

@@ -1,5 +1,5 @@
 // Host-side helpers shared by the .cu translation units: error capture for the C ABI, the driver entry point
-// for tensor-map encoding (no link-time dependency on libcuda), SM count cache.
+// for tensor-map encoding (no link-time dependency on libcuda), SM count cache, kernel launches.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -8,6 +8,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <string>
+#include <utility>
 
 namespace dcr {
 
@@ -48,6 +49,25 @@ bool tuning_flag(const char* name);   // true when tuning is enabled and the var
 
 // cached per current device; returns nullptr and sets the error on failure
 const DeviceInfo* device_info();
+
+// 0 on an sm_90 device, else -1 with an error naming `who`: the tensor-core kernels are built for sm_90a only
+int require_sm90a(const DeviceInfo* di, const char* who);
+
+// Lets `func` be launched with `bytes` of dynamic shared memory on the current device.  Above the default 48 KB the
+// kernel's limit is raised to the most the device allows it (the opt-in maximum less its static shared memory), once per
+// (kernel, device), so every later size is covered; more than that is refused (-1, naming `who`).
+int allow_dynamic_smem(const void* func, size_t bytes, const char* who);
+
+// kern<<<grid, block, smem, stream>>>(args...) after allow_dynamic_smem, counted, with the launch error checked
+template <class... Params, class... Args>
+int launch(void (*kern)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, const char* who,
+           Args&&... args) {
+  if (int rc = allow_dynamic_smem(reinterpret_cast<const void*>(kern), smem, who)) return rc;
+  kern<<<grid, block, smem, stream>>>(std::forward<Args>(args)...);
+  count_launch();
+  DCR_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
 
 // blocks for a grid-stride loop over work_items: one item per thread, at most 16 blocks per SM
 inline int grid_for(long long work_items, int block, int num_sms) {

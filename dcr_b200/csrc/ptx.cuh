@@ -1,7 +1,9 @@
-// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (tiled + im2col), wgmma.  Everything here is device-only and header-only.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (tiled + im2col loads, tiled stores), wgmma, the ping-pong
+// hand-off between two consumer warpgroups.  Everything here is device-only and header-only.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
 namespace dcr {
@@ -9,6 +11,18 @@ namespace dcr {
 #define DCR_DEVICE __device__ __forceinline__
 
 DCR_DEVICE uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
+
+// Dynamic shared memory rounded up to 1024 bytes: the 128-byte swizzle of TMA and wgmma repeats every 1024 bytes, so
+// tile bases carved from here line up with it.  Launches reserve 1024 bytes of slack for this.
+DCR_DEVICE uint8_t* smem_align1024(uint8_t* p) {
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
+}
+
+// two floats -> round-to-nearest bf16 pair, `lo` in the lower half (the lower address once stored)
+DCR_DEVICE uint32_t pack_bf16x2(float lo, float hi) {
+  __nv_bfloat162 p = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&p);
+}
 
 DCR_DEVICE bool elect_one() {
   uint32_t pred = 0;
@@ -89,6 +103,22 @@ DCR_DEVICE void named_bar_sync(uint32_t id, uint32_t threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
+// Ping-pong hand-off of two consumer warpgroups that take a CTA's tiles alternately, warpgroup 0 first: a warpgroup
+// starts the k-loop of its tile once the other one has issued its last k-block, so each epilogue runs under the other
+// warpgroup's k-loop.  turn[g] (count 4: the other warpgroup's warps) completes a phase per hand-over to warpgroup g.
+// Warpgroup 1's tile tc waits for phase tc of turn[1] (warpgroup 0's tile tc), warpgroup 0's tile tc > 0 for phase
+// tc - 1 of turn[0] (warpgroup 1's tile tc - 1).  A barrier never runs a phase ahead of its waiter, because the next
+// hand-over to a warpgroup needs that warpgroup's own hand-over first, so the parity of the phase is enough.
+struct PingPong {
+  uint64_t* turn;   // [2]
+  // tc: tiles this warpgroup has run so far
+  DCR_DEVICE void wait(uint32_t wg, uint32_t tc) const {
+    if (wg == 1 || tc > 0) mbar_wait(&turn[wg], (wg == 1 ? tc : tc - 1) & 1);
+  }
+  // one lane of each of the warpgroup's four warps, once the tile's last wgmma has been issued
+  DCR_DEVICE void hand_over(uint32_t wg) const { mbar_arrive(&turn[wg ^ 1]); }
+};
+
 // ----------------------------------------------------------------------------------------------
 // TMA
 DCR_DEVICE void tma_prefetch_desc(const void* tmap) {
@@ -116,12 +146,25 @@ DCR_DEVICE void tma_load_4d(void* dst, const void* tmap, uint64_t* bar, int c0, 
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(hint)
       : "memory");
 }
-DCR_DEVICE void tma_store_4d(const void* tmap, const void* src_smem, int c0, int c1, int c2, int c3) {
+DCR_DEVICE void tma_store_4d(const void* tmap, uint32_t src_smem, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(tmap)),
-               "r"(smem_u32(src_smem)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               "r"(src_smem), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
+DCR_DEVICE void tma_store_2d(const void* tmap, uint32_t src_smem, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(tmap)),
+               "r"(src_smem), "r"(c0), "r"(c1)
+               : "memory");
+}
+// Tiled stores are issued by one thread and tracked in bulk groups: commit closes the group of the stores issued since
+// the last commit; wait_read<N> returns once at most N groups still read their shared-memory source (the older sources
+// may be overwritten); wait_all returns once every committed store is complete.
+DCR_DEVICE void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+DCR_DEVICE void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+DCR_DEVICE void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // im2col-mode load of an NHWC tensor: coordinates {c, w, h, n} of the first base pixel, filter-tap offsets {w, h}
 DCR_DEVICE void tma_load_im2col_4d(void* dst, const void* tmap, uint64_t* bar, int c, int w, int h, int n,

@@ -135,13 +135,9 @@ int topk_merge(const float* scores, const long long* idx, int nq, int nlists, in
   const int wpb = 4;
   const int m = nlists * k_in;
   const size_t smem = ((static_cast<size_t>(wpb) * m * 4 + 15) & ~size_t(15)) + static_cast<size_t>(wpb) * m * 8;
-  DCR_CUDA_CHECK(cudaFuncSetAttribute(topk_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      static_cast<int>(smem)));
   const int blocks = std::min((nq + wpb - 1) / wpb, di->num_sms * 8);
-  topk_merge_kernel<<<blocks, wpb * 32, smem, stream>>>(scores, idx, nq, nlists, k_in, k_out, out_scores, out_idx);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(topk_merge_kernel, blocks, wpb * 32, smem, stream, "topk_merge", scores, idx, nq, nlists, k_in, k_out,
+                out_scores, out_idx);
 }
 
 }  // namespace dcr

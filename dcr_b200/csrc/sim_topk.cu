@@ -511,7 +511,7 @@ struct FusedPipe {
   uint8_t* tail;
   DCR_DEVICE FusedPipe(uint8_t* smem_raw, int nkb, int stream, int stages, size_t list_bytes) {
     // all tile bases 1024-byte aligned for the 128B swizzle
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* smem = smem_align1024(smem_raw);
     stream_a = stream != 0;
     num_kb = nkb;
     stage_bytes = kBlockN * kBlockK * 2 + (stream_a ? kATileBytes : 0);
@@ -1883,20 +1883,16 @@ int launch_fused(const SimPlan& pl, const PassPlan& pp, const __nv_bfloat16* qb,
   p.clk = clk;
   p.gthr = gthr;
   DCR_CUDA_CHECK(cudaMemsetAsync(gthr, 0, static_cast<size_t>(pp.nq_pad) * 4, stream));
-  auto launch = [&](auto kern) -> int {
-    DCR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pp.smem_bytes)));
-    kern<<<pp.n_units, 32 + 128 * pp.n_sets, pp.smem_bytes, stream>>>(tq, tg, p);
-    count_launch();
-    DCR_CUDA_CHECK(cudaGetLastError());
-    return 0;
+  auto sweep = [&](auto kern) {
+    return launch(kern, pp.n_units, 32 + 128 * pp.n_sets, pp.smem_bytes, stream, "sim_topk", tq, tg, p);
   };
   // both variants are launched; the one that does not match the device flag (query centring on / off) returns at once
   if (pp.n_sets == 2) {
-    if (int rc = launch(sim_topk_kernel<false, 2>)) return rc;
-    return launch(sim_topk_kernel<true, 2>);
+    if (int rc = sweep(sim_topk_kernel<false, 2>)) return rc;
+    return sweep(sim_topk_kernel<true, 2>);
   }
-  if (int rc = launch(sim_topk_kernel<false, 1>)) return rc;
-  return launch(sim_topk_kernel<true, 1>);
+  if (int rc = sweep(sim_topk_kernel<false, 1>)) return rc;
+  return sweep(sim_topk_kernel<true, 1>);
 }
 
 // Stage 1 of both entry points: the centres, the decision whether to centre the queries, and the bf16 operands with the
@@ -2023,11 +2019,8 @@ int split_rescore(const float* q, const float* g, int nq, int d, int n_chunks, i
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0,
               "split_rescore: q/g must be 16-byte aligned");
   const size_t smem = ((static_cast<size_t>(d / n_chunks) * 4 + 15) & ~size_t(15)) + static_cast<size_t>(n_cand) * 16;
-  DCR_CUDA_CHECK(cudaFuncSetAttribute(split_rescore_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  split_rescore_kernel<<<nq, 128, smem, stream>>>(q, g, d, n_chunks, cross, cand, n_cand, k, out_scores, out_idx);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(split_rescore_kernel, nq, 128, smem, stream, "split_rescore", q, g, d, n_chunks, cross, cand, n_cand, k,
+                out_scores, out_idx);
 }
 
 size_t sim_topk_workspace_size(int nq, int ng, int d, int k) {
@@ -2043,8 +2036,7 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
              cudaStream_t stream, SimStats* stats) {
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  DCR_REQUIRE(di->cc_major == 9 && di->cc_minor == 0, "sim_topk: this build targets sm_90a; device reports sm_%d%d", di->cc_major,
-              di->cc_minor);
+  if (int rc = require_sm90a(di, "sim_topk")) return rc;
   SimPlan pl;
   if (int rc = make_plan(nq, ng, d, k, di->num_sms, di->max_smem_optin, &pl)) return rc;
   DCR_REQUIRE(ws != nullptr && ws_bytes >= pl.total, "sim_topk: workspace too small (%zu < %zu)", ws_bytes, pl.total);
@@ -2111,11 +2103,7 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     const int per_block = warp_form ? kRescoreThreads / 32 : 1;
     const size_t smem = per_block * per_query;
     auto kern = warp_form ? rescore_select_kernel<32> : rescore_select_kernel<kRescoreThreads>;
-    DCR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    kern<<<(pp.nq + per_block - 1) / per_block, kRescoreThreads, smem, stream>>>(rp);
-    count_launch();
-    DCR_CUDA_CHECK(cudaGetLastError());
-    return 0;
+    return launch(kern, (pp.nq + per_block - 1) / per_block, kRescoreThreads, smem, stream, "sim_topk", rp);
   };
   if (int rc = rescore(pl.p0, nullptr, flag0, counts + 0, thr1)) return rc;
 
@@ -2148,12 +2136,11 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     // queries per brute-force launch: as many as fit in shared memory next to each other (32 up to d = 1536)
     const int ex_batch = std::max(1, std::min<int>(kExactBatch, static_cast<int>(192 * 1024 / (static_cast<size_t>(d) * 4))));
     const size_t ex_smem = static_cast<size_t>(ex_batch) * d * 4;
-    DCR_CUDA_CHECK(cudaFuncSetAttribute(exact_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(ex_smem)));
     const int* n_dev = (exact_list == flag0) ? counts + 0 : counts + 1;
     for (int done = 0; done < n_exact; done += ex_batch) {
-      exact_scan_kernel<<<di->num_sms * 2, 256, ex_smem, stream>>>(q, g, ng, d, exact_list, done, n_dev, exact, ex_batch);
-      count_launch();
+      if (int rc = launch(exact_scan_kernel, di->num_sms * 2, 256, ex_smem, stream, "sim_topk", q, g, ng, d, exact_list, done,
+                          n_dev, exact, ex_batch))
+        return rc;
       exact_select_kernel<<<ex_batch, 256, 0, stream>>>(exact, ng, k, exact_list, done, n_dev, g_index_base,
                                                            g_index_stride, out_scores, out_idx);
       count_launch();
@@ -2195,8 +2182,7 @@ int sim_range(const float* q, int nq, const float* g, int ng, int d, float thres
               long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  DCR_REQUIRE(di->cc_major == 9 && di->cc_minor == 0, "sim_range: this build targets sm_90a; device reports sm_%d%d", di->cc_major,
-              di->cc_minor);
+  if (int rc = require_sm90a(di, "sim_range")) return rc;
   DCR_REQUIRE(!std::isnan(threshold), "sim_range: threshold is NaN");
   DCR_REQUIRE(g_index_stride >= 1, "sim_range: g_index_stride=%lld < 1", g_index_stride);
   RangePlan rp;
@@ -2253,16 +2239,10 @@ int sim_range(const float* q, int nq, const float* g, int ng, int d, float thres
   p.seg = seg;
   p.row_cand = row_cand;
   p.cand_idx = cand_idx;
-  auto launch = [&](auto kern) -> int {
-    DCR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(rp.smem_bytes)));
-    kern<<<rp.n_units, 32 + 128, rp.smem_bytes, stream>>>(tq, tg, p);
-    count_launch();
-    DCR_CUDA_CHECK(cudaGetLastError());
-    return 0;
-  };
+  auto sweep = [&](auto kern) { return launch(kern, rp.n_units, 32 + 128, rp.smem_bytes, stream, "sim_range", tq, tg, p); };
   // both centring variants are launched; the one that does not match the device flag returns at once
-  if (int rc = launch(sim_range_kernel<false, false>)) return rc;
-  if (int rc = launch(sim_range_kernel<true, false>)) return rc;
+  if (int rc = sweep(sim_range_kernel<false, false>)) return rc;
+  if (int rc = sweep(sim_range_kernel<true, false>)) return rc;
   range_slot_scan_kernel<<<(nq + 255) / 256, 256, 0, stream>>>(seg, nq, rp.n_qtiles, geo.n_gtiles, geo.gchunk,
                                                                 geo.n_chunks, rp.n_units, row_cnt, row_pcnt);
   count_launch();
@@ -2282,13 +2262,11 @@ int sim_range(const float* q, int nq, const float* g, int ng, int d, float thres
                      n_cand, max_pairs);
 
   if (n_pieces > 0) {
-    if (int rc = launch(sim_range_kernel<false, true>)) return rc;
-    if (int rc = launch(sim_range_kernel<true, true>)) return rc;
-    const size_t smem = static_cast<size_t>(d) * 8;
-    DCR_CUDA_CHECK(cudaFuncSetAttribute(range_rescore_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    range_rescore_kernel<<<static_cast<unsigned>(n_pieces), kRescoreThreads, smem, stream>>>(
-        q, g, nq, d, threshold, row_cand, row_piece, cand_idx, cand_score, piece_kept);
-    count_launch();
+    if (int rc = sweep(sim_range_kernel<false, true>)) return rc;
+    if (int rc = sweep(sim_range_kernel<true, true>)) return rc;
+    if (int rc = launch(range_rescore_kernel, static_cast<unsigned>(n_pieces), kRescoreThreads, static_cast<size_t>(d) * 8,
+                        stream, "sim_range", q, g, nq, d, threshold, row_cand, row_piece, cand_idx, cand_score, piece_kept))
+      return rc;
   }
   exclusive_scan_kernel<int><<<1, 1024, 0, stream>>>(piece_kept, n_pieces, piece_excl);
   count_launch();

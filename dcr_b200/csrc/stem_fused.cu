@@ -74,11 +74,6 @@ DCR_DEVICE void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* 
                : "memory");
 }
 
-DCR_DEVICE uint32_t pack2s(float a, float b) {
-  __nv_bfloat162 p = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&p);
-}
-
 // first position of a unit
 DCR_DEVICE int unit_begin(const StemParams& p, int part, bool pool) {
   if (!pool) return part * kSTile;
@@ -92,7 +87,7 @@ DCR_DEVICE int unit_begin(const StemParams& p, int part, bool pool) {
 template <bool kPool>
 __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_constant__ CUtensorMap tmap_w, const StemParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   const int win_bytes = p.win_units * 16;                       // per plane
   const int stage_bytes = (2 * win_bytes + 1023) & ~1023;
   uint8_t* s_w = smem;                                          // 32 KB, 4 k-blocks
@@ -212,14 +207,14 @@ __global__ void __launch_bounds__(kSThreads, 1) stem_conv_kernel(const __grid_co
           uint4 v[4];
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
-            v[q].x = pack2s(fmaxf(fmaf(__uint_as_float(r[q * 8 + 0]), sc[q * 8 + 0], bi[q * 8 + 0]), 0.f),
-                            fmaxf(fmaf(__uint_as_float(r[q * 8 + 1]), sc[q * 8 + 1], bi[q * 8 + 1]), 0.f));
-            v[q].y = pack2s(fmaxf(fmaf(__uint_as_float(r[q * 8 + 2]), sc[q * 8 + 2], bi[q * 8 + 2]), 0.f),
-                            fmaxf(fmaf(__uint_as_float(r[q * 8 + 3]), sc[q * 8 + 3], bi[q * 8 + 3]), 0.f));
-            v[q].z = pack2s(fmaxf(fmaf(__uint_as_float(r[q * 8 + 4]), sc[q * 8 + 4], bi[q * 8 + 4]), 0.f),
-                            fmaxf(fmaf(__uint_as_float(r[q * 8 + 5]), sc[q * 8 + 5], bi[q * 8 + 5]), 0.f));
-            v[q].w = pack2s(fmaxf(fmaf(__uint_as_float(r[q * 8 + 6]), sc[q * 8 + 6], bi[q * 8 + 6]), 0.f),
-                            fmaxf(fmaf(__uint_as_float(r[q * 8 + 7]), sc[q * 8 + 7], bi[q * 8 + 7]), 0.f));
+            v[q].x = pack_bf16x2(fmaxf(fmaf(__uint_as_float(r[q * 8 + 0]), sc[q * 8 + 0], bi[q * 8 + 0]), 0.f),
+                                 fmaxf(fmaf(__uint_as_float(r[q * 8 + 1]), sc[q * 8 + 1], bi[q * 8 + 1]), 0.f));
+            v[q].y = pack_bf16x2(fmaxf(fmaf(__uint_as_float(r[q * 8 + 2]), sc[q * 8 + 2], bi[q * 8 + 2]), 0.f),
+                                 fmaxf(fmaf(__uint_as_float(r[q * 8 + 3]), sc[q * 8 + 3], bi[q * 8 + 3]), 0.f));
+            v[q].z = pack_bf16x2(fmaxf(fmaf(__uint_as_float(r[q * 8 + 4]), sc[q * 8 + 4], bi[q * 8 + 4]), 0.f),
+                                 fmaxf(fmaf(__uint_as_float(r[q * 8 + 5]), sc[q * 8 + 5], bi[q * 8 + 5]), 0.f));
+            v[q].w = pack_bf16x2(fmaxf(fmaf(__uint_as_float(r[q * 8 + 6]), sc[q * 8 + 6], bi[q * 8 + 6]), 0.f),
+                                 fmaxf(fmaf(__uint_as_float(r[q * 8 + 7]), sc[q * 8 + 7], bi[q * 8 + 7]), 0.f));
           }
           const int mblk = m0 + mb * 128;
           if constexpr (!kPool) {
@@ -329,8 +324,7 @@ int stem_conv(const __nv_bfloat16* planes, int B, int OH, int OW, const __nv_bfl
               __nv_bfloat16* out, cudaStream_t stream, int pool) {
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  DCR_REQUIRE(di->cc_major == 9 && di->cc_minor == 0, "stem_conv: this build targets sm_90a; device reports sm_%d%d", di->cc_major,
-              di->cc_minor);
+  if (int rc = require_sm90a(di, "stem_conv")) return rc;
   if (B == 0) return 0;
   StemParams p;
   memset(&p, 0, sizeof(p));
@@ -371,24 +365,8 @@ int stem_conv(const __nv_bfloat16* planes, int B, int OH, int OW, const __nv_bfl
   DCR_REQUIRE(fixed + stage <= di->max_smem_optin, "stem_conv: image too wide for the window buffers (OW = %d)", OW);
   p.win_stages = static_cast<int>(std::min<size_t>(4, (di->max_smem_optin - fixed) / stage));
   const size_t smem = fixed + p.win_stages * stage;
-  static bool attr_set[64][2] = {};
   const int grid = std::min(p.num_units, di->num_sms);
-  if (pool) {
-    if (!attr_set[di->device & 63][1]) {
-      DCR_CUDA_CHECK(cudaFuncSetAttribute(stem_conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(di->max_smem_optin)));
-      attr_set[di->device & 63][1] = true;
-    }
-    stem_conv_kernel<true><<<grid, kSThreads, smem, stream>>>(tw, p);
-  } else {
-    if (!attr_set[di->device & 63][0]) {
-      DCR_CUDA_CHECK(cudaFuncSetAttribute(stem_conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(di->max_smem_optin)));
-      attr_set[di->device & 63][0] = true;
-    }
-    stem_conv_kernel<false><<<grid, kSThreads, smem, stream>>>(tw, p);
-  }
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(pool ? stem_conv_kernel<true> : stem_conv_kernel<false>, grid, kSThreads, smem, stream, "stem_conv", tw, p);
 }
 
 }  // namespace dcr

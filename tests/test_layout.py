@@ -63,3 +63,13 @@ def test_similarity_planner_accepts_the_supported_shape_range():
     for nq, ng, d, k in [(0, 10, 64, 1), (10, 10, 64, 17), (10, 5, 64, 8), (10, 10, 8200, 1), (10, 0, 64, 1)]:
         assert lib.dcr_sim_topk_workspace_size(nq, ng, d, k) == 0
         assert lib.dcr_last_error().decode() != ""
+
+
+def test_hopper_scaffolding_has_one_definition():
+    """The opt-in to large dynamic shared memory, the TMA bulk-store group and the 1024-byte alignment of dynamic shared
+    memory are each written once (host_util.cu, ptx.cuh); kernels and launch sites use those instead of a private copy."""
+    csrc = os.path.join(ROOT, "dcr_b200", "csrc")
+    texts = {f: open(os.path.join(csrc, f)).read() for f in sorted(os.listdir(csrc)) if f.endswith((".cu", ".cuh", ".h"))}
+    for needle, home in [("cudaFuncSetAttribute", "host_util.cu"), ("cp.async.bulk.commit_group", "ptx.cuh"),
+                         ("cp.async.bulk.wait_group", "ptx.cuh"), ("~uintptr_t(1023)", "ptx.cuh")]:
+        assert [f for f, t in texts.items() if needle in t] == [home], needle
