@@ -69,6 +69,19 @@ int launch(void (*kern)(Params...), dim3 grid, dim3 block, size_t smem, cudaStre
   return 0;
 }
 
+// Cuts a workspace into buffers, each 256-byte aligned on its own, so the size does not depend on their order.  A
+// planner runs the same code as its entry point on a null base: `bytes` is then the workspace size it reports.
+struct Carve {
+  uint8_t* base = nullptr;
+  size_t bytes = 0;
+  template <class T>
+  T* take(size_t count) {
+    T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+    bytes += (count * sizeof(T) + 255) / 256 * 256;
+    return p;
+  }
+};
+
 // blocks for a grid-stride loop over work_items: one item per thread, at most 16 blocks per SM
 inline int grid_for(long long work_items, int block, int num_sms) {
   const long long blocks = (work_items + block - 1) / block;

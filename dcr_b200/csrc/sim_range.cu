@@ -1,0 +1,454 @@
+// Threshold search for sm_90a (dcr_sim_range): every pair scoring at least tau, exact, in CSR form.  It replaces the saved
+// score matrices of diff_retrieval.py:402-403, 414-415 and the threshold of :454.  Stage 1 and the fused sweep are the
+// top-k search's (sim_sweep.cuh): the sweep's epilogue compares each approximate score against a per-row threshold that
+// no qualifying pair can fall below, and the candidates are re-scored with the same fp64 dot product.
+#include <algorithm>
+#include <cmath>
+
+#include "../../include/dcr_b200.h"
+#include "dcr_internal.cuh"
+#include "sim_sweep.cuh"
+
+namespace dcr {
+
+namespace {
+
+// ------------------------------------------------------------------------------------------------------------
+// Threshold search (dcr_sim_range): every pair with fp32(exact score) >= tau, in CSR form.
+//   1. range_threshold_kernel  per query row the candidate threshold t_i on the approximate score: no pair whose fp32
+//                              exact score reaches tau has an approximate score below t_i (row_bound)
+//   2. sim_range_kernel<*, 0>  count sweep: candidates per (segment slot, row)
+//   3. range_slot_scan_kernel + exclusive_scan_kernel: per row, the slots' offsets in gallery order; the rows' offsets
+//   4. sim_range_kernel<*, 1>  emit sweep: the same decisions again, each row's candidates written in ascending order
+//   5. range_rescore_kernel    exact scores in pieces of kRangePiece candidates of one row, stable compaction to the
+//                              pairs that reach tau
+//   6. exclusive_scan_kernel over the pieces, range_output_kernel / range_row_offsets_kernel: the CSR arrays
+// Everything is a fixed function of the inputs (no atomics decide an order), so every call returns the same bits.
+constexpr int kRangePiece = 512;   // candidates of one row re-scored by one block
+
+struct RangeParams : SweepHead {
+  int stages;
+  const int* bias_flag;
+  const float* col_bias;
+  const float* thr;            // [nq] candidate threshold t_i
+  int* seg;                    // [n_slots][128] count sweep: candidates; emit sweep: offset inside the row
+  const long long* row_cand;   // [nq + 1] emit sweep: first candidate of each row
+  int* cand_idx;               // emit sweep: local gallery rows
+};
+
+// Candidate columns of one 32-column chunk of an accumulator row: bit c is set when the approximate score of column
+// col0 + c is not below t (NaN included: the exact score decides) and c < n_valid.  Columns past the gallery are cut by
+// n_valid rather than by mask_tail: at t = -inf their -inf would pass.
+template <bool kBias>
+DCR_DEVICE uint32_t range_hits(const uint32_t (&r)[32], const float* sb, float t, int n_valid) {
+  float v[32];
+#pragma unroll
+  for (int c = 0; c < 32; ++c) v[c] = __uint_as_float(r[c]);
+  if constexpr (kBias) {   // the same fp32 additions as scan_chunk
+#pragma unroll
+    for (int c = 0; c < 32; c += 4) {
+      const float4 b = *reinterpret_cast<const float4*>(sb + c);
+      v[c] += b.x; v[c + 1] += b.y; v[c + 2] += b.z; v[c + 3] += b.w;
+    }
+  }
+  uint32_t m = 0;
+#pragma unroll
+  for (int c = 0; c < 32; ++c) m |= static_cast<uint32_t>(!(v[c] < t)) << c;
+  if (n_valid < 32) m &= n_valid <= 0 ? 0u : (1u << n_valid) - 1u;
+  return m;
+}
+
+// The fused sweep of the threshold search: the work decomposition, pipeline and k-loop of sim_topk_kernel with one
+// consumer warpgroup, an epilogue that compares every accumulator column against its row's threshold, and no warm-up.
+// kEmit = 0 counts the candidates of every (segment slot, row); kEmit = 1 writes them at the offsets the scan derived
+// from those counts.  Both make the same decisions: same tiles, same wgmma sequence, same thresholds.
+template <bool kBias, bool kEmit>
+__global__ void __launch_bounds__(32 + 128, 1)
+    sim_range_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_g,
+                     const RangeParams p) {
+  if (((p.bias_flag != nullptr) && (*p.bias_flag != 0)) != kBias) return;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const FusedPipe pp(smem_raw, p.num_kb, p.stream_a, p.stages, 0);   // then barriers, then 4 transpose buffers
+  const uint32_t warp = threadIdx.x >> 5;
+  const uint32_t lane = threadIdx.x & 31;
+  pp.init(&tmap_q, &tmap_g, p.stages, 4);
+  const long long n_units = gridDim.x;
+  const long long unit = blockIdx.x;
+  SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
+  if (warp == 4) {
+    fused_producer(pp, &tmap_q, &tmap_g, p.stages, w, [](const SegWalker&) { return 0; });
+  } else {
+    const uint32_t row = warp * 32 + lane;   // query row inside the tile
+    const uint32_t xacc = smem_u32(pp.tail) + warp * kAccXposeWarpBytes;
+    const uint32_t a_base = smem_u32(pp.stream_a ? pp.smem_b + kBTileBytes : pp.smem_a);
+    const uint32_t b_base = smem_u32(pp.smem_b);
+    PipeState st(p.stages);
+    uint32_t seg = 0;
+    while (w.next()) {
+      const int qrow = w.qi * kBlockM + static_cast<int>(row);
+      const bool row_ok = qrow < p.nq;
+      const float t = row_ok ? p.thr[qrow] : INFINITY;
+      const size_t sr = static_cast<size_t>(slot_index(w.chunk, static_cast<int>(unit), w.qi, 0, static_cast<int>(n_units),
+                                                       p.n_qtiles, 1)) * kBlockM + row;
+      int cnt = 0;
+      int* out = nullptr;
+      if (kEmit && row_ok) out = p.cand_idx + p.row_cand[qrow] + p.seg[sr];
+      if (!pp.stream_a) mbar_wait(pp.a_full, seg & 1);
+#pragma unroll 1
+      for (int j = 0; j < w.ntiles; ++j) {
+        WgAcc<kBlockN> acc;
+        fused_tile_mma(acc, st, pp, a_base, b_base, j == w.ntiles - 1, lane);
+        const int gcol0 = (w.g_begin + j) * kBlockN;
+#pragma unroll
+        for (int ch = 0; ch < kBlockN / 32; ++ch) {
+          uint32_t r[32];
+          acc.rows32(ch, r, xacc, lane);
+          const int col0 = gcol0 + ch * 32;
+          const uint32_t hits = range_hits<kBias>(r, kBias ? p.col_bias + col0 : nullptr, t, row_ok ? p.ng - col0 : 0);
+          if constexpr (kEmit) {
+            for (uint32_t h = hits; h; h &= h - 1) *out++ = col0 + __ffs(h) - 1;   // ascending columns
+          } else {
+            cnt += __popc(hits);
+          }
+        }
+      }
+      ++seg;
+      if (!kEmit) p.seg[sr] = cnt;
+    }
+  }
+  __syncthreads();
+}
+
+// t_i = tau - q.mu - eps - slack - margin, rounded down at every step.  fp32(s) >= tau needs s >= tau - half an fp32 ulp
+// (margin), hence approximate score >= t_i (row_bound).  A warp per query row.
+__global__ void __launch_bounds__(128)
+    range_threshold_kernel(const float* __restrict__ q, int nq, int d, int d_pad, float tau,
+                           const float* __restrict__ q_norm_hat, const float* __restrict__ q_norm_res,
+                           const float* __restrict__ q_norm_x, const unsigned int* __restrict__ g_max,
+                           const float* __restrict__ mu, const float* __restrict__ nu, const int* __restrict__ nu_flag,
+                           float* __restrict__ thr) {
+  const int row = blockIdx.x * 4 + static_cast<int>(threadIdx.x >> 5);
+  const uint32_t lane = threadIdx.x & 31;
+  if (row >= nq) return;
+  const RowBound rb = row_bound(q + static_cast<size_t>(row) * d, d, d_pad, row, q_norm_hat, q_norm_res, q_norm_x, g_max,
+                                mu, nu, nu_flag, lane);
+  if (lane == 0) {
+    const double margin = isfinite(tau) ? fabs(static_cast<double>(tau)) * 1.2e-7 + 1e-45 : 0.0;
+    double t = __dsub_rd(static_cast<double>(tau), rb.qmu);
+    t = __dsub_rd(t, static_cast<double>(rb.eps));
+    t = __dsub_rd(t, rb.slack);
+    t = __dsub_rd(t, margin);
+    thr[row] = __double2float_rd(t);
+  }
+}
+
+// Per query row (a thread each): walk the row's segment slots in gallery order -- chunk by chunk, and inside a chunk unit
+// by unit (a unit's tiles follow the previous unit's) -- replacing each count by the row's candidates before it.
+__global__ void __launch_bounds__(256)
+    range_slot_scan_kernel(int* __restrict__ seg, int nq, int n_qtiles, int n_gtiles, int gchunk, int n_chunks,
+                           int n_units, long long* __restrict__ row_cnt, long long* __restrict__ row_pieces) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= nq) return;
+  const int qi = row / kBlockM, r = row % kBlockM;
+  int acc = 0;
+  for (int chunk = 0; chunk < n_chunks; ++chunk) {
+    const int ncg = min(gchunk, n_gtiles - chunk * gchunk);
+    const long long T = static_cast<long long>(n_qtiles) * ncg;
+    const int u_lo = static_cast<int>(owner_unit(static_cast<long long>(qi) * ncg, T, n_units));
+    const int u_hi = static_cast<int>(owner_unit(static_cast<long long>(qi + 1) * ncg - 1, T, n_units));
+    for (int u = u_lo; u <= u_hi; ++u) {
+      const size_t sr = static_cast<size_t>(slot_index(chunk, u, qi, 0, n_units, n_qtiles, 1)) * kBlockM + r;
+      const int c = seg[sr];
+      seg[sr] = acc;
+      acc += c;
+    }
+  }
+  row_cnt[row] = acc;
+  row_pieces[row] = (acc + kRangePiece - 1) / kRangePiece;
+}
+
+// out[0..n] = exclusive prefix sums of in[0..n-1] (out[n] = total), one block: thread t sums a contiguous run, the runs'
+// sums are scanned in shared memory, then each thread writes its run.  Fixed association.
+template <typename T>
+__global__ void __launch_bounds__(1024) exclusive_scan_kernel(const T* __restrict__ in, long long n, long long* __restrict__ out) {
+  __shared__ long long part[32];
+  const int tid = threadIdx.x, lane = tid & 31, wp = tid >> 5;
+  const long long per = (n + 1023) / 1024;
+  const long long lo = min(n, tid * per), hi = min(n, lo + per);
+  long long s = 0;
+  for (long long i = lo; i < hi; ++i) s += in[i];
+  long long incl = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const long long v = __shfl_up_sync(kFull, incl, o);
+    if (lane >= o) incl += v;
+  }
+  if (lane == 31) part[wp] = incl;
+  __syncthreads();
+  if (wp == 0) {
+    long long x = part[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const long long v = __shfl_up_sync(kFull, x, o);
+      if (lane >= o) x += v;
+    }
+    part[lane] = x;   // inclusive over warps
+  }
+  __syncthreads();
+  long long run = incl - s + (wp > 0 ? part[wp - 1] : 0);
+  for (long long i = lo; i < hi; ++i) {
+    out[i] = run;
+    run += in[i];
+  }
+  if (tid == 0) out[n] = part[31];
+}
+
+// piece w: row, first candidate and candidate count (row_piece[0] = 0 <= w < row_piece[nq])
+DCR_DEVICE void range_piece(long long w, const long long* __restrict__ row_cand, const long long* __restrict__ row_piece,
+                            int nq, int& row, long long& start, int& n) {
+  int lo = 0, hi = nq;   // row_piece[lo] <= w < row_piece[hi]
+  while (hi - lo > 1) {
+    const int mid = lo + (hi - lo) / 2;
+    if (row_piece[mid] <= w) lo = mid;
+    else hi = mid;
+  }
+  row = lo;
+  start = row_cand[lo] + (w - row_piece[lo]) * kRangePiece;
+  n = static_cast<int>(min(static_cast<long long>(kRangePiece), row_cand[lo + 1] - start));
+}
+
+// Exact scores of one piece (exact_dot: the values dcr_sim_topk reports), then a stable in-place
+// compaction of the pairs with fp32 score >= tau.  piece_kept[w] = pairs kept.
+__global__ void __launch_bounds__(kRescoreThreads)
+    range_rescore_kernel(const float* __restrict__ q, const float* __restrict__ g, int nq, int d, float tau,
+                         const long long* __restrict__ row_cand, const long long* __restrict__ row_piece,
+                         int* __restrict__ cand_idx, float* __restrict__ cand_score, int* __restrict__ piece_kept) {
+  extern __shared__ __align__(16) uint8_t sm[];
+  double* qs = reinterpret_cast<double*>(sm);   // [d] the query row, widened once
+  const int tid = threadIdx.x;
+  const uint32_t lane = threadIdx.x & 31;
+  const int warp = tid >> 5;
+  int row, n;
+  long long start;
+  range_piece(blockIdx.x, row_cand, row_piece, nq, row, start, n);
+  for (int c = tid; c < d; c += kRescoreThreads) qs[c] = static_cast<double>(q[static_cast<size_t>(row) * d + c]);
+  __syncthreads();
+  int* ci = cand_idx + start;
+  float* cs = cand_score + start;
+  for (int c = 2 * warp; c < n; c += 2 * (kRescoreThreads / 32)) {
+    double v0, v1 = 0.0;
+    if (c + 1 < n) exact_dot<2>(qs, g + static_cast<size_t>(ci[c]) * d, g + static_cast<size_t>(ci[c + 1]) * d, d, lane, v0, v1);
+    else exact_dot<1>(qs, g + static_cast<size_t>(ci[c]) * d, nullptr, d, lane, v0, v1);
+    if (lane == 0) {
+      cs[c] = static_cast<float>(v0);
+      if (c + 1 < n) cs[c + 1] = static_cast<float>(v1);
+    }
+  }
+  __syncthreads();
+  // round by round: every read of a round happens before the barrier inside group_scan, every write after it, and a
+  // round writes only below the positions later rounds read
+  int kept = 0;
+  for (int c0 = 0; c0 < n; c0 += kRescoreThreads) {
+    const int c = c0 + tid;
+    int idx = 0;
+    float s = 0.f;
+    bool keep = false;
+    if (c < n) {
+      idx = ci[c];
+      s = cs[c];
+      keep = s >= tau;   // NaN never
+    }
+    int total;
+    const int pos = kept + group_scan<kRescoreThreads>(keep ? 1 : 0, total);
+    if (keep) {
+      ci[pos] = idx;
+      cs[pos] = s;
+    }
+    kept += total;
+  }
+  if (tid == 0) piece_kept[blockIdx.x] = kept;
+}
+
+// piece w's kept pairs -> the output at piece_excl[w] (global gallery indices)
+__global__ void __launch_bounds__(256)
+    range_output_kernel(const long long* __restrict__ row_cand, const long long* __restrict__ row_piece, int nq,
+                        const long long* __restrict__ piece_excl, const int* __restrict__ cand_idx,
+                        const float* __restrict__ cand_score, long long g_index_base, long long g_index_stride,
+                        long long* __restrict__ out_idx, float* __restrict__ out_scores) {
+  int row, n;
+  long long start;
+  range_piece(blockIdx.x, row_cand, row_piece, nq, row, start, n);
+  const long long o = piece_excl[blockIdx.x];
+  const int kept = static_cast<int>(piece_excl[blockIdx.x + 1] - o);
+  for (int j = threadIdx.x; j < kept; j += blockDim.x) {
+    out_idx[o + j] = g_index_base + g_index_stride * cand_idx[start + j];
+    out_scores[o + j] = cand_score[start + j];
+  }
+}
+
+// row i starts at the output position of its first piece (rows without candidates: of the next row's first piece)
+__global__ void range_row_offsets_kernel(const long long* __restrict__ row_piece, const long long* __restrict__ piece_excl,
+                                         int nq, long long* __restrict__ row_offsets) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= nq; i += gridDim.x * blockDim.x)
+    row_offsets[i] = piece_excl[row_piece[i]];
+}
+
+constexpr long long kMaxRangePairs = 1ll << 40;   // capacity accepted by the planner (keeps the byte counts in range)
+
+struct RangePlan {
+  SweepGeometry geo;
+  int nq_pad, n_qtiles, n_units, n_slots, stages;
+  size_t smem_bytes;
+  long long max_pieces;   // pieces of kRangePiece candidates when max_pairs candidates fill the rows worst
+  size_t total;           // workspace bytes
+};
+
+// The threshold search's workspace: the operands, the per-row thresholds, the slot counts / offsets, the row and piece
+// scans, and the candidates with their scores
+struct RangeBuffers {
+  Operands ops;
+  float* thr;
+  int* seg;
+  long long *row_cnt, *row_cand, *row_pcnt, *row_piece;
+  int* cand_idx;
+  float* cand_score;
+  int* piece_kept;
+  long long* piece_excl;
+};
+
+RangeBuffers carve_range(const RangePlan& rp, int nq, int d, long long max_pairs, Carve& w) {
+  RangeBuffers b;
+  b.ops = carve_operands(w, rp.nq_pad, rp.geo, d);
+  b.ops.qflag = w.take<int>(4);
+  b.thr = w.take<float>(nq);
+  b.seg = w.take<int>(static_cast<size_t>(rp.n_slots) * kBlockM);
+  b.row_cnt = w.take<long long>(nq);
+  b.row_cand = w.take<long long>(static_cast<size_t>(nq) + 1);
+  b.row_pcnt = w.take<long long>(nq);
+  b.row_piece = w.take<long long>(static_cast<size_t>(nq) + 1);
+  b.cand_idx = w.take<int>(max_pairs);
+  b.cand_score = w.take<float>(max_pairs);
+  b.piece_kept = w.take<int>(rp.max_pieces);
+  b.piece_excl = w.take<long long>(static_cast<size_t>(rp.max_pieces) + 1);
+  return b;
+}
+
+int make_range_plan(int nq, int ng, int d, long long max_pairs, int num_sms, size_t max_smem, RangePlan* rp) {
+  DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "sim_range: empty problem (nq=%d ng=%d d=%d)", nq, ng, d);
+  DCR_REQUIRE(d <= kMaxDim, "sim_range: descriptor dim %d > %d not supported", d, kMaxDim);
+  DCR_REQUIRE(d % 4 == 0, "sim_range: descriptor dim %d is not a multiple of 4", d);
+  DCR_REQUIRE(max_pairs >= 0 && max_pairs <= kMaxRangePairs, "sim_range: max_pairs=%lld outside [0, 2^40]", max_pairs);
+  plan_geometry(ng, d, &rp->geo);
+  const SweepGeometry& g = rp->geo;
+  rp->n_qtiles = (nq + kBlockM - 1) / kBlockM;
+  rp->nq_pad = rp->n_qtiles * kBlockM;
+  // shared memory: the pipeline, then the accumulator transposes of 4 warps
+  auto smem = [&](int st) { return FusedPipe::smem_bytes(g.num_kb, g.stream_a, st, 0, 4 * kAccXposeWarpBytes); };
+  int stages = 2;
+  DCR_REQUIRE(max_smem >= smem(stages), "sim_range: not enough shared memory (%zu B) for d=%d", max_smem, d);
+  while (stages < 8 && max_smem >= smem(stages + 1)) ++stages;
+  rp->stages = stages;
+  rp->smem_bytes = smem(stages);
+  // every unit owns at least one tile of every chunk (the last chunk is the smallest): every slot the scan walks is written
+  const int last = g.n_gtiles - (g.n_chunks - 1) * g.gchunk;
+  rp->n_units = static_cast<int>(std::min<long long>(num_sms, static_cast<long long>(rp->n_qtiles) * last));
+  rp->n_slots = g.n_chunks * (rp->n_units + rp->n_qtiles);
+  rp->max_pieces = max_pairs / kRangePiece + nq;
+  Carve size;
+  carve_range(*rp, nq, d, max_pairs, size);
+  rp->total = size.bytes;
+  return 0;
+}
+
+}  // namespace
+
+size_t sim_range_workspace_size(int nq, int ng, int d, long long max_pairs) {
+  const DeviceInfo* di = device_info();
+  RangePlan rp;
+  if (make_range_plan(nq, ng, d, max_pairs, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &rp) != 0) return 0;
+  return rp.total;
+}
+
+int sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, long long g_index_base,
+              long long g_index_stride, long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,
+              long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  const DeviceInfo* di = device_info();
+  if (!di) return -2;
+  if (int rc = require_sm90a(di, "sim_range")) return rc;
+  DCR_REQUIRE(!std::isnan(threshold), "sim_range: threshold is NaN");
+  DCR_REQUIRE(g_index_stride >= 1, "sim_range: g_index_stride=%lld < 1", g_index_stride);
+  RangePlan rp;
+  if (int rc = make_range_plan(nq, ng, d, max_pairs, di->num_sms, di->max_smem_optin, &rp)) return rc;
+  DCR_REQUIRE(ws != nullptr && ws_bytes >= rp.total, "sim_range: workspace too small (%zu < %zu)", ws_bytes, rp.total);
+  DCR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "sim_range: workspace must be 256-byte aligned");
+  DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0,
+              "sim_range: q/g must be 16-byte aligned");
+  const SweepGeometry& geo = rp.geo;
+  Carve w{static_cast<uint8_t*>(ws)};
+  const RangeBuffers b = carve_range(rp, nq, d, max_pairs, w);
+  const Operands& o = b.ops;
+  if (int rc = prepare_operands(q, nq, rp.nq_pad, g, ng, d, geo, di, o, stream)) return rc;
+  if (int rc = launch(range_threshold_kernel, (nq + 3) / 4, 128, 0, stream, "sim_range", q, nq, d, geo.d_pad, threshold,
+                      o.qnh, o.qnr, o.qnx, o.gmax, o.mu, o.nu, o.qflag, b.thr))
+    return rc;
+
+  CUtensorMap tq, tg;
+  RangeParams p;
+  if (int rc = sweep_setup(geo, nq, rp.n_qtiles, ng, geo.gchunk, geo.n_chunks, o.qb, o.gb, &p, &tq, &tg)) return rc;
+  p.stages = rp.stages;
+  p.bias_flag = o.qflag;
+  p.col_bias = o.bias;
+  p.thr = b.thr;
+  p.seg = b.seg;
+  p.row_cand = b.row_cand;
+  p.cand_idx = b.cand_idx;
+  auto sweep = [&](auto off, auto on) {
+    return launch_sweep(off, on, rp.n_units, 32 + 128, rp.smem_bytes, stream, "sim_range", tq, tg, p);
+  };
+  if (int rc = sweep(sim_range_kernel<false, false>, sim_range_kernel<true, false>)) return rc;
+  if (int rc = launch(range_slot_scan_kernel, (nq + 255) / 256, 256, 0, stream, "sim_range", b.seg, nq, rp.n_qtiles,
+                      geo.n_gtiles, geo.gchunk, geo.n_chunks, rp.n_units, b.row_cnt, b.row_pcnt))
+    return rc;
+  if (int rc = exclusive_scan_i64(b.row_cnt, nq, b.row_cand, stream)) return rc;
+  if (int rc = exclusive_scan_i64(b.row_pcnt, nq, b.row_piece, stream)) return rc;
+  long long h_tot[2] = {0, 0};   // candidates, pieces
+  DCR_CUDA_CHECK(cudaMemcpyAsync(h_tot, b.row_cand + nq, 8, cudaMemcpyDeviceToHost, stream));
+  DCR_CUDA_CHECK(cudaMemcpyAsync(h_tot + 1, b.row_piece + nq, 8, cudaMemcpyDeviceToHost, stream));
+  DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
+  const long long n_cand = h_tot[0], n_pieces = h_tot[1];
+  counts[0] = 0;
+  counts[1] = n_cand;
+  if (n_cand > max_pairs)
+    return set_error(DCR_ERR_CAPACITY, "sim_range: %lld candidate pairs exceed max_pairs=%lld (call again with that capacity)",
+                     n_cand, max_pairs);
+
+  if (n_pieces > 0) {
+    if (int rc = sweep(sim_range_kernel<false, true>, sim_range_kernel<true, true>)) return rc;
+    if (int rc = launch(range_rescore_kernel, static_cast<unsigned>(n_pieces), kRescoreThreads, static_cast<size_t>(d) * 8,
+                        stream, "sim_range", q, g, nq, d, threshold, b.row_cand, b.row_piece, b.cand_idx, b.cand_score,
+                        b.piece_kept))
+      return rc;
+  }
+  if (int rc = launch(exclusive_scan_kernel<int>, 1, 1024, 0, stream, "sim_range", b.piece_kept, n_pieces, b.piece_excl))
+    return rc;
+  if (n_pieces > 0) {
+    if (int rc = launch(range_output_kernel, static_cast<unsigned>(n_pieces), 256, 0, stream, "sim_range", b.row_cand,
+                        b.row_piece, nq, b.piece_excl, b.cand_idx, b.cand_score, g_index_base, g_index_stride, out_idx,
+                        out_scores))
+      return rc;
+  }
+  if (int rc = launch(range_row_offsets_kernel, grid_for(nq + 1, 256, di->num_sms), 256, 0, stream, "sim_range", b.row_piece,
+                      b.piece_excl, nq, row_offsets))
+    return rc;
+  long long h_pairs = 0;
+  DCR_CUDA_CHECK(cudaMemcpyAsync(&h_pairs, b.piece_excl + n_pieces, 8, cudaMemcpyDeviceToHost, stream));
+  DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
+  counts[0] = h_pairs;
+  return 0;
+}
+
+int exclusive_scan_i64(const long long* in, long long n, long long* out, cudaStream_t stream) {
+  return launch(exclusive_scan_kernel<long long>, 1, 1024, 0, stream, "exclusive_scan_i64", in, n, out);
+}
+
+}  // namespace dcr

@@ -33,8 +33,6 @@ constexpr int kMaxWorld = 65535;                            // ranks: the merge 
 constexpr long long kMaxLocalPairs = 1ll << 40;             // as sim_range's max_pairs
 enum { H_MAGIC, H_STATUS, H_PAIRS, H_CAND, H_CAND_CAP, H_MAX_PAIRS, H_NQ, H_D, H_THR, H_RESERVED };
 
-inline size_t up256(size_t x) { return (x + 255) / 256 * 256; }
-
 // bytes of a message holding `pairs` pairs: int64 offsets[nq + 1], int64 idx[pairs], fp32 scores[pairs], 16-byte multiple
 inline size_t msg_bytes(int nq, long long pairs) {
   return (8 * (static_cast<size_t>(nq) + 1) + 12 * static_cast<size_t>(pairs) + 15) / 16 * 16;
@@ -43,12 +41,17 @@ inline size_t msg_bytes(int nq, long long pairs) {
 // the header buffers [send | world receive slots] at the head of the workspace
 inline size_t header_bytes(int world) { return kHdrWords * sizeof(long long) * (static_cast<size_t>(world) + 1); }
 
+// The workspace: the header buffers, the local search's workspace, the send and receive buffers, the merged row counts
+// and a flag.  With a null base only L->total is meaningful.
 struct ShardLayout {
   size_t inner;                      // sim_range workspace of the local search
-  size_t off_inner, off_send, off_recv, off_row_cnt, off_flag, total;
+  uint8_t *inner_ws, *send, *recv;
+  long long* row_cnt;
+  int* flag;
+  size_t total;
 };
 
-int shard_layout(int nq, int ng_local, int d, int world, long long cap, ShardLayout* L) {
+int shard_layout(int nq, int ng_local, int d, int world, long long cap, void* base, ShardLayout* L) {
   DCR_REQUIRE(world >= 1 && world <= kMaxWorld, "sim_range_sharded: world=%d outside [1, %d]", world, kMaxWorld);
   DCR_REQUIRE(nq >= 1 && ng_local >= 0, "sim_range_sharded: bad problem (nq=%d ng_local=%d)", nq, ng_local);
   DCR_REQUIRE(cap >= 0 && cap <= kMaxLocalPairs, "sim_range_sharded: max_local_pairs=%lld outside [0, 2^40]", cap);
@@ -57,12 +60,14 @@ int shard_layout(int nq, int ng_local, int d, int world, long long cap, ShardLay
   if (L->inner == 0) return -1;
   if (ng_local == 0) L->inner = 0;
   const size_t msg = msg_bytes(nq, cap);
-  L->off_inner = up256(header_bytes(world));
-  L->off_send = L->off_inner + up256(L->inner);
-  L->off_recv = L->off_send + up256(msg);
-  L->off_row_cnt = L->off_recv + up256(msg * static_cast<size_t>(world));
-  L->off_flag = L->off_row_cnt + up256(static_cast<size_t>(nq) * 8);
-  L->total = L->off_flag + 256;
+  Carve w{static_cast<uint8_t*>(base)};
+  w.take<uint8_t>(header_bytes(world));
+  L->inner_ws = w.take<uint8_t>(L->inner);
+  L->send = w.take<uint8_t>(msg);
+  L->recv = w.take<uint8_t>(msg * static_cast<size_t>(world));
+  L->row_cnt = w.take<long long>(nq);
+  L->flag = w.take<int>(1);
+  L->total = w.bytes;
   return 0;
 }
 
@@ -161,7 +166,7 @@ struct HeaderBuf {
 
 size_t sim_range_sharded_workspace_size(int nq, int ng_local, int d, int world, long long max_local_pairs) {
   ShardLayout L;
-  if (shard_layout(nq, ng_local, d, world, max_local_pairs, &L) != 0) return 0;
+  if (shard_layout(nq, ng_local, d, world, max_local_pairs, nullptr, &L) != 0) return 0;
   return L.total;
 }
 
@@ -194,10 +199,10 @@ int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int 
     DCR_REQUIRE(!std::isnan(threshold), "sim_range_sharded: threshold is NaN");
     DCR_REQUIRE(g_index_stride >= 1, "sim_range_sharded: g_index_stride=%lld < 1", g_index_stride);
     DCR_REQUIRE(max_pairs >= 0, "sim_range_sharded: max_pairs=%lld < 0", max_pairs);
-    if (int rc = shard_layout(nq, ng_local, d, world, max_local_pairs, &L)) return rc;
+    if (int rc = shard_layout(nq, ng_local, d, world, max_local_pairs, w, &L)) return rc;
     DCR_REQUIRE(w != nullptr && ws_bytes >= L.total, "sim_range_sharded: workspace too small (%zu < %zu)", ws_bytes, L.total);
     DCR_REQUIRE((reinterpret_cast<uintptr_t>(w) & 255) == 0, "sim_range_sharded: workspace must be 256-byte aligned");
-    long long* send_off = reinterpret_cast<long long*>(w + L.off_send);
+    long long* send_off = reinterpret_cast<long long*>(L.send);
     if (ng_local == 0) {
       DCR_CUDA_CHECK(cudaMemsetAsync(send_off, 0, 8 * (static_cast<size_t>(nq) + 1), stream));
       return 0;
@@ -205,10 +210,10 @@ int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int 
     // indices go straight into the message; the scores wait in the (not yet used) receive buffer and follow the
     // indices once their count is known
     long long* send_idx = send_off + nq + 1;
-    float* tmp_scores = reinterpret_cast<float*>(w + L.off_recv);
+    float* tmp_scores = reinterpret_cast<float*>(L.recv);
     long long c[2] = {0, 0};
     const int rc = sim_range(q, nq, g, ng_local, d, threshold, g_index_base, g_index_stride, send_off, send_idx, tmp_scores,
-                             max_local_pairs, c, w + L.off_inner, L.inner, stream);
+                             max_local_pairs, c, L.inner_ws, L.inner, stream);
     hdr[H_CAND] = c[1];
     if (rc) return rc;
     hdr[H_PAIRS] = c[0];
@@ -273,16 +278,14 @@ int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int 
 
   // 3. the messages, each padded to the largest
   const size_t msg = msg_bytes(nq, p_max);
-  uint8_t* send = w + L.off_send;
-  uint8_t* recv = w + L.off_recv;
-  if (int rc = exchange(send, recv, msg)) return rc;
+  if (int rc = exchange(L.send, L.recv, msg)) return rc;
 
   // 4. the merge
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  long long* row_cnt = reinterpret_cast<long long*>(w + L.off_row_cnt);
-  int* bad = reinterpret_cast<int*>(w + L.off_flag);
-  const ShardMsgs m = {recv, msg, h_recv, nq, world};
+  long long* row_cnt = L.row_cnt;
+  int* bad = L.flag;
+  const ShardMsgs m = {L.recv, msg, h_recv, nq, world};
   const dim3 grid(static_cast<unsigned>(std::max(1, grid_for(std::max(p_max, 1ll), 256, di->num_sms) / world)),
                   static_cast<unsigned>(world));
   DCR_CUDA_CHECK(cudaMemsetAsync(bad, 0, 4, stream));

@@ -8,6 +8,7 @@
 //
 // The [Q,G] score matrix is never written.  Three stages, all on the caller's stream:
 //   1. to_bf16_rows_kernel   fp32 descriptors -> zero-padded bf16 rows + per-row norms of the rounding residual
+//                            (sim_sweep.cu, shared with the threshold search in sim_range.cu)
 //   2. sim_topk_kernel       wgmma bf16 GEMM (fp32 accumulate in registers) whose epilogue keeps, per query, the
 //                            kp (>= k) best approximate scores of its gallery segment (threshold filter on the
 //                            accumulator registers, warp-cooperative compaction in shared memory)
@@ -18,46 +19,22 @@
 //                            compute the same values.  Queries failing the certificate are recomputed by brute force in
 //                            fp64 (exact_scan_kernel / exact_select_kernel).
 // Result: indices identical to ranking all G exact dot products with ties broken by lowest index.
-//
-// The same stages 1 and 2 also serve the threshold search (sim_range: every pair scoring at least tau, exact, in CSR
-// form; it replaces the saved score matrices of diff_retrieval.py:402-403, 414-415 and the threshold of :454): the
-// fused sweep's epilogue then compares each approximate score against a per-row threshold that no qualifying pair can
-// fall below, and the candidates are re-scored with the same fp64 dot products.
-#include <cuda_bf16.h>
-
 #include <algorithm>
-#include <cmath>
 #include <type_traits>
 
 #include "../../include/dcr_b200.h"
 #include "dcr_internal.cuh"
-#include "host_util.cuh"
-#include "ptx.cuh"
+#include "sim_sweep.cuh"
 
 namespace dcr {
 
 namespace {
 
-constexpr int kBlockM = 128;      // query rows per CTA
-constexpr int kBlockN = 128;      // gallery rows per tile (accumulator columns: 128 registers per thread with one warpgroup)
-constexpr int kBlockK = 64;       // bf16 elements per 128-byte swizzled smem row
-constexpr int kMaxKB = 8;         // d_pad <= 512: the query tile stays resident in shared memory; larger: streamed
-constexpr int kMaxDim = 8192;     // largest descriptor dimension accepted
 constexpr int kKPMax = 32;        // max candidates kept per (query, segment)
 constexpr int kWarmTiles = 4;     // tiles replayed at the start of every segment to seed the threshold
-constexpr uint32_t kFull = 0xffffffffu;
-constexpr int kATileBytes = kBlockM * kBlockK * 2;  // 16 KB
-constexpr int kBTileBytes = kBlockN * kBlockK * 2;  // 16 KB
 constexpr int kMaxSlotsPerQuery = 512;  // (chunk, unit) segments that may cover one q-tile
 
-struct SimParams {
-  int nq, ng;
-  int num_kb;          // d_pad / 64
-  int stream_a;        // 1 (d_pad > 512): query k-blocks travel with the gallery k-blocks instead of staying resident
-  int n_qtiles;        // ceil(nq / 128)
-  int n_gtiles;        // ceil(ng / 128)
-  int gchunk;          // gallery tiles per L2-sized chunk (all units sweep chunk c before chunk c+1)
-  int n_chunks;
+struct SimParams : SweepHead {
   int kp;              // candidates kept per (query, segment): 8, 16 or 32
   int cap;             // shared-memory list capacity per query row (kp + 16 .. 64)
   int stages;          // B pipeline depth
@@ -71,192 +48,6 @@ struct SimParams {
                            // unsigned key (0 = none)
   unsigned long long* clk; // [4] clock64 / globaltimer at the start and end of CTA 0 (SM clock under this kernel); null = off
 };
-
-// ------------------------------------------------------------------------------------------------------------
-// stage 1: fp32 rows -> bf16 rows (zero padded to [n_pad, d_pad]) + norms needed by the error bound
-//   norms[0][r] = ||bf16(x_r)||, norms[1][r] = ||x_r - bf16(x_r)||, gmax[0] = max_r ||x_r||, gmax[1] = max_r residual
-// mu (optional): a vector subtracted from every row before rounding (gallery centring: q.g = q.(g-mu) + q.mu and the
-// second term does not depend on g, so the ranking is unchanged while the bf16 rounding error now scales with the
-// SPREAD of the gallery instead of its norm).
-template <int kIter>
-__global__ void __launch_bounds__(256) to_bf16_rows_kernel(const float* __restrict__ x, int n, int d, int n_pad, int d_pad,
-                                    const float* __restrict__ mu, __nv_bfloat16* __restrict__ out,
-                                    float* __restrict__ norm_hat, float* __restrict__ norm_res,
-                                    float* __restrict__ norm_x, unsigned int* __restrict__ gmax,
-                                    const float* __restrict__ nu, float* __restrict__ bias_out,
-                                    const int* __restrict__ mu_flag, const int* __restrict__ nu_flag) {
-  if (mu_flag && *mu_flag == 0) mu = nullptr;   // device-side decision (centre_decision_kernel)
-  if (nu_flag && *nu_flag == 0) nu = nullptr;
-  const int warps_per_block = blockDim.x >> 5;
-  const int lane = threadIdx.x & 31;
-  // gmax: one global atomic per BLOCK (100k same-address atomics, one per row, serialise in L2 and dominated this kernel)
-  __shared__ unsigned int s_gmax[2];
-  if (threadIdx.x < 2) s_gmax[threadIdx.x] = 0u;
-  __syncthreads();
-  unsigned int w_nx = 0u, w_nr = 0u;   // this warp's running maxima (lane 0)
-  for (int row = blockIdx.x * warps_per_block + (threadIdx.x >> 5); row < n_pad; row += gridDim.x * warps_per_block) {
-    float s_hat = 0.f, s_res = 0.f, s_x = 0.f;
-    double s_bias = 0.0;   // nu . (x - mu) in fp64: the per-gallery-row score offset of query centring
-    __nv_bfloat16* o = out + static_cast<size_t>(row) * d_pad;
-    if (row < n) {
-      const float* xr = x + static_cast<size_t>(row) * d;
-      // kIter float4 loads per lane issued back to back (the row's whole HBM read is in flight before the first value
-      // is used: the kernel is a pure stream, 12 B/element read+written, and was latency bound with one load at a time)
-      for (int c0 = 0; c0 < d_pad; c0 += 128 * kIter) {
-        float4 v[kIter];
-#pragma unroll
-        for (int i = 0; i < kIter; ++i) {
-          const int c = c0 + i * 128 + lane * 4;
-          v[i] = (c + 3 < d) ? *reinterpret_cast<const float4*>(xr + c) : make_float4(0.f, 0.f, 0.f, 0.f);   // d % 4 == 0
-        }
-#pragma unroll
-        for (int i = 0; i < kIter; ++i) {
-          const int c = c0 + i * 128 + lane * 4;
-          if (c >= d_pad) continue;
-          if (c + 3 < d) {
-            if (mu) {
-              const float4 m = *reinterpret_cast<const float4*>(mu + c);
-              v[i].x -= m.x; v[i].y -= m.y; v[i].z -= m.z; v[i].w -= m.w;
-            }
-            if (nu) {
-              const float4 u = *reinterpret_cast<const float4*>(nu + c);
-              s_bias = fma(static_cast<double>(u.x), static_cast<double>(v[i].x), s_bias);
-              s_bias = fma(static_cast<double>(u.y), static_cast<double>(v[i].y), s_bias);
-              s_bias = fma(static_cast<double>(u.z), static_cast<double>(v[i].z), s_bias);
-              s_bias = fma(static_cast<double>(u.w), static_cast<double>(v[i].w), s_bias);
-            }
-          }
-          const __nv_bfloat16 h0 = __float2bfloat16_rn(v[i].x), h1 = __float2bfloat16_rn(v[i].y);
-          const __nv_bfloat16 h2 = __float2bfloat16_rn(v[i].z), h3 = __float2bfloat16_rn(v[i].w);
-          const float f0 = __bfloat162float(h0), f1 = __bfloat162float(h1), f2 = __bfloat162float(h2), f3 = __bfloat162float(h3);
-          s_hat += f0 * f0 + f1 * f1 + f2 * f2 + f3 * f3;
-          s_res += (v[i].x - f0) * (v[i].x - f0) + (v[i].y - f1) * (v[i].y - f1) + (v[i].z - f2) * (v[i].z - f2) + (v[i].w - f3) * (v[i].w - f3);
-          s_x += v[i].x * v[i].x + v[i].y * v[i].y + v[i].z * v[i].z + v[i].w * v[i].w;
-          uint2 pk;
-          pk.x = static_cast<uint32_t>(__bfloat16_as_ushort(h0)) | (static_cast<uint32_t>(__bfloat16_as_ushort(h1)) << 16);
-          pk.y = static_cast<uint32_t>(__bfloat16_as_ushort(h2)) | (static_cast<uint32_t>(__bfloat16_as_ushort(h3)) << 16);
-          *reinterpret_cast<uint2*>(o + c) = pk;
-        }
-      }
-    } else {
-      for (int c = lane * 2; c < d_pad; c += 64) *reinterpret_cast<uint32_t*>(o + c) = 0u;
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      s_hat += __shfl_xor_sync(kFull, s_hat, off);
-      s_res += __shfl_xor_sync(kFull, s_res, off);
-      s_x += __shfl_xor_sync(kFull, s_x, off);
-      s_bias += __shfl_xor_sync(kFull, s_bias, off);
-    }
-    if (lane == 0 && bias_out) bias_out[row] = (row < n) ? static_cast<float>(s_bias) : 0.f;
-    if (lane == 0 && row < n) {
-      // 1.0001: cover the fp32 rounding of the squared sums so the stored values are upper bounds
-      float nh = sqrtf(s_hat) * 1.0001f, nr = sqrtf(s_res) * 1.0001f, nx = sqrtf(s_x) * 1.0001f;
-      if (norm_hat) norm_hat[row] = nh;
-      if (norm_res) norm_res[row] = nr;
-      if (norm_x) norm_x[row] = nx;
-      w_nx = max(w_nx, __float_as_uint(nx));     // non-negative floats order like their bit patterns
-      w_nr = max(w_nr, __float_as_uint(nr));
-    }
-  }
-  if (gmax) {
-    if (lane == 0) {
-      atomicMax(&s_gmax[0], w_nx);
-      atomicMax(&s_gmax[1], w_nr);
-    }
-    __syncthreads();
-    if (threadIdx.x < 2) atomicMax(gmax + threadIdx.x, s_gmax[threadIdx.x]);
-  }
-}
-
-// column sums of x[n, d] accumulated in double; mean = sum / n afterwards (rows r*row_stride, r < n: any fixed vector works
-// as the centre, so a strided sample of the gallery is enough).  A thread owns one 16-byte column group and a slice of the
-// block's rows (independent loads, four in flight), the slices meet in shared memory and the block does ONE atomicAdd per
-// column instead of every block adding all d columns (hundreds of thousands of same-address double atomics).
-constexpr int kColSumThreads = 512;
-__global__ void __launch_bounds__(kColSumThreads)
-    col_sum_kernel(const float* __restrict__ x, int n, int row_stride, int d, double* __restrict__ sums,
-                   double* __restrict__ sq_sums) {
-  __shared__ double red[kColSumThreads][8];
-  const int groups = d >> 2;                                   // d % 4 == 0 (checked by the caller)
-  const int G = min(groups, kColSumThreads), S = kColSumThreads / G;
-  const int tg = threadIdx.x % G, sl = threadIdx.x / G;         // threads with sl >= S idle (G does not divide the block)
-  const int rows_per_block = (n + gridDim.x - 1) / gridDim.x;
-  const int r0 = blockIdx.x * rows_per_block, r1 = min(n, r0 + rows_per_block);
-  for (int cg = tg; cg < groups; cg += G) {
-    double da[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) da[e] = 0.0;
-    if (sl < S) {
-      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f), acc2 = make_float4(0.f, 0.f, 0.f, 0.f);
-      int cnt = 0;
-#pragma unroll 4
-      for (int r = r0 + sl; r < r1; r += S) {
-        const float4 v = *reinterpret_cast<const float4*>(x + static_cast<size_t>(r) * row_stride * d + cg * 4);
-        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-        acc2.x += v.x * v.x; acc2.y += v.y * v.y; acc2.z += v.z * v.z; acc2.w += v.w * v.w;
-        if (++cnt == 256) {   // flush the fp32 partials into the double accumulators every 256 rows
-          da[0] += acc.x; da[1] += acc.y; da[2] += acc.z; da[3] += acc.w;
-          da[4] += acc2.x; da[5] += acc2.y; da[6] += acc2.z; da[7] += acc2.w;
-          acc = make_float4(0.f, 0.f, 0.f, 0.f);
-          acc2 = make_float4(0.f, 0.f, 0.f, 0.f);
-          cnt = 0;
-        }
-      }
-      da[0] += acc.x; da[1] += acc.y; da[2] += acc.z; da[3] += acc.w;
-      da[4] += acc2.x; da[5] += acc2.y; da[6] += acc2.z; da[7] += acc2.w;
-    }
-#pragma unroll
-    for (int e = 0; e < 8; ++e) red[threadIdx.x][e] = da[e];
-    __syncthreads();
-    if (sl == 0 && r1 > r0) {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        double t = 0.0;
-        for (int s2 = 0; s2 < S; ++s2) t += red[s2 * G + tg][e];   // fixed order within the block
-        if (e < 4) atomicAdd(sums + cg * 4 + e, t);
-        else if (sq_sums) atomicAdd(sq_sums + cg * 4 + (e - 4), t);
-      }
-    }
-    __syncthreads();
-  }
-}
-__global__ void col_mean_finish_kernel(const double* __restrict__ sums, int n, int d, float* __restrict__ mu) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < d) mu[c] = static_cast<float>(sums[c] / n);
-}
-// Query centring pays only when the centred queries are much shorter than the queries themselves (the bf16 error
-// bound shrinks by ||q-nu|| / ||q||) -- and costs a per-column offset in the fused epilogue.  flag = 1 when the
-// mean squared norm of the centred sample is below 1/16 of the uncentred one (a 4x tighter bound).
-__global__ void __launch_bounds__(256)
-    centre_decision_kernel(const double* __restrict__ sums, const double* __restrict__ sq_sums, int n, int d,
-                           int* __restrict__ flag) {
-  __shared__ double s_m2[8], s_nu2[8];
-  double m2 = 0.0, nu2 = 0.0;
-  for (int c = threadIdx.x; c < d; c += blockDim.x) {
-    m2 += sq_sums[c] / n;
-    const double m = sums[c] / n;
-    nu2 += m * m;
-  }
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) {
-    m2 += __shfl_xor_sync(kFull, m2, off);
-    nu2 += __shfl_xor_sync(kFull, nu2, off);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    s_m2[threadIdx.x >> 5] = m2;
-    s_nu2[threadIdx.x >> 5] = nu2;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    m2 = nu2 = 0.0;
-    for (int w = 0; w < 8; ++w) {
-      m2 += s_m2[w];
-      nu2 += s_nu2[w];
-    }
-    *flag = (m2 - nu2 < m2 / 16.0) ? 1 : 0;
-  }
-}
 
 // second-chance pass: copy the bf16 rows of the flagged queries into a compact matrix (zero rows up to n_pad)
 __global__ void gather_rows_kernel(const __nv_bfloat16* __restrict__ src, const int* __restrict__ rows, int n, int n_pad,
@@ -441,180 +232,6 @@ DCR_DEVICE float seed_threshold(float (&slot)[32], int kp) {
   return thr;
 }
 
-// Work decomposition shared by the three warp roles and rescore_select_kernel: for every gallery chunk c (chunks are
-// L2-sized so that the units, which all sweep chunk c at about the same time, share its tiles in L2) the
-// (q-tile, g-tile-in-chunk) grid is linearised q-major into T tiles and cut into n_units equal contiguous ranges, unit u
-// owning [u*T/U, (u+1)*T/U); a unit's range is walked as segments = maximal runs inside one q-tile.
-
-// owner unit of linear tile t
-DCR_DEVICE long long owner_unit(long long t, long long T, long long U) { return ((t + 1) * U + T - 1) / T - 1; }
-
-// Candidate slot of the segment (chunk, unit, q-tile qi) and epilogue set: the q-tiles of a unit's range never lie below
-// those of the previous unit, so unit + qi is distinct within a chunk and below n_units + n_qtiles.
-DCR_DEVICE int slot_index(int chunk, int unit, int qi, int set, int n_units, int n_qtiles, int n_sets) {
-  return (chunk * (n_units + n_qtiles) + unit + qi) * n_sets + set;
-}
-
-// Thresholds carry over from chunk to chunk: `carried` says that this unit finished a segment of the same q-tile before
-// (its final per-row thresholds are valid lower bounds, so no warm-up replay is needed).
-struct SegWalker {
-  int n_qtiles, n_gtiles, gchunk, n_chunks;
-  long long unit, n_units;
-  // current segment
-  int chunk, qi, g_begin, ntiles;
-  bool carried;
-  // state
-  long long t, t_end;
-  int ncg, g_lo;
-  int tag[4];
-  __device__ SegWalker(int nq_t, int ng_t, int gc, int nc, long long u, long long nu)
-      : n_qtiles(nq_t), n_gtiles(ng_t), gchunk(gc), n_chunks(nc), unit(u), n_units(nu), chunk(-1), t(0), t_end(0) {
-    tag[0] = tag[1] = tag[2] = tag[3] = -1;
-  }
-  __device__ bool next() {
-    if (chunk >= 0) {   // close the previous segment
-      const int s4 = qi & 3;
-      if (s4 == 0) tag[0] = qi; else if (s4 == 1) tag[1] = qi; else if (s4 == 2) tag[2] = qi; else tag[3] = qi;
-    }
-    while (t >= t_end) {
-      ++chunk;
-      if (chunk >= n_chunks) return false;
-      g_lo = chunk * gchunk;
-      ncg = min(gchunk, n_gtiles - g_lo);
-      const long long T = static_cast<long long>(n_qtiles) * ncg;
-      t = unit * T / n_units;
-      t_end = (unit + 1) * T / n_units;
-    }
-    qi = static_cast<int>(t / ncg);
-    g_begin = g_lo + static_cast<int>(t % ncg);
-    const long long seg_end = min(t_end, static_cast<long long>(qi + 1) * ncg);
-    ntiles = static_cast<int>(seg_end - t);
-    const int s4 = qi & 3;
-    const int tg = s4 == 0 ? tag[0] : (s4 == 1 ? tag[1] : (s4 == 2 ? tag[2] : tag[3]));
-    carried = (tg == qi);
-    t = seg_end;
-    return true;
-  }
-};
-
-// Shared-memory pipeline of a fused sweep (sim_topk_kernel, sim_range_kernel):
-//   resident mode: [num_kb x 16 KB query tile][stages x gallery tile]; streamed mode (d_pad > 512, the query tile no
-//   longer fits): [stages x (gallery tile | 16 KB query k-block)] -- twice the L2->SMEM traffic per FLOP
-// followed by `list_bytes` of the caller's own, the barriers, and whatever the caller puts after them (`tail`).
-struct FusedPipe {
-  bool stream_a;
-  int num_kb, stage_bytes;
-  uint8_t* smem_a;     // num_kb x 16 KB (resident mode)
-  uint8_t* smem_b;     // stages x stage_bytes
-  uint8_t* lists;
-  uint64_t *b_full, *b_empty, *a_full, *a_empty;
-  uint8_t* tail;
-  DCR_DEVICE FusedPipe(uint8_t* smem_raw, int nkb, int stream, int stages, size_t list_bytes) {
-    // all tile bases 1024-byte aligned for the 128B swizzle
-    uint8_t* smem = smem_align1024(smem_raw);
-    stream_a = stream != 0;
-    num_kb = nkb;
-    stage_bytes = kBlockN * kBlockK * 2 + (stream_a ? kATileBytes : 0);
-    smem_a = smem;
-    smem_b = smem_a + (stream_a ? 0 : num_kb * kATileBytes);
-    lists = smem_b + stages * stage_bytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(lists + list_bytes);
-    b_full = bars;          // [stages]
-    b_empty = bars + 8;     // [stages]
-    a_full = bars + 16;
-    a_empty = bars + 17;
-    tail = reinterpret_cast<uint8_t*>(bars + 32);
-  }
-  // producer warp = consumer_warps (the last warp); every thread of the CTA calls this
-  DCR_DEVICE void init(const CUtensorMap* tq, const CUtensorMap* tg, int stages, uint32_t consumer_warps) const {
-    const uint32_t warp = threadIdx.x >> 5;
-    if (warp == consumer_warps && elect_one()) {
-      tma_prefetch_desc(tq);
-      tma_prefetch_desc(tg);
-    }
-    if (warp == 0 && elect_one()) {
-      for (int s = 0; s < stages; ++s) {
-        mbar_init(&b_full[s], 1);
-        mbar_init(&b_empty[s], consumer_warps);   // one arrive per consumer warp
-      }
-      mbar_init(a_full, 1);
-      mbar_init(a_empty, consumer_warps);
-      fence_mbar_init();
-    }
-    __syncthreads();
-  }
-};
-
-// TMA producer of a fused sweep.  The whole warp walks the loop (warp-uniform values stay in uniform registers) and one
-// elected lane issues.  Per segment: the query tile (resident mode), then warm + ntiles gallery tiles of num_kb k-blocks,
-// the first `warm` of them replayed from the segment start; warm_of(walker) says how many.
-template <class WarmOf>
-DCR_DEVICE void fused_producer(const FusedPipe& pp, const CUtensorMap* tq, const CUtensorMap* tg, int stages, SegWalker& w,
-                               WarmOf warm_of) {
-  uint32_t seg = 0;
-  PipeState st(stages);
-  while (w.next()) {
-    const int qi = w.qi, g_begin = w.g_begin, ntiles = w.ntiles;
-    const int warm = warm_of(w);
-    const int q_row = qi * kBlockM;
-    if (!pp.stream_a) {   // resident query tile
-      mbar_wait(pp.a_empty, (seg & 1) ^ 1);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(pp.a_full, pp.num_kb * kATileBytes);
-        for (int kb = 0; kb < pp.num_kb; ++kb)
-          tma_load_2d(pp.smem_a + kb * kATileBytes, tq, pp.a_full, kb * kBlockK, q_row, kEvictNormal);
-      }
-      __syncwarp();
-    }
-    for (int j = 0; j < warm + ntiles; ++j) {
-      const int gi = g_begin + (j < warm ? j : j - warm);
-      const int g_row = gi * kBlockN;
-      for (int kb = 0; kb < pp.num_kb; ++kb, st.next()) {
-        const uint32_t s = st.s, ph = st.ph;
-        mbar_wait(&pp.b_empty[s], ph ^ 1);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(&pp.b_full[s], pp.stage_bytes);
-          tma_load_2d(pp.smem_b + s * pp.stage_bytes, tg, &pp.b_full[s], kb * kBlockK, g_row, kEvictNormal);
-          if (pp.stream_a)
-            tma_load_2d(pp.smem_b + s * pp.stage_bytes + kBTileBytes, tq, &pp.b_full[s], kb * kBlockK, q_row, kEvictNormal);
-        }
-        __syncwarp();
-      }
-    }
-    ++seg;
-  }
-}
-
-// One 128-row accumulator tile of a consumer warpgroup: the wgmma k-loop over the pipeline stages.  The stage of k-block
-// kb is released once wgmma_wait<1> in k-block kb+1 has seen its MMAs complete; `last` also releases the resident query
-// tile (last tile of the segment).  a_base / b_base: shared addresses of the query tile and of this warpgroup's columns
-// of gallery stage 0.
-template <int kCols>
-DCR_DEVICE void fused_tile_mma(WgAcc<kCols>& acc, PipeState& st, const FusedPipe& pp, uint32_t a_base, uint32_t b_base,
-                               bool last, uint32_t lane) {
-  const uint32_t a_step = pp.stream_a ? 0u : static_cast<uint32_t>(kATileBytes);   // per k-block (resident query tile)
-  uint32_t prev_s = 0;
-  for (int kb = 0; kb < pp.num_kb; ++kb, st.next()) {
-    const uint32_t s = st.s;
-    mbar_wait(&pp.b_full[s], st.ph);
-    const uint32_t a_addr = a_base + (pp.stream_a ? s * static_cast<uint32_t>(pp.stage_bytes) : static_cast<uint32_t>(kb) * a_step);
-    const uint32_t b_addr = b_base + s * static_cast<uint32_t>(pp.stage_bytes);
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < kBlockK / 16; ++k) acc.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), (kb | k) != 0);
-    wgmma_commit();
-    wgmma_wait<1>();
-    if (kb > 0 && lane == 0) mbar_arrive(&pp.b_empty[prev_s]);
-    prev_s = s;
-  }
-  wgmma_wait<0>();
-  acc.fence_regs();
-  if (lane == 0) {
-    mbar_arrive(&pp.b_empty[prev_s]);
-    if (!pp.stream_a && last) mbar_arrive(pp.a_empty);
-  }
-}
-
 // ------------------------------------------------------------------------------------------------------------
 // stage 2: the fused kernel.  One CTA per work unit; kSets consumer warpgroups (warps 0 .. 4 kSets - 1) each issue the
 // wgmma for their column range of every 128 x 128 tile (fp32 accumulators in registers) and filter it; the last warp is
@@ -774,61 +391,19 @@ __global__ void __launch_bounds__(32 + 128 * kSets, 1)
   }
 }
 
-// ------------------------------------------------------------------------------------------------------------
-// exact dot product, fp64 accumulate, fixed association: lane l owns elements l*4 + 128*i (float4 granules),
-// accumulates them in order, then a fixed xor-butterfly.  Used by both the re-score and the brute-force path so
-// that the two produce bit-identical values.
-DCR_DEVICE double exact_dot_warp(const float* __restrict__ a_smem, const float* __restrict__ b, int d, uint32_t lane) {
-  double acc = 0.0;
-  for (int c = lane * 4; c < d; c += 128) {
-    if (c + 3 < d) {
-      const float4 bv = *reinterpret_cast<const float4*>(b + c);
-      acc = fma(static_cast<double>(a_smem[c]), static_cast<double>(bv.x), acc);
-      acc = fma(static_cast<double>(a_smem[c + 1]), static_cast<double>(bv.y), acc);
-      acc = fma(static_cast<double>(a_smem[c + 2]), static_cast<double>(bv.z), acc);
-      acc = fma(static_cast<double>(a_smem[c + 3]), static_cast<double>(bv.w), acc);
-    } else {
-      for (int e = c; e < d; ++e) acc = fma(static_cast<double>(a_smem[e]), static_cast<double>(b[e]), acc);
-    }
-  }
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(kFull, acc, off);
-  return acc;
-}
-
-// Same values, same association as exact_dot_warp with the query row already widened to fp64 in shared memory (the widening
-// is exact): the re-score kernel is bound by the fp64 pipe -- per gallery row 512 fma plus 1024 fp32->fp64 conversions --
-// and this halves the conversions.
-DCR_DEVICE double exact_dot_warp_qd(const double* __restrict__ a_smem, const float* __restrict__ b, int d, uint32_t lane) {
-  double acc = 0.0;
-  for (int c = lane * 4; c < d; c += 128) {
-    if (c + 3 < d) {
-      const float4 bv = *reinterpret_cast<const float4*>(b + c);
-      const double2 a01 = *reinterpret_cast<const double2*>(a_smem + c);
-      const double2 a23 = *reinterpret_cast<const double2*>(a_smem + c + 2);
-      acc = fma(a01.x, static_cast<double>(bv.x), acc);
-      acc = fma(a01.y, static_cast<double>(bv.y), acc);
-      acc = fma(a23.x, static_cast<double>(bv.z), acc);
-      acc = fma(a23.y, static_cast<double>(bv.w), acc);
-    } else {
-      for (int e = c; e < d; ++e) acc = fma(a_smem[e], static_cast<double>(b[e]), acc);
-    }
-  }
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(kFull, acc, off);
-  return acc;
-}
-
 // order (score desc, index asc)
 DCR_DEVICE bool better(double s, long long i, double bs, long long bi) { return (s > bs) || (s == bs && i < bi); }
 
-// block-wide arg-best over (key desc, index asc) of 128 threads; every thread passes its local best (pos < 0 = none)
+// block-wide arg-best over (key desc, index asc) of kWarps warps; every thread passes its local best (pos < 0 = none) and
+// receives the block's
+template <int kWarps>
 struct BlockBest {
-  double key[4];
-  long long idx[4];
-  int pos[4];
+  double key[kWarps];
+  long long idx[kWarps];
+  int pos[kWarps];
 };
-DCR_DEVICE void block_argbest(double& bs, long long& bi, int& bp, BlockBest* sb, uint32_t lane, uint32_t warp) {
+template <int kWarps>
+DCR_DEVICE void block_argbest(double& bs, long long& bi, int& bp, BlockBest<kWarps>* sb, uint32_t lane, uint32_t warp) {
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) {
     const double os = __shfl_xor_sync(kFull, bs, off);
@@ -850,75 +425,13 @@ DCR_DEVICE void block_argbest(double& bs, long long& bi, int& bp, BlockBest* sb,
   bi = sb->idx[0];
   bp = sb->pos[0];
 #pragma unroll
-  for (int w = 1; w < 4; ++w)
+  for (int w = 1; w < kWarps; ++w)
     if (sb->pos[w] >= 0 && (bp < 0 || better(sb->key[w], sb->idx[w], bs, bi))) {
       bs = sb->key[w];
       bi = sb->idx[w];
       bp = sb->pos[w];
     }
   __syncthreads();
-}
-
-// two rows, each with exactly the association of exact_dot_warp_qd; both rows' loads are issued before the first fma
-DCR_DEVICE void exact_dot_warp_qd2(const double* __restrict__ a_smem, const float* __restrict__ b0,
-                                   const float* __restrict__ b1, int d, uint32_t lane, double& out0, double& out1) {
-  double acc0 = 0.0, acc1 = 0.0;
-  if ((d & 127) == 0 && d <= 512) {
-    // every lane owns d/128 whole 16-byte granules of each row: all (up to eight) loads are issued before the first fma --
-    // written as a loop, each 128-column step waited for its own two loads (40 serial memory latencies per query)
-    float4 v0[4], v1[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      if (i * 128 < d) {
-        v0[i] = *reinterpret_cast<const float4*>(b0 + lane * 4 + i * 128);
-        v1[i] = *reinterpret_cast<const float4*>(b1 + lane * 4 + i * 128);
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      if (i * 128 < d) {
-        const double2 a01 = *reinterpret_cast<const double2*>(a_smem + lane * 4 + i * 128);
-        const double2 a23 = *reinterpret_cast<const double2*>(a_smem + lane * 4 + i * 128 + 2);
-        acc0 = fma(a01.x, static_cast<double>(v0[i].x), acc0);
-        acc0 = fma(a01.y, static_cast<double>(v0[i].y), acc0);
-        acc0 = fma(a23.x, static_cast<double>(v0[i].z), acc0);
-        acc0 = fma(a23.y, static_cast<double>(v0[i].w), acc0);
-        acc1 = fma(a01.x, static_cast<double>(v1[i].x), acc1);
-        acc1 = fma(a01.y, static_cast<double>(v1[i].y), acc1);
-        acc1 = fma(a23.x, static_cast<double>(v1[i].z), acc1);
-        acc1 = fma(a23.y, static_cast<double>(v1[i].w), acc1);
-      }
-    }
-  } else {
-    for (int c = lane * 4; c < d; c += 128) {
-      if (c + 3 < d) {
-        const float4 v0 = *reinterpret_cast<const float4*>(b0 + c);
-        const float4 v1 = *reinterpret_cast<const float4*>(b1 + c);
-        const double2 a01 = *reinterpret_cast<const double2*>(a_smem + c);
-        const double2 a23 = *reinterpret_cast<const double2*>(a_smem + c + 2);
-        acc0 = fma(a01.x, static_cast<double>(v0.x), acc0);
-        acc0 = fma(a01.y, static_cast<double>(v0.y), acc0);
-        acc0 = fma(a23.x, static_cast<double>(v0.z), acc0);
-        acc0 = fma(a23.y, static_cast<double>(v0.w), acc0);
-        acc1 = fma(a01.x, static_cast<double>(v1.x), acc1);
-        acc1 = fma(a01.y, static_cast<double>(v1.y), acc1);
-        acc1 = fma(a23.x, static_cast<double>(v1.z), acc1);
-        acc1 = fma(a23.y, static_cast<double>(v1.w), acc1);
-      } else {
-        for (int e = c; e < d; ++e) {
-          acc0 = fma(a_smem[e], static_cast<double>(b0[e]), acc0);
-          acc1 = fma(a_smem[e], static_cast<double>(b1[e]), acc1);
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) {
-    acc0 += __shfl_xor_sync(kFull, acc0, off);
-    acc1 += __shfl_xor_sync(kFull, acc1, off);
-  }
-  out0 = acc0;
-  out1 = acc1;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -931,8 +444,6 @@ DCR_DEVICE void exact_dot_warp_qd2(const double* __restrict__ a_smem, const floa
 //   3. exact fp64 scores of the survivors, selection by (score desc, index asc)
 //   4. certificate against the rows the fused kernel dropped; failures are appended to `flagged` together with
 //      a threshold for the second-chance pass (thr_next).
-constexpr int kRescoreThreads = 128;   // block size of both widths
-
 struct RescoreParams {
   const float* q;                   // the caller's query rows [*][d]
   const float* g;                   // [ng][d]
@@ -972,107 +483,6 @@ struct RescoreSmem {
     bytes = kc + mc * 4;
   }
 };
-
-// Collectives of a group.  Every thread of the group calls them; the 128-wide forms go through a 4-entry shared array.
-template <int kThreads>
-DCR_DEVICE void group_sync() {
-  if constexpr (kThreads == 32) __syncwarp();
-  else __syncthreads();
-}
-
-// float or double; fmax ignores NaN
-template <int kThreads, typename T>
-DCR_DEVICE T group_max(T v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(kFull, v, o));
-  if constexpr (kThreads > 32) {
-    __shared__ T part[4];
-    __syncthreads();   // the previous call's readers are done
-    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
-    __syncthreads();
-    v = fmax(fmax(part[0], part[1]), fmax(part[2], part[3]));
-  }
-  return v;
-}
-
-// exclusive prefix sum over the group in thread order; total = the group's sum
-template <int kThreads>
-DCR_DEVICE int group_scan(int v, int& total) {
-  const int lane = threadIdx.x & 31;
-  int incl = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(kFull, incl, o);
-    if (lane >= o) incl += t;
-  }
-  total = __shfl_sync(kFull, incl, 31);
-  if constexpr (kThreads == 32) {
-    return incl - v;
-  } else {
-    __shared__ int part[4];
-    const int w = threadIdx.x >> 5;
-    __syncthreads();
-    if (lane == 0) part[w] = total;
-    __syncthreads();
-    for (int i = 0; i < w; ++i) incl += part[i];
-    total = part[0] + part[1] + part[2] + part[3];
-    return incl - v;
-  }
-}
-
-// How far an approximate score of the fused sweeps can lie from the exact one, for query row qrow.  Whole warp; q is the
-// query row (fp32 in global memory or already widened to fp64 in shared memory: the same values).
-//   eps   bounds |tensor-core score of (bf16 q', bf16 (g-mu)) (+ the column offset nu.(g-mu)) - q.(g-mu)| from the
-//         measured norms (DESIGN.md section 4): bf16 rounding of both operands, fp32 accumulation, fp32 roundings of
-//         q - nu, g - mu, the offset and its addition
-//   qmu   q . mu in fp64: the constant the centred approximate scores are offset by
-//   slack covers the fp64 rounding of an exact score and of q.mu themselves (each a d-term dot of vectors no longer than
-//         (|q'| + |nu|), (|g'| + |mu|)): irrelevant next to eps except when the centred gallery is (nearly) zero -- all
-//         rows identical -- and eps with it
-// So the fp64 score of a pair whose approximate score is a satisfies  s <= a + eps + qmu + slack  and
-// s >= a - eps + qmu - slack.
-struct RowBound {
-  float eps;
-  double qmu, slack;
-};
-template <typename TQ>
-DCR_DEVICE RowBound row_bound(const TQ* __restrict__ q, int d, int d_pad, int qrow, const float* __restrict__ q_norm_hat,
-                              const float* __restrict__ q_norm_res, const float* __restrict__ q_norm_x,
-                              const unsigned int* __restrict__ g_max, const float* __restrict__ mu,
-                              const float* __restrict__ nu, const int* __restrict__ nu_flag, uint32_t lane) {
-  const float g_norm = __uint_as_float(g_max[0]), g_res = __uint_as_float(g_max[1]);
-  const float qh = q_norm_hat[qrow], qr = q_norm_res[qrow], qx = q_norm_x[qrow];
-  float eps = 1.001f * (qh * g_res + qr * g_norm) + d_pad * 2.4e-7f * qh * (g_norm + g_res) + 1e-30f;
-  float nun = 0.f, mun = 0.f;   // |nu|, |mu| (upper bounds)
-  {
-    float acc = 0.f;
-    if (nu && nu_flag && *nu_flag)
-      for (int c = lane; c < d; c += 32) acc += nu[c] * nu[c];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
-    nun = sqrtf(acc) * 1.001f;
-    eps += 3e-7f * (qx + nun) * g_norm;
-  }
-  double qmu = 0.0;
-  {
-    float mu2 = 0.f;
-    for (int c = lane; c < d; c += 32) {
-      qmu = fma(static_cast<double>(q[c]), static_cast<double>(mu[c]), qmu);
-      mu2 = fmaf(mu[c], mu[c], mu2);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      qmu += __shfl_xor_sync(kFull, qmu, o);
-      mu2 += __shfl_xor_sync(kFull, mu2, o);
-    }
-    mun = sqrtf(mu2) * 1.001f;
-  }
-  RowBound rb;
-  rb.eps = eps;
-  rb.qmu = qmu;
-  rb.slack = 4.6e-16 * (d + 8) * static_cast<double>(qx + nun) * static_cast<double>(g_norm + mun);
-  return rb;
-}
 
 template <int kThreads>
 __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const RescoreParams p) {
@@ -1213,8 +623,8 @@ __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const R
   // ---- exact scores of the survivors (two rows in flight per warp), then selection by (score desc, index asc) ----
   for (int c = 2 * warp; c < m; c += 2 * kWarps) {
     double v0, v1 = 0.0;
-    if (c + 1 < m) exact_dot_warp_qd2(qs, p.g + static_cast<size_t>(kc[c]) * d, p.g + static_cast<size_t>(kc[c + 1]) * d, d, lane, v0, v1);
-    else v0 = exact_dot_warp_qd(qs, p.g + static_cast<size_t>(kc[c]) * d, d, lane);
+    if (c + 1 < m) exact_dot<2>(qs, p.g + static_cast<size_t>(kc[c]) * d, p.g + static_cast<size_t>(kc[c + 1]) * d, d, lane, v0, v1);
+    else exact_dot<1>(qs, p.g + static_cast<size_t>(kc[c]) * d, nullptr, d, lane, v0, v1);
     if (lane == 0) {
       sc[c] = v0;
       if (c + 1 < m) sc[c + 1] = v1;
@@ -1274,7 +684,7 @@ __global__ void __launch_bounds__(128)
   float* qs = reinterpret_cast<float*>(sm);                              // [p]
   double* sc = reinterpret_cast<double*>(sm + ((p * 4 + 15) & ~15));      // [n_cand]
   long long* ci = reinterpret_cast<long long*>(sc + n_cand);              // [n_cand], -1 = duplicate / taken
-  __shared__ BlockBest s_bb;
+  __shared__ BlockBest<4> s_bb;
   const int qrow = blockIdx.x;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int c = threadIdx.x; c < n_cand; c += blockDim.x) ci[c] = cand[static_cast<size_t>(qrow) * n_cand + c];
@@ -1299,10 +709,15 @@ __global__ void __launch_bounds__(128)
       if (ci[c] < 0) continue;   // warp-uniform
       double best = sc[c];
       if (cross) {   // 'cross' (einsum_in_chunks, diff_retrieval.py:652-654): every gallery part against every query part
-        for (int part = 0; part < n_chunks; ++part)
-          best = fmax(best, exact_dot_warp(qs, g + static_cast<size_t>(ci[c]) * d + part * p, p, lane));
+        for (int part = 0; part < n_chunks; ++part) {
+          double v;
+          exact_dot<1>(qs, g + static_cast<size_t>(ci[c]) * d + part * p, nullptr, p, lane, v, v);
+          best = fmax(best, v);
+        }
       } else {
-        best = fmax(best, exact_dot_warp(qs, g + static_cast<size_t>(ci[c]) * d + qp * p, p, lane));
+        double v;
+        exact_dot<1>(qs, g + static_cast<size_t>(ci[c]) * d + qp * p, nullptr, p, lane, v, v);
+        best = fmax(best, v);
       }
       if (lane == 0) sc[c] = best;   // ranked on the float64 value (as dcr_sim_topk), reported as fp32
     }
@@ -1350,7 +765,8 @@ __global__ void __launch_bounds__(256)
   for (int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < ng; row += warps) {
     const float* gr = g + static_cast<size_t>(row) * d;
     for (int f = 0; f < nb; ++f) {
-      const double v = exact_dot_warp(qs + f * d, gr, d, lane);
+      double v;
+      exact_dot<1>(qs + f * d, gr, nullptr, d, lane, v, v);
       if (lane == 0) scores[static_cast<size_t>(f) * ng + row] = v;
     }
   }
@@ -1364,335 +780,33 @@ __global__ void __launch_bounds__(256)
   if (f_begin + f >= *n_flagged) return;
   const int qrow = flagged[f_begin + f];
   double* s = scores + static_cast<size_t>(f) * ng;
-  __shared__ double s_best[8];
-  __shared__ int s_besti[8];
+  __shared__ BlockBest<8> s_bb;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int round = 0; round < k; ++round) {
     double bs = -INFINITY;
-    int bi = -1;
+    long long bi = -1;
+    int bp = -1;   // = bi: the position is the gallery row
     for (int c = threadIdx.x; c < ng; c += blockDim.x) {
       const double v = s[c];
-      if (!(v != v) && (bi < 0 || v > bs)) {   // ascending c per thread => first (lowest index) max kept
+      if (!(v != v) && (bp < 0 || v > bs)) {   // NaN skipped; ascending c per thread => first (lowest index) max kept
         bs = v;
-        bi = c;
+        bi = bp = c;
       }
     }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      const double os = __shfl_xor_sync(kFull, bs, off);
-      const int oi = __shfl_xor_sync(kFull, bi, off);
-      if (oi >= 0 && (bi < 0 || os > bs || (os == bs && oi < bi))) {
-        bs = os;
-        bi = oi;
-      }
-    }
-    if (lane == 0) {
-      s_best[warp] = bs;
-      s_besti[warp] = bi;
-    }
-    __syncthreads();
+    block_argbest(bs, bi, bp, &s_bb, lane, warp);
     if (threadIdx.x == 0) {
-      for (int w = 1; w < 8; ++w)
-        if (s_besti[w] >= 0 && (s_besti[0] < 0 || s_best[w] > s_best[0] ||
-                                (s_best[w] == s_best[0] && s_besti[w] < s_besti[0]))) {
-          s_best[0] = s_best[w];
-          s_besti[0] = s_besti[w];
-        }
-      if (s_besti[0] < 0) {   // every remaining score is NaN (NaN query row, or k > number of non-NaN scores)
+      if (bp < 0) {   // every remaining score is NaN (NaN query row, or k > number of non-NaN scores)
         out_scores[static_cast<size_t>(qrow) * k + round] = __int_as_float(0x7fc00000);
         out_idx[static_cast<size_t>(qrow) * k + round] = -1;
       } else {
-        out_scores[static_cast<size_t>(qrow) * k + round] = static_cast<float>(s_best[0]);
-        out_idx[static_cast<size_t>(qrow) * k + round] = g_index_base + g_index_stride * s_besti[0];
-        s[s_besti[0]] = __longlong_as_double(0x7ff8000000000000LL);  // NaN marks "taken"
+        out_scores[static_cast<size_t>(qrow) * k + round] = static_cast<float>(bs);
+        out_idx[static_cast<size_t>(qrow) * k + round] = g_index_base + g_index_stride * bi;
+        s[bp] = __longlong_as_double(0x7ff8000000000000LL);  // NaN marks "taken"
       }
     }
     __syncthreads();
   }
 }
-
-// ------------------------------------------------------------------------------------------------------------
-// Threshold search (dcr_sim_range): every pair with fp32(exact score) >= tau, in CSR form.
-//   1. range_threshold_kernel  per query row the candidate threshold t_i on the approximate score: no pair whose fp32
-//                              exact score reaches tau has an approximate score below t_i (row_bound)
-//   2. sim_range_kernel<*, 0>  count sweep: candidates per (segment slot, row)
-//   3. range_slot_scan_kernel + exclusive_scan_kernel: per row, the slots' offsets in gallery order; the rows' offsets
-//   4. sim_range_kernel<*, 1>  emit sweep: the same decisions again, each row's candidates written in ascending order
-//   5. range_rescore_kernel    exact scores in pieces of kRangePiece candidates of one row, stable compaction to the
-//                              pairs that reach tau
-//   6. exclusive_scan_kernel over the pieces, range_output_kernel / range_row_offsets_kernel: the CSR arrays
-// Everything is a fixed function of the inputs (no atomics decide an order), so every call returns the same bits.
-constexpr int kRangePiece = 512;   // candidates of one row re-scored by one block
-
-struct RangeParams {
-  int nq, ng;
-  int num_kb, stream_a, n_qtiles, n_gtiles, gchunk, n_chunks, stages;   // as SimParams
-  const int* bias_flag;
-  const float* col_bias;
-  const float* thr;            // [nq] candidate threshold t_i
-  int* seg;                    // [n_slots][128] count sweep: candidates; emit sweep: offset inside the row
-  const long long* row_cand;   // [nq + 1] emit sweep: first candidate of each row
-  int* cand_idx;               // emit sweep: local gallery rows
-};
-
-// Candidate columns of one 32-column chunk of an accumulator row: bit c is set when the approximate score of column
-// col0 + c is not below t (NaN included: the exact score decides) and c < n_valid.  Columns past the gallery are cut by
-// n_valid rather than by mask_tail: at t = -inf their -inf would pass.
-template <bool kBias>
-DCR_DEVICE uint32_t range_hits(const uint32_t (&r)[32], const float* sb, float t, int n_valid) {
-  float v[32];
-#pragma unroll
-  for (int c = 0; c < 32; ++c) v[c] = __uint_as_float(r[c]);
-  if constexpr (kBias) {   // the same fp32 additions as scan_chunk
-#pragma unroll
-    for (int c = 0; c < 32; c += 4) {
-      const float4 b = *reinterpret_cast<const float4*>(sb + c);
-      v[c] += b.x; v[c + 1] += b.y; v[c + 2] += b.z; v[c + 3] += b.w;
-    }
-  }
-  uint32_t m = 0;
-#pragma unroll
-  for (int c = 0; c < 32; ++c) m |= static_cast<uint32_t>(!(v[c] < t)) << c;
-  if (n_valid < 32) m &= n_valid <= 0 ? 0u : (1u << n_valid) - 1u;
-  return m;
-}
-
-// The fused sweep of the threshold search: the work decomposition, pipeline and k-loop of sim_topk_kernel with one
-// consumer warpgroup, an epilogue that compares every accumulator column against its row's threshold, and no warm-up.
-// kEmit = 0 counts the candidates of every (segment slot, row); kEmit = 1 writes them at the offsets the scan derived
-// from those counts.  Both make the same decisions: same tiles, same wgmma sequence, same thresholds.
-template <bool kBias, bool kEmit>
-__global__ void __launch_bounds__(32 + 128, 1)
-    sim_range_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_g,
-                     const RangeParams p) {
-  if (((p.bias_flag != nullptr) && (*p.bias_flag != 0)) != kBias) return;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const FusedPipe pp(smem_raw, p.num_kb, p.stream_a, p.stages, 0);   // then barriers, then 4 transpose buffers
-  const uint32_t warp = threadIdx.x >> 5;
-  const uint32_t lane = threadIdx.x & 31;
-  pp.init(&tmap_q, &tmap_g, p.stages, 4);
-  const long long n_units = gridDim.x;
-  const long long unit = blockIdx.x;
-  SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
-  if (warp == 4) {
-    fused_producer(pp, &tmap_q, &tmap_g, p.stages, w, [](const SegWalker&) { return 0; });
-  } else {
-    const uint32_t row = warp * 32 + lane;   // query row inside the tile
-    const uint32_t xacc = smem_u32(pp.tail) + warp * kAccXposeWarpBytes;
-    const uint32_t a_base = smem_u32(pp.stream_a ? pp.smem_b + kBTileBytes : pp.smem_a);
-    const uint32_t b_base = smem_u32(pp.smem_b);
-    PipeState st(p.stages);
-    uint32_t seg = 0;
-    while (w.next()) {
-      const int qrow = w.qi * kBlockM + static_cast<int>(row);
-      const bool row_ok = qrow < p.nq;
-      const float t = row_ok ? p.thr[qrow] : INFINITY;
-      const size_t sr = static_cast<size_t>(slot_index(w.chunk, static_cast<int>(unit), w.qi, 0, static_cast<int>(n_units),
-                                                       p.n_qtiles, 1)) * kBlockM + row;
-      int cnt = 0;
-      int* out = nullptr;
-      if (kEmit && row_ok) out = p.cand_idx + p.row_cand[qrow] + p.seg[sr];
-      if (!pp.stream_a) mbar_wait(pp.a_full, seg & 1);
-#pragma unroll 1
-      for (int j = 0; j < w.ntiles; ++j) {
-        WgAcc<kBlockN> acc;
-        fused_tile_mma(acc, st, pp, a_base, b_base, j == w.ntiles - 1, lane);
-        const int gcol0 = (w.g_begin + j) * kBlockN;
-#pragma unroll
-        for (int ch = 0; ch < kBlockN / 32; ++ch) {
-          uint32_t r[32];
-          acc.rows32(ch, r, xacc, lane);
-          const int col0 = gcol0 + ch * 32;
-          const uint32_t hits = range_hits<kBias>(r, kBias ? p.col_bias + col0 : nullptr, t, row_ok ? p.ng - col0 : 0);
-          if constexpr (kEmit) {
-            for (uint32_t h = hits; h; h &= h - 1) *out++ = col0 + __ffs(h) - 1;   // ascending columns
-          } else {
-            cnt += __popc(hits);
-          }
-        }
-      }
-      ++seg;
-      if (!kEmit) p.seg[sr] = cnt;
-    }
-  }
-  __syncthreads();
-}
-
-// t_i = tau - q.mu - eps - slack - margin, rounded down at every step.  fp32(s) >= tau needs s >= tau - half an fp32 ulp
-// (margin), hence approximate score >= t_i (row_bound).  A warp per query row.
-__global__ void __launch_bounds__(128)
-    range_threshold_kernel(const float* __restrict__ q, int nq, int d, int d_pad, float tau,
-                           const float* __restrict__ q_norm_hat, const float* __restrict__ q_norm_res,
-                           const float* __restrict__ q_norm_x, const unsigned int* __restrict__ g_max,
-                           const float* __restrict__ mu, const float* __restrict__ nu, const int* __restrict__ nu_flag,
-                           float* __restrict__ thr) {
-  const int row = blockIdx.x * 4 + static_cast<int>(threadIdx.x >> 5);
-  const uint32_t lane = threadIdx.x & 31;
-  if (row >= nq) return;
-  const RowBound rb = row_bound(q + static_cast<size_t>(row) * d, d, d_pad, row, q_norm_hat, q_norm_res, q_norm_x, g_max,
-                                mu, nu, nu_flag, lane);
-  if (lane == 0) {
-    const double margin = isfinite(tau) ? fabs(static_cast<double>(tau)) * 1.2e-7 + 1e-45 : 0.0;
-    double t = __dsub_rd(static_cast<double>(tau), rb.qmu);
-    t = __dsub_rd(t, static_cast<double>(rb.eps));
-    t = __dsub_rd(t, rb.slack);
-    t = __dsub_rd(t, margin);
-    thr[row] = __double2float_rd(t);
-  }
-}
-
-// Per query row (a thread each): walk the row's segment slots in gallery order -- chunk by chunk, and inside a chunk unit
-// by unit (a unit's tiles follow the previous unit's) -- replacing each count by the row's candidates before it.
-__global__ void __launch_bounds__(256)
-    range_slot_scan_kernel(int* __restrict__ seg, int nq, int n_qtiles, int n_gtiles, int gchunk, int n_chunks,
-                           int n_units, long long* __restrict__ row_cnt, long long* __restrict__ row_pieces) {
-  const int row = blockIdx.x * blockDim.x + threadIdx.x;
-  if (row >= nq) return;
-  const int qi = row / kBlockM, r = row % kBlockM;
-  int acc = 0;
-  for (int chunk = 0; chunk < n_chunks; ++chunk) {
-    const int ncg = min(gchunk, n_gtiles - chunk * gchunk);
-    const long long T = static_cast<long long>(n_qtiles) * ncg;
-    const int u_lo = static_cast<int>(owner_unit(static_cast<long long>(qi) * ncg, T, n_units));
-    const int u_hi = static_cast<int>(owner_unit(static_cast<long long>(qi + 1) * ncg - 1, T, n_units));
-    for (int u = u_lo; u <= u_hi; ++u) {
-      const size_t sr = static_cast<size_t>(slot_index(chunk, u, qi, 0, n_units, n_qtiles, 1)) * kBlockM + r;
-      const int c = seg[sr];
-      seg[sr] = acc;
-      acc += c;
-    }
-  }
-  row_cnt[row] = acc;
-  row_pieces[row] = (acc + kRangePiece - 1) / kRangePiece;
-}
-
-// out[0..n] = exclusive prefix sums of in[0..n-1] (out[n] = total), one block: thread t sums a contiguous run, the runs'
-// sums are scanned in shared memory, then each thread writes its run.  Fixed association.
-template <typename T>
-__global__ void __launch_bounds__(1024) exclusive_scan_kernel(const T* __restrict__ in, long long n, long long* __restrict__ out) {
-  __shared__ long long part[32];
-  const int tid = threadIdx.x, lane = tid & 31, wp = tid >> 5;
-  const long long per = (n + 1023) / 1024;
-  const long long lo = min(n, tid * per), hi = min(n, lo + per);
-  long long s = 0;
-  for (long long i = lo; i < hi; ++i) s += in[i];
-  long long incl = s;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const long long v = __shfl_up_sync(kFull, incl, o);
-    if (lane >= o) incl += v;
-  }
-  if (lane == 31) part[wp] = incl;
-  __syncthreads();
-  if (wp == 0) {
-    long long x = part[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const long long v = __shfl_up_sync(kFull, x, o);
-      if (lane >= o) x += v;
-    }
-    part[lane] = x;   // inclusive over warps
-  }
-  __syncthreads();
-  long long run = incl - s + (wp > 0 ? part[wp - 1] : 0);
-  for (long long i = lo; i < hi; ++i) {
-    out[i] = run;
-    run += in[i];
-  }
-  if (tid == 0) out[n] = part[31];
-}
-
-// piece w: row, first candidate and candidate count (row_piece[0] = 0 <= w < row_piece[nq])
-DCR_DEVICE void range_piece(long long w, const long long* __restrict__ row_cand, const long long* __restrict__ row_piece,
-                            int nq, int& row, long long& start, int& n) {
-  int lo = 0, hi = nq;   // row_piece[lo] <= w < row_piece[hi]
-  while (hi - lo > 1) {
-    const int mid = lo + (hi - lo) / 2;
-    if (row_piece[mid] <= w) lo = mid;
-    else hi = mid;
-  }
-  row = lo;
-  start = row_cand[lo] + (w - row_piece[lo]) * kRangePiece;
-  n = static_cast<int>(min(static_cast<long long>(kRangePiece), row_cand[lo + 1] - start));
-}
-
-// Exact scores of one piece (the association of exact_dot_warp: the values dcr_sim_topk reports), then a stable in-place
-// compaction of the pairs with fp32 score >= tau.  piece_kept[w] = pairs kept.
-__global__ void __launch_bounds__(kRescoreThreads)
-    range_rescore_kernel(const float* __restrict__ q, const float* __restrict__ g, int nq, int d, float tau,
-                         const long long* __restrict__ row_cand, const long long* __restrict__ row_piece,
-                         int* __restrict__ cand_idx, float* __restrict__ cand_score, int* __restrict__ piece_kept) {
-  extern __shared__ __align__(16) uint8_t sm[];
-  double* qs = reinterpret_cast<double*>(sm);   // [d] the query row, widened once
-  const int tid = threadIdx.x;
-  const uint32_t lane = threadIdx.x & 31;
-  const int warp = tid >> 5;
-  int row, n;
-  long long start;
-  range_piece(blockIdx.x, row_cand, row_piece, nq, row, start, n);
-  for (int c = tid; c < d; c += kRescoreThreads) qs[c] = static_cast<double>(q[static_cast<size_t>(row) * d + c]);
-  __syncthreads();
-  int* ci = cand_idx + start;
-  float* cs = cand_score + start;
-  for (int c = 2 * warp; c < n; c += 2 * (kRescoreThreads / 32)) {
-    double v0, v1 = 0.0;
-    if (c + 1 < n) exact_dot_warp_qd2(qs, g + static_cast<size_t>(ci[c]) * d, g + static_cast<size_t>(ci[c + 1]) * d, d, lane, v0, v1);
-    else v0 = exact_dot_warp_qd(qs, g + static_cast<size_t>(ci[c]) * d, d, lane);
-    if (lane == 0) {
-      cs[c] = static_cast<float>(v0);
-      if (c + 1 < n) cs[c + 1] = static_cast<float>(v1);
-    }
-  }
-  __syncthreads();
-  // round by round: every read of a round happens before the barrier inside group_scan, every write after it, and a
-  // round writes only below the positions later rounds read
-  int kept = 0;
-  for (int c0 = 0; c0 < n; c0 += kRescoreThreads) {
-    const int c = c0 + tid;
-    int idx = 0;
-    float s = 0.f;
-    bool keep = false;
-    if (c < n) {
-      idx = ci[c];
-      s = cs[c];
-      keep = s >= tau;   // NaN never
-    }
-    int total;
-    const int pos = kept + group_scan<kRescoreThreads>(keep ? 1 : 0, total);
-    if (keep) {
-      ci[pos] = idx;
-      cs[pos] = s;
-    }
-    kept += total;
-  }
-  if (tid == 0) piece_kept[blockIdx.x] = kept;
-}
-
-// piece w's kept pairs -> the output at piece_excl[w] (global gallery indices)
-__global__ void __launch_bounds__(256)
-    range_output_kernel(const long long* __restrict__ row_cand, const long long* __restrict__ row_piece, int nq,
-                        const long long* __restrict__ piece_excl, const int* __restrict__ cand_idx,
-                        const float* __restrict__ cand_score, long long g_index_base, long long g_index_stride,
-                        long long* __restrict__ out_idx, float* __restrict__ out_scores) {
-  int row, n;
-  long long start;
-  range_piece(blockIdx.x, row_cand, row_piece, nq, row, start, n);
-  const long long o = piece_excl[blockIdx.x];
-  const int kept = static_cast<int>(piece_excl[blockIdx.x + 1] - o);
-  for (int j = threadIdx.x; j < kept; j += blockDim.x) {
-    out_idx[o + j] = g_index_base + g_index_stride * cand_idx[start + j];
-    out_scores[o + j] = cand_score[start + j];
-  }
-}
-
-// row i starts at the output position of its first piece (rows without candidates: of the next row's first piece)
-__global__ void range_row_offsets_kernel(const long long* __restrict__ row_piece, const long long* __restrict__ piece_excl,
-                                         int nq, long long* __restrict__ row_offsets) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= nq; i += gridDim.x * blockDim.x)
-    row_offsets[i] = piece_excl[row_piece[i]];
-}
-
-inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 // launch geometry of one fused pass over nq queries
 struct PassPlan {
@@ -1702,17 +816,11 @@ struct PassPlan {
   size_t smem_bytes;
 };
 
-struct SimPlan {
-  int d_pad, num_kb, ng_pad, n_gtiles, rows_per_qtile;
-  int stream_a;  // d_pad > 512: query tile streamed with the gallery k-blocks
+struct SimPlan : SweepGeometry {
   int max_sets;  // upper bound for PassPlan::n_sets (1 or 2)
-  int gchunk, n_chunks;   // preferred gallery chunking (a pass may use fewer chunks)
   int kp0, kp1;           // candidates kept by the first pass / by the second-chance pass (0 = no second pass)
   PassPlan p0, p1;        // p1 is sized for the worst case (every query flagged)
-  // workspace offsets
-  size_t off_qb, off_qb1, off_gb, off_qnh, off_qnr, off_qnx, off_gmax, off_colsum, off_mu, off_cand, off_cnt, off_thr,
-      off_flag0, off_flag1, off_thr1, off_counts, off_exact, off_nu, off_bias, off_clk, off_gthr;
-  size_t total;
+  size_t total;           // workspace bytes
 };
 
 int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, int d, int k, PassPlan* pp) {
@@ -1720,12 +828,13 @@ int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, i
   pp->n_qtiles = (nq + sp.rows_per_qtile - 1) / sp.rows_per_qtile;
   pp->nq_pad = pp->n_qtiles * sp.rows_per_qtile;
   pp->kp = kp;
-  // ---- shared memory: resident A + stages*B + n_sets * cap KB of lists + barriers + carried thresholds ----
-  const size_t a_bytes = sp.stream_a ? 0 : static_cast<size_t>(sp.num_kb) * kATileBytes;
-  const size_t b_tile = static_cast<size_t>(kBlockN) * kBlockK * 2 + (sp.stream_a ? kATileBytes : 0);
-  const size_t fixed = 1024 /*align slack*/ + 256 /*barriers*/ + 4096 /*carried thresholds*/;
-  auto per_set = [&](int cp) { return static_cast<size_t>(cp) * 1024 + 4 * kAccXposeWarpBytes; };   // lists + transposes
-  auto fits = [&](int st, int cp, int sets) { return max_smem >= a_bytes + st * b_tile + per_set(cp) * sets + fixed; };
+  // ---- shared memory: the pipeline with n_sets x cap KB of lists, then carried thresholds (4 KB, whatever n_sets) and
+  // the accumulator transposes of 4 n_sets warps ----
+  auto smem = [&](int st, int cp, int sets) {
+    return FusedPipe::smem_bytes(sp.num_kb, sp.stream_a, st, static_cast<size_t>(sets) * cp * 128 * 8,
+                                 4096 + static_cast<size_t>(sets) * 4 * kAccXposeWarpBytes);
+  };
+  auto fits = [&](int st, int cp, int sets) { return max_smem >= smem(st, cp, sets); };
   // two epilogue warp sets whenever their lists (at least kp + 8 entries per row and set) fit next to 3 B stages
   int sets = (sp.max_sets >= 2 && fits(3, kp + 8, 2)) ? 2 : 1;
   int cap = kp + (sets == 2 ? 8 : 16);
@@ -1740,7 +849,7 @@ int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, i
   pp->cap = cap;
   pp->stages = stages;
   pp->n_sets = sets;
-  pp->smem_bytes = fixed + a_bytes + stages * b_tile + per_set(cap) * sets;
+  pp->smem_bytes = smem(stages, cap, sets);
 
   // ---- gallery chunking and work units ----
   pp->gchunk = sp.gchunk;
@@ -1776,23 +885,42 @@ int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, i
   return 0;
 }
 
-// tiles, padding and gallery chunking of a fused sweep (both entry points)
-void plan_geometry(int ng, int d, SimPlan* pl) {
-  pl->d_pad = static_cast<int>(align_up(d, kBlockK));
-  pl->num_kb = pl->d_pad / kBlockK;
-  pl->stream_a = pl->num_kb > kMaxKB ? 1 : 0;
-  pl->rows_per_qtile = kBlockM;
-  pl->n_gtiles = (ng + kBlockN - 1) / kBlockN;
-  pl->ng_pad = pl->n_gtiles * kBlockN;
-  // gallery chunks of ~40 MB of bf16 rows: the units sweep one chunk at a time so that it stays L2 resident
-  const long long chunk_bytes = 40ll << 20;
-  int gchunk = static_cast<int>(std::max<long long>(16, chunk_bytes / (static_cast<long long>(kBlockN) * pl->d_pad * 2)));
-  int n_chunks = (pl->n_gtiles + gchunk - 1) / gchunk;
-  if (n_chunks > 64) n_chunks = 64;
-  gchunk = (pl->n_gtiles + n_chunks - 1) / n_chunks;   // equal chunks
-  n_chunks = (pl->n_gtiles + gchunk - 1) / gchunk;
-  pl->gchunk = gchunk;
-  pl->n_chunks = n_chunks;
+struct PassBuffers {
+  uint2* cand;
+  int* ccnt;
+  float* cthr;
+};
+
+// The top-k search's workspace: the operands, the second pass's compacted queries, the candidate slots (sized for the
+// larger pass), the flagged queries and the brute-force scores
+struct TopkBuffers {
+  Operands ops;   // ops.qflag is counts + 2
+  __nv_bfloat16* qb1;
+  PassBuffers pb;
+  int *flag0, *flag1;
+  float* thr1;
+  int* counts;   // [0] flagged by pass 0, [1] flagged by pass 1, [2] the query-centring flag
+  unsigned long long* clk;
+  unsigned int* gthr;
+  double* exact;
+};
+
+TopkBuffers carve_topk(const SimPlan& pl, int nq, int ng, int d, Carve& w) {
+  TopkBuffers b;
+  b.ops = carve_operands(w, pl.p0.nq_pad, pl, d);
+  b.qb1 = w.take<__nv_bfloat16>(pl.kp1 ? static_cast<size_t>(pl.p1.nq_pad) * pl.d_pad : 0);
+  const size_t slot_rows = static_cast<size_t>(std::max(pl.p0.n_slots, pl.kp1 ? pl.p1.n_slots : 0)) * pl.rows_per_qtile;   // n_slots counts sets
+  b.pb.cand = w.take<uint2>(slot_rows * kKPMax);
+  b.pb.ccnt = w.take<int>(slot_rows);
+  b.pb.cthr = w.take<float>(slot_rows);
+  b.flag0 = w.take<int>(nq);
+  b.flag1 = w.take<int>(nq);
+  b.thr1 = w.take<float>(nq);
+  b.counts = w.take<int>(4);
+  b.clk = w.take<unsigned long long>(4);
+  b.gthr = w.take<unsigned int>(std::max(pl.p0.nq_pad, pl.kp1 ? pl.p1.nq_pad : 0));
+  b.exact = w.take<double>(static_cast<size_t>(kExactBatch) * ng);
+  return b;
 }
 
 int make_plan(int nq, int ng, int d, int k, int num_sms, size_t max_smem, SimPlan* pl) {
@@ -1815,62 +943,19 @@ int make_plan(int nq, int ng, int d, int k, int num_sms, size_t max_smem, SimPla
   if (pl->kp1) {
     if (plan_pass(nq, pl->kp1, *pl, num_sms, max_smem, d, k, &pl->p1) != 0) pl->kp1 = 0;   // does not fit: skip
   }
-  const PassPlan& big = pl->p0;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    size_t o = off;
-    off = align_up(off + bytes, 256);
-    return o;
-  };
-  pl->off_qb = take(static_cast<size_t>(big.nq_pad) * pl->d_pad * 2);
-  pl->off_qb1 = take(pl->kp1 ? static_cast<size_t>(pl->p1.nq_pad) * pl->d_pad * 2 : 0);
-  pl->off_gb = take(static_cast<size_t>(pl->ng_pad) * pl->d_pad * 2);
-  pl->off_qnh = take(static_cast<size_t>(big.nq_pad) * 4);
-  pl->off_qnr = take(static_cast<size_t>(big.nq_pad) * 4);
-  pl->off_qnx = take(static_cast<size_t>(big.nq_pad) * 4);
-  pl->off_gmax = take(16);
-  pl->off_colsum = take(static_cast<size_t>(d) * 16);   // column sums + column sums of squares
-  pl->off_mu = take(static_cast<size_t>(d) * 4);
-  pl->off_nu = take(static_cast<size_t>(d) * 4);
-  pl->off_bias = take(static_cast<size_t>(pl->ng_pad) * 4);
-  const size_t slot_rows = static_cast<size_t>(std::max(pl->p0.n_slots, pl->kp1 ? pl->p1.n_slots : 0)) * pl->rows_per_qtile;   // n_slots counts sets
-  pl->off_cand = take(slot_rows * kKPMax * 8);
-  pl->off_cnt = take(slot_rows * 4);
-  pl->off_thr = take(slot_rows * 4);
-  pl->off_flag0 = take(static_cast<size_t>(nq) * 4);
-  pl->off_flag1 = take(static_cast<size_t>(nq) * 4);
-  pl->off_thr1 = take(static_cast<size_t>(nq) * 4);
-  pl->off_counts = take(16);
-  pl->off_clk = take(32);
-  pl->off_gthr = take(static_cast<size_t>(std::max(big.nq_pad, pl->kp1 ? pl->p1.nq_pad : 0)) * 4);
-  pl->off_exact = take(static_cast<size_t>(kExactBatch) * ng * 8);
-  pl->total = off;
+  Carve size;
+  carve_topk(*pl, nq, ng, d, size);
+  pl->total = size.bytes;
   return 0;
 }
-
-
-struct PassBuffers {
-  uint2* cand;
-  int* ccnt;
-  float* cthr;
-};
 
 // one fused pass: qb (bf16, padded) x gb (bf16, centred, padded) -> candidate slots
 int launch_fused(const SimPlan& pl, const PassPlan& pp, const __nv_bfloat16* qb, const __nv_bfloat16* gb, int ng,
                  const PassBuffers& pb, const float* col_bias, const int* bias_flag, const float* thr_init,
                  unsigned long long* clk, unsigned int* gthr, cudaStream_t stream) {
   CUtensorMap tq, tg;
-  if (int rc = make_tmap_2d_bf16(&tq, qb, pp.nq_pad, pl.d_pad, pl.d_pad, kBlockM, kBlockK)) return rc;
-  if (int rc = make_tmap_2d_bf16(&tg, gb, pl.ng_pad, pl.d_pad, pl.d_pad, kBlockN, kBlockK)) return rc;
   SimParams p;
-  p.nq = pp.nq;
-  p.ng = ng;
-  p.num_kb = pl.num_kb;
-  p.stream_a = pl.stream_a;
-  p.n_qtiles = pp.n_qtiles;
-  p.n_gtiles = pl.n_gtiles;
-  p.gchunk = pp.gchunk;
-  p.n_chunks = pp.n_chunks;
+  if (int rc = sweep_setup(pl, pp.nq, pp.n_qtiles, ng, pp.gchunk, pp.n_chunks, qb, gb, &p, &tq, &tg)) return rc;
   p.kp = pp.kp;
   p.cap = pp.cap;
   p.stages = pp.stages;
@@ -1883,130 +968,10 @@ int launch_fused(const SimPlan& pl, const PassPlan& pp, const __nv_bfloat16* qb,
   p.clk = clk;
   p.gthr = gthr;
   DCR_CUDA_CHECK(cudaMemsetAsync(gthr, 0, static_cast<size_t>(pp.nq_pad) * 4, stream));
-  auto sweep = [&](auto kern) {
-    return launch(kern, pp.n_units, 32 + 128 * pp.n_sets, pp.smem_bytes, stream, "sim_topk", tq, tg, p);
-  };
-  // both variants are launched; the one that does not match the device flag (query centring on / off) returns at once
-  if (pp.n_sets == 2) {
-    if (int rc = sweep(sim_topk_kernel<false, 2>)) return rc;
-    return sweep(sim_topk_kernel<true, 2>);
-  }
-  if (int rc = sweep(sim_topk_kernel<false, 1>)) return rc;
-  return sweep(sim_topk_kernel<true, 1>);
-}
-
-// Stage 1 of both entry points: the centres, the decision whether to centre the queries, and the bf16 operands with the
-// norms their error bound needs.
-struct Operands {
-  __nv_bfloat16 *qb, *gb;   // [nq_pad, d_pad], [ng_pad, d_pad]
-  float *qnh, *qnr, *qnx;   // per query row, see to_bf16_rows_kernel
-  unsigned int* gmax;       // [2]
-  double* colsum;           // [2 d] scratch
-  float *mu, *nu, *bias;    // gallery centre, query centre, per-gallery-row offset nu.(g - mu)
-  int* qflag;               // device flag: query centring on / off
-};
-
-int prepare_operands(const float* q, int nq, int nq_pad, const float* g, int ng, int d, const SimPlan& pl,
-                     const DeviceInfo* di, const Operands& o, cudaStream_t stream) {
-  DCR_CUDA_CHECK(cudaMemsetAsync(o.gmax, 0, 16, stream));
-  const int conv_blocks = di->num_sms * 8;
-  auto sampled_mean = [&](const float* x, int n, float* out, bool decide) -> int {
-    // any fixed vector works as a centre, so a strided sample of <= 8192 rows is enough
-    DCR_CUDA_CHECK(cudaMemsetAsync(o.colsum, 0, static_cast<size_t>(d) * 16, stream));
-    const int row_stride = std::max(1, n / 8192);
-    const int n_sample = (n + row_stride - 1) / row_stride;
-    col_sum_kernel<<<std::max(1, std::min((n_sample + 63) / 64, di->num_sms)), kColSumThreads, 0, stream>>>(
-        x, n_sample, row_stride, d, o.colsum, decide ? o.colsum + d : nullptr);
-    count_launch();
-    col_mean_finish_kernel<<<(d + 255) / 256, 256, 0, stream>>>(o.colsum, n_sample, d, out);
-    count_launch();
-    if (decide) {
-      centre_decision_kernel<<<1, 256, 0, stream>>>(o.colsum, o.colsum + d, n_sample, d, o.qflag);
-      count_launch();
-    }
-    return 0;
-  };
-  if (int rc = sampled_mean(g, ng, o.mu, false)) return rc;    // gallery centre mu (always used)
-  if (int rc = sampled_mean(q, nq, o.nu, true)) return rc;     // query centre nu + the decision whether to use it
-  // q' = q - nu, g' = g - mu:  q.g = q'.g' + nu.g' + q.mu  -- the tensor cores see only the centred parts, nu.g' is a
-  // per-gallery-row offset added to the accumulator columns, q.mu a per-query constant that cannot change the ranking
-  // d_pad <= 256: 2 loads per lane cover the row; otherwise 4 per round (512 dims = one round)
-  auto convert = (pl.d_pad <= 256) ? to_bf16_rows_kernel<2> : to_bf16_rows_kernel<4>;
-  convert<<<conv_blocks, 256, 0, stream>>>(q, nq, d, nq_pad, pl.d_pad, o.nu, o.qb, o.qnh, o.qnr, o.qnx, nullptr,
-                                           nullptr, nullptr, o.qflag, nullptr);
-  count_launch();
-  convert<<<conv_blocks, 256, 0, stream>>>(g, ng, d, pl.ng_pad, pl.d_pad, o.mu, o.gb, nullptr, nullptr, nullptr,
-                                           o.gmax, o.nu, o.bias, nullptr, o.qflag);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
-
-constexpr long long kMaxRangePairs = 1ll << 40;   // capacity accepted by the planner (keeps the byte counts in range)
-
-struct RangePlan {
-  SimPlan geo;   // plan_geometry fields only
-  int nq_pad, n_qtiles, n_units, n_slots, stages;
-  size_t smem_bytes;
-  long long max_pieces;   // pieces of kRangePiece candidates when max_pairs candidates fill the rows worst
-  size_t off_qb, off_gb, off_qnh, off_qnr, off_qnx, off_gmax, off_colsum, off_mu, off_nu, off_bias, off_flag, off_thr,
-      off_seg, off_row_cnt, off_row_cand, off_row_pcnt, off_row_piece, off_cand_idx, off_cand_score, off_piece_kept,
-      off_piece_excl;
-  size_t total;
-};
-
-int make_range_plan(int nq, int ng, int d, long long max_pairs, int num_sms, size_t max_smem, RangePlan* rp) {
-  DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "sim_range: empty problem (nq=%d ng=%d d=%d)", nq, ng, d);
-  DCR_REQUIRE(d <= kMaxDim, "sim_range: descriptor dim %d > %d not supported", d, kMaxDim);
-  DCR_REQUIRE(d % 4 == 0, "sim_range: descriptor dim %d is not a multiple of 4", d);
-  DCR_REQUIRE(max_pairs >= 0 && max_pairs <= kMaxRangePairs, "sim_range: max_pairs=%lld outside [0, 2^40]", max_pairs);
-  plan_geometry(ng, d, &rp->geo);
-  const SimPlan& g = rp->geo;
-  rp->n_qtiles = (nq + kBlockM - 1) / kBlockM;
-  rp->nq_pad = rp->n_qtiles * kBlockM;
-  // shared memory: resident query tile + stages x gallery stage + barriers + the transpose buffers of 4 warps
-  const size_t a_bytes = g.stream_a ? 0 : static_cast<size_t>(g.num_kb) * kATileBytes;
-  const size_t b_tile = static_cast<size_t>(kBTileBytes) + (g.stream_a ? kATileBytes : 0);
-  const size_t fixed = 1024 /*align slack*/ + 256 /*barriers*/ + 4 * kAccXposeWarpBytes;
-  int stages = 2;
-  DCR_REQUIRE(max_smem >= fixed + a_bytes + stages * b_tile, "sim_range: not enough shared memory (%zu B) for d=%d", max_smem, d);
-  while (stages < 8 && max_smem >= fixed + a_bytes + (stages + 1) * b_tile) ++stages;
-  rp->stages = stages;
-  rp->smem_bytes = fixed + a_bytes + stages * b_tile;
-  // every unit owns at least one tile of every chunk (the last chunk is the smallest): every slot the scan walks is written
-  const int last = g.n_gtiles - (g.n_chunks - 1) * g.gchunk;
-  rp->n_units = static_cast<int>(std::min<long long>(num_sms, static_cast<long long>(rp->n_qtiles) * last));
-  rp->n_slots = g.n_chunks * (rp->n_units + rp->n_qtiles);
-  rp->max_pieces = max_pairs / kRangePiece + nq;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    size_t o = off;
-    off = align_up(off + bytes, 256);
-    return o;
-  };
-  rp->off_qb = take(static_cast<size_t>(rp->nq_pad) * g.d_pad * 2);
-  rp->off_gb = take(static_cast<size_t>(g.ng_pad) * g.d_pad * 2);
-  rp->off_qnh = take(static_cast<size_t>(rp->nq_pad) * 4);
-  rp->off_qnr = take(static_cast<size_t>(rp->nq_pad) * 4);
-  rp->off_qnx = take(static_cast<size_t>(rp->nq_pad) * 4);
-  rp->off_gmax = take(16);
-  rp->off_colsum = take(static_cast<size_t>(d) * 16);
-  rp->off_mu = take(static_cast<size_t>(d) * 4);
-  rp->off_nu = take(static_cast<size_t>(d) * 4);
-  rp->off_bias = take(static_cast<size_t>(g.ng_pad) * 4);
-  rp->off_flag = take(16);
-  rp->off_thr = take(static_cast<size_t>(nq) * 4);
-  rp->off_seg = take(static_cast<size_t>(rp->n_slots) * kBlockM * 4);
-  rp->off_row_cnt = take(static_cast<size_t>(nq) * 8);
-  rp->off_row_cand = take((static_cast<size_t>(nq) + 1) * 8);
-  rp->off_row_pcnt = take(static_cast<size_t>(nq) * 8);
-  rp->off_row_piece = take((static_cast<size_t>(nq) + 1) * 8);
-  rp->off_cand_idx = take(static_cast<size_t>(max_pairs) * 4);
-  rp->off_cand_score = take(static_cast<size_t>(max_pairs) * 4);
-  rp->off_piece_kept = take(static_cast<size_t>(rp->max_pieces) * 4);
-  rp->off_piece_excl = take((static_cast<size_t>(rp->max_pieces) + 1) * 8);
-  rp->total = off;
-  return 0;
+  const bool two = pp.n_sets == 2;
+  return launch_sweep(two ? sim_topk_kernel<false, 2> : sim_topk_kernel<false, 1>,
+                      two ? sim_topk_kernel<true, 2> : sim_topk_kernel<true, 1>, pp.n_units, 32 + 128 * pp.n_sets,
+                      pp.smem_bytes, stream, "sim_topk", tq, tg, p);
 }
 
 }  // namespace
@@ -2043,34 +1008,12 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "sim_topk: workspace must be 256-byte aligned");
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0 && d % 4 == 0,
               "sim_topk: q/g must be 16-byte aligned with d %% 4 == 0 (d=%d)", d);
-  uint8_t* w = static_cast<uint8_t*>(ws);
-  auto* qb = reinterpret_cast<__nv_bfloat16*>(w + pl.off_qb);
-  auto* qb1 = reinterpret_cast<__nv_bfloat16*>(w + pl.off_qb1);
-  auto* gb = reinterpret_cast<__nv_bfloat16*>(w + pl.off_gb);
-  auto* qnh = reinterpret_cast<float*>(w + pl.off_qnh);
-  auto* qnr = reinterpret_cast<float*>(w + pl.off_qnr);
-  auto* qnx = reinterpret_cast<float*>(w + pl.off_qnx);
-  auto* gmax = reinterpret_cast<unsigned int*>(w + pl.off_gmax);
-  auto* colsum = reinterpret_cast<double*>(w + pl.off_colsum);
-  auto* mu = reinterpret_cast<float*>(w + pl.off_mu);
-  auto* nu = reinterpret_cast<float*>(w + pl.off_nu);
-  auto* bias = reinterpret_cast<float*>(w + pl.off_bias);
-  PassBuffers pb;
-  pb.cand = reinterpret_cast<uint2*>(w + pl.off_cand);
-  pb.ccnt = reinterpret_cast<int*>(w + pl.off_cnt);
-  pb.cthr = reinterpret_cast<float*>(w + pl.off_thr);
-  auto* flag0 = reinterpret_cast<int*>(w + pl.off_flag0);
-  auto* flag1 = reinterpret_cast<int*>(w + pl.off_flag1);
-  auto* thr1 = reinterpret_cast<float*>(w + pl.off_thr1);
-  auto* counts = reinterpret_cast<int*>(w + pl.off_counts);   // [0] flagged by pass 0, [1] flagged by pass 1
-  auto* exact = reinterpret_cast<double*>(w + pl.off_exact);
-  auto* clk = reinterpret_cast<unsigned long long*>(w + pl.off_clk);
-  auto* gthr = reinterpret_cast<unsigned int*>(w + pl.off_gthr);
-
-  DCR_CUDA_CHECK(cudaMemsetAsync(counts, 0, 16, stream));   // [0],[1] flagged counts, [2] query-centring flag
-  int* qflag = counts + 2;   // device flag: query centring on/off
-  const Operands ops = {qb, gb, qnh, qnr, qnx, gmax, colsum, mu, nu, bias, qflag};
-  if (int rc = prepare_operands(q, nq, pl.p0.nq_pad, g, ng, d, pl, di, ops, stream)) return rc;
+  Carve w{static_cast<uint8_t*>(ws)};
+  TopkBuffers b = carve_topk(pl, nq, ng, d, w);
+  DCR_CUDA_CHECK(cudaMemsetAsync(b.counts, 0, 16, stream));
+  b.ops.qflag = b.counts + 2;
+  const Operands& o = b.ops;
+  if (int rc = prepare_operands(q, nq, pl.p0.nq_pad, g, ng, d, pl, di, o, stream)) return rc;
 
   // CUDA events around the first fused pass only (thread-local, created once): bench.py's roofline numerator
   // (events belong to the device that was current when they were created: one pair per device)
@@ -2082,7 +1025,7 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     DCR_CUDA_CHECK(cudaEventCreate(&ev1));
   }
   DCR_CUDA_CHECK(cudaEventRecord(ev0, stream));
-  if (int rc = launch_fused(pl, pl.p0, qb, gb, ng, pb, bias, qflag, nullptr, clk, gthr, stream)) return rc;
+  if (int rc = launch_fused(pl, pl.p0, o.qb, o.gb, ng, b.pb, o.bias, o.qflag, nullptr, b.clk, b.gthr, stream)) return rc;
   DCR_CUDA_CHECK(cudaEventRecord(ev1, stream));
 
   auto rescore = [&](const PassPlan& pp, const int* qmap, int* flagged, int* n_flagged, float* thr_next) -> int {
@@ -2090,9 +1033,9 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     rp.q = q, rp.g = g, rp.nq = pp.nq, rp.d = d, rp.d_pad = pl.d_pad, rp.k = k;
     rp.n_qtiles = pp.n_qtiles, rp.n_gtiles = pl.n_gtiles, rp.gchunk = pp.gchunk, rp.n_chunks = pp.n_chunks;
     rp.n_units = pp.n_units, rp.n_sets = pp.n_sets, rp.max_cand = pp.max_cand;
-    rp.cand = pb.cand, rp.cand_cnt = pb.ccnt, rp.cand_thr = pb.cthr, rp.qmap = qmap;
-    rp.mu = mu, rp.nu = nu, rp.nu_flag = qflag;
-    rp.q_norm_hat = qnh, rp.q_norm_res = qnr, rp.q_norm_x = qnx, rp.g_max = gmax;
+    rp.cand = b.pb.cand, rp.cand_cnt = b.pb.ccnt, rp.cand_thr = b.pb.cthr, rp.qmap = qmap;
+    rp.mu = o.mu, rp.nu = o.nu, rp.nu_flag = o.qflag;
+    rp.q_norm_hat = o.qnh, rp.q_norm_res = o.qnr, rp.q_norm_x = o.qnx, rp.g_max = o.gmax;
     rp.g_index_base = g_index_base, rp.g_index_stride = g_index_stride, rp.out_scores = out_scores, rp.out_idx = out_idx;
     rp.flagged = flagged, rp.n_flagged = n_flagged, rp.thr_next = thr_next;
     // one warp per query when a q-tile's candidate slots fit a lane each and four queries' rows fit a block's shared memory
@@ -2105,29 +1048,29 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     auto kern = warp_form ? rescore_select_kernel<32> : rescore_select_kernel<kRescoreThreads>;
     return launch(kern, (pp.nq + per_block - 1) / per_block, kRescoreThreads, smem, stream, "sim_topk", rp);
   };
-  if (int rc = rescore(pl.p0, nullptr, flag0, counts + 0, thr1)) return rc;
+  if (int rc = rescore(pl.p0, nullptr, b.flag0, b.counts + 0, b.thr1)) return rc;
 
   int h_counts[2] = {0, 0};
   unsigned long long h_clk[4] = {0, 0, 0, 0};
-  DCR_CUDA_CHECK(cudaMemcpyAsync(h_counts, counts, 8, cudaMemcpyDeviceToHost, stream));
-  DCR_CUDA_CHECK(cudaMemcpyAsync(h_clk, clk, 32, cudaMemcpyDeviceToHost, stream));
+  DCR_CUDA_CHECK(cudaMemcpyAsync(h_counts, b.counts, 8, cudaMemcpyDeviceToHost, stream));
+  DCR_CUDA_CHECK(cudaMemcpyAsync(h_clk, b.clk, 32, cudaMemcpyDeviceToHost, stream));
   DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
   int n_second = 0;
-  const int* exact_list = flag0;
+  const int* exact_list = b.flag0;
   int n_exact = h_counts[0];
   if (h_counts[0] > 0 && pl.kp1) {
     // second chance: the flagged queries alone, 32 candidates per (query, segment)
     n_second = h_counts[0];
     PassPlan p1;
     if (int rc = plan_pass(n_second, pl.kp1, pl, di->num_sms, di->max_smem_optin, d, k, &p1)) return rc;
-    gather_rows_kernel<<<std::min(di->num_sms * 8, (p1.nq_pad * (pl.d_pad / 8) + 255) / 256), 256, 0, stream>>>(
-        qb, flag0, n_second, p1.nq_pad, pl.d_pad, qb1);
-    count_launch();
-    if (int rc = launch_fused(pl, p1, qb1, gb, ng, pb, bias, qflag, thr1, nullptr, gthr, stream)) return rc;
-    if (int rc = rescore(p1, flag0, flag1, counts + 1, nullptr)) return rc;
-    DCR_CUDA_CHECK(cudaMemcpyAsync(h_counts, counts, 8, cudaMemcpyDeviceToHost, stream));
+    if (int rc = launch(gather_rows_kernel, std::min(di->num_sms * 8, (p1.nq_pad * (pl.d_pad / 8) + 255) / 256), 256, 0,
+                        stream, "sim_topk", o.qb, b.flag0, n_second, p1.nq_pad, pl.d_pad, b.qb1))
+      return rc;
+    if (int rc = launch_fused(pl, p1, b.qb1, o.gb, ng, b.pb, o.bias, o.qflag, b.thr1, nullptr, b.gthr, stream)) return rc;
+    if (int rc = rescore(p1, b.flag0, b.flag1, b.counts + 1, nullptr)) return rc;
+    DCR_CUDA_CHECK(cudaMemcpyAsync(h_counts, b.counts, 8, cudaMemcpyDeviceToHost, stream));
     DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
-    exact_list = flag1;
+    exact_list = b.flag1;
     n_exact = h_counts[1];
   }
 
@@ -2136,16 +1079,15 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     // queries per brute-force launch: as many as fit in shared memory next to each other (32 up to d = 1536)
     const int ex_batch = std::max(1, std::min<int>(kExactBatch, static_cast<int>(192 * 1024 / (static_cast<size_t>(d) * 4))));
     const size_t ex_smem = static_cast<size_t>(ex_batch) * d * 4;
-    const int* n_dev = (exact_list == flag0) ? counts + 0 : counts + 1;
+    const int* n_dev = (exact_list == b.flag0) ? b.counts + 0 : b.counts + 1;
     for (int done = 0; done < n_exact; done += ex_batch) {
       if (int rc = launch(exact_scan_kernel, di->num_sms * 2, 256, ex_smem, stream, "sim_topk", q, g, ng, d, exact_list, done,
-                          n_dev, exact, ex_batch))
+                          n_dev, b.exact, ex_batch))
         return rc;
-      exact_select_kernel<<<ex_batch, 256, 0, stream>>>(exact, ng, k, exact_list, done, n_dev, g_index_base,
-                                                           g_index_stride, out_scores, out_idx);
-      count_launch();
+      if (int rc = launch(exact_select_kernel, ex_batch, 256, 0, stream, "sim_topk", b.exact, ng, k, exact_list, done, n_dev,
+                          g_index_base, g_index_stride, out_scores, out_idx))
+        return rc;
     }
-    DCR_CUDA_CHECK(cudaGetLastError());
     DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
   }
 
@@ -2167,129 +1109,6 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     stats->n_second = n_second;
     stats->d_pad = pl.d_pad;
   }
-  return 0;
-}
-
-size_t sim_range_workspace_size(int nq, int ng, int d, long long max_pairs) {
-  const DeviceInfo* di = device_info();
-  RangePlan rp;
-  if (make_range_plan(nq, ng, d, max_pairs, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &rp) != 0) return 0;
-  return rp.total;
-}
-
-int sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, long long g_index_base,
-              long long g_index_stride, long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,
-              long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
-  const DeviceInfo* di = device_info();
-  if (!di) return -2;
-  if (int rc = require_sm90a(di, "sim_range")) return rc;
-  DCR_REQUIRE(!std::isnan(threshold), "sim_range: threshold is NaN");
-  DCR_REQUIRE(g_index_stride >= 1, "sim_range: g_index_stride=%lld < 1", g_index_stride);
-  RangePlan rp;
-  if (int rc = make_range_plan(nq, ng, d, max_pairs, di->num_sms, di->max_smem_optin, &rp)) return rc;
-  DCR_REQUIRE(ws != nullptr && ws_bytes >= rp.total, "sim_range: workspace too small (%zu < %zu)", ws_bytes, rp.total);
-  DCR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "sim_range: workspace must be 256-byte aligned");
-  DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0,
-              "sim_range: q/g must be 16-byte aligned");
-  const SimPlan& geo = rp.geo;
-  uint8_t* w = static_cast<uint8_t*>(ws);
-  auto* qb = reinterpret_cast<__nv_bfloat16*>(w + rp.off_qb);
-  auto* gb = reinterpret_cast<__nv_bfloat16*>(w + rp.off_gb);
-  auto* qnh = reinterpret_cast<float*>(w + rp.off_qnh);
-  auto* qnr = reinterpret_cast<float*>(w + rp.off_qnr);
-  auto* qnx = reinterpret_cast<float*>(w + rp.off_qnx);
-  auto* gmax = reinterpret_cast<unsigned int*>(w + rp.off_gmax);
-  auto* mu = reinterpret_cast<float*>(w + rp.off_mu);
-  auto* nu = reinterpret_cast<float*>(w + rp.off_nu);
-  auto* bias = reinterpret_cast<float*>(w + rp.off_bias);
-  auto* qflag = reinterpret_cast<int*>(w + rp.off_flag);
-  auto* thr = reinterpret_cast<float*>(w + rp.off_thr);
-  auto* seg = reinterpret_cast<int*>(w + rp.off_seg);
-  auto* row_cnt = reinterpret_cast<long long*>(w + rp.off_row_cnt);
-  auto* row_cand = reinterpret_cast<long long*>(w + rp.off_row_cand);
-  auto* row_pcnt = reinterpret_cast<long long*>(w + rp.off_row_pcnt);
-  auto* row_piece = reinterpret_cast<long long*>(w + rp.off_row_piece);
-  auto* cand_idx = reinterpret_cast<int*>(w + rp.off_cand_idx);
-  auto* cand_score = reinterpret_cast<float*>(w + rp.off_cand_score);
-  auto* piece_kept = reinterpret_cast<int*>(w + rp.off_piece_kept);
-  auto* piece_excl = reinterpret_cast<long long*>(w + rp.off_piece_excl);
-
-  const Operands ops = {qb, gb, qnh, qnr, qnx, gmax, reinterpret_cast<double*>(w + rp.off_colsum), mu, nu, bias, qflag};
-  if (int rc = prepare_operands(q, nq, rp.nq_pad, g, ng, d, geo, di, ops, stream)) return rc;
-  range_threshold_kernel<<<(nq + 3) / 4, 128, 0, stream>>>(q, nq, d, geo.d_pad, threshold, qnh, qnr, qnx, gmax, mu, nu,
-                                                           qflag, thr);
-  count_launch();
-
-  CUtensorMap tq, tg;
-  if (int rc = make_tmap_2d_bf16(&tq, qb, rp.nq_pad, geo.d_pad, geo.d_pad, kBlockM, kBlockK)) return rc;
-  if (int rc = make_tmap_2d_bf16(&tg, gb, geo.ng_pad, geo.d_pad, geo.d_pad, kBlockN, kBlockK)) return rc;
-  RangeParams p;
-  p.nq = nq;
-  p.ng = ng;
-  p.num_kb = geo.num_kb;
-  p.stream_a = geo.stream_a;
-  p.n_qtiles = rp.n_qtiles;
-  p.n_gtiles = geo.n_gtiles;
-  p.gchunk = geo.gchunk;
-  p.n_chunks = geo.n_chunks;
-  p.stages = rp.stages;
-  p.bias_flag = qflag;
-  p.col_bias = bias;
-  p.thr = thr;
-  p.seg = seg;
-  p.row_cand = row_cand;
-  p.cand_idx = cand_idx;
-  auto sweep = [&](auto kern) { return launch(kern, rp.n_units, 32 + 128, rp.smem_bytes, stream, "sim_range", tq, tg, p); };
-  // both centring variants are launched; the one that does not match the device flag returns at once
-  if (int rc = sweep(sim_range_kernel<false, false>)) return rc;
-  if (int rc = sweep(sim_range_kernel<true, false>)) return rc;
-  range_slot_scan_kernel<<<(nq + 255) / 256, 256, 0, stream>>>(seg, nq, rp.n_qtiles, geo.n_gtiles, geo.gchunk,
-                                                                geo.n_chunks, rp.n_units, row_cnt, row_pcnt);
-  count_launch();
-  exclusive_scan_kernel<long long><<<1, 1024, 0, stream>>>(row_cnt, nq, row_cand);
-  count_launch();
-  exclusive_scan_kernel<long long><<<1, 1024, 0, stream>>>(row_pcnt, nq, row_piece);
-  count_launch();
-  long long h_tot[2] = {0, 0};   // candidates, pieces
-  DCR_CUDA_CHECK(cudaMemcpyAsync(h_tot, row_cand + nq, 8, cudaMemcpyDeviceToHost, stream));
-  DCR_CUDA_CHECK(cudaMemcpyAsync(h_tot + 1, row_piece + nq, 8, cudaMemcpyDeviceToHost, stream));
-  DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
-  const long long n_cand = h_tot[0], n_pieces = h_tot[1];
-  counts[0] = 0;
-  counts[1] = n_cand;
-  if (n_cand > max_pairs)
-    return set_error(DCR_ERR_CAPACITY, "sim_range: %lld candidate pairs exceed max_pairs=%lld (call again with that capacity)",
-                     n_cand, max_pairs);
-
-  if (n_pieces > 0) {
-    if (int rc = sweep(sim_range_kernel<false, true>)) return rc;
-    if (int rc = sweep(sim_range_kernel<true, true>)) return rc;
-    if (int rc = launch(range_rescore_kernel, static_cast<unsigned>(n_pieces), kRescoreThreads, static_cast<size_t>(d) * 8,
-                        stream, "sim_range", q, g, nq, d, threshold, row_cand, row_piece, cand_idx, cand_score, piece_kept))
-      return rc;
-  }
-  exclusive_scan_kernel<int><<<1, 1024, 0, stream>>>(piece_kept, n_pieces, piece_excl);
-  count_launch();
-  if (n_pieces > 0) {
-    range_output_kernel<<<static_cast<unsigned>(n_pieces), 256, 0, stream>>>(row_cand, row_piece, nq, piece_excl, cand_idx,
-                                                                             cand_score, g_index_base, g_index_stride,
-                                                                             out_idx, out_scores);
-    count_launch();
-  }
-  range_row_offsets_kernel<<<grid_for(nq + 1, 256, di->num_sms), 256, 0, stream>>>(row_piece, piece_excl, nq, row_offsets);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  long long h_pairs = 0;
-  DCR_CUDA_CHECK(cudaMemcpyAsync(&h_pairs, piece_excl + n_pieces, 8, cudaMemcpyDeviceToHost, stream));
-  DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
-  counts[0] = h_pairs;
-  return 0;
-}
-
-int exclusive_scan_i64(const long long* in, long long n, long long* out, cudaStream_t stream) {
-  exclusive_scan_kernel<long long><<<1, 1024, 0, stream>>>(in, n, out);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 

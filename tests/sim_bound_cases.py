@@ -1,7 +1,7 @@
 """Operands that drive the bf16 error of the fused similarity sweep to its bound (test infrastructure only).
 
 dcr_sim_topk and dcr_sim_range both rank on a bf16 tensor-core score and trust one number per query, the `eps` of
-row_bound (dcr_b200/csrc/sim_topk.cu), to bound |approximate score - exact centred score|.  Random descriptors keep that
+row_bound (dcr_b200/csrc/sim_sweep.cuh), to bound |approximate score - exact centred score|.  Random descriptors keep that
 error far below the bound.  The instances built here reach it, and they are built so that a CPU restatement of stage 1
 reproduces the kernel's operands bit for bit:
 

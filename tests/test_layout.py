@@ -73,3 +73,6 @@ def test_hopper_scaffolding_has_one_definition():
     for needle, home in [("cudaFuncSetAttribute", "host_util.cu"), ("cp.async.bulk.commit_group", "ptx.cuh"),
                          ("cp.async.bulk.wait_group", "ptx.cuh"), ("~uintptr_t(1023)", "ptx.cuh")]:
         assert [f for f, t in texts.items() if needle in t] == [home], needle
+    # the similarity engine launches every kernel through host_util's launch(): counted, error-checked, smem opted in
+    for f in ("sim_sweep.cu", "sim_topk.cu", "sim_range.cu"):
+        assert "<<<" not in texts[f], f
