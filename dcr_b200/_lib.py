@@ -26,6 +26,9 @@ SIGNATURES = {
     "dcr_sim_topk_workspace_size": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "dcr_sim_topk": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64,
                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dcr_sim_topk_split_workspace_size": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "dcr_sim_topk_split": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64,
+                                     C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "dcr_sim_topk_host": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                     C.c_void_p]),
     "dcr_sim_topk_sharded_workspace_size": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),

@@ -211,18 +211,24 @@ def main_worker(gpu, ngpus_per_node, args) -> int:
         out = retrieval.run_retrieval(net, query_u8, values_u8, k=k, with_background=(split == 1), num_loss_chunks=split,
                                       cross=cross, threshold=args.sim_threshold)
     else:
-        if split > 1:
-            raise NotImplementedError("--similarity_metric splitloss runs on one GPU (the sharded path merges dot-product lists)")
         embed = retrieval.extract_features_multiscale if isinstance(net, (list, tuple)) else retrieval.extract_features
         gf = similarity.l2_normalize_(embed(net, values_u8))                                    # :386, :388
         qf = similarity.l2_normalize_(embed(net, query_u8))                                     # :387, :389
         q_sizes = [b - a for a, b in (ddist.shard_bounds(len(q_files), r, world) for r in range(world))]
         v_sizes = [b - a for a, b in (ddist.shard_bounds(len(v_files), r, world) for r in range(world))]
-        main_v, main_l = ddist.sharded_topk(qf, gf, k, vlo, ddist.cuda_local_topk, ddist.cuda_merge, query_sizes=q_sizes)
-        bg, _ = ddist.sharded_topk(gf, gf, min(2, len(v_files)), vlo, ddist.cuda_local_topk, ddist.cuda_merge,
-                                   query_sizes=v_sizes)                                         # :403, :418
-        out = {"values": main_v, "indices": main_l, "bg_values": bg[:, -1],
-               "stats": retrieval.retrieval_stats(main_v[:, 0], bg[:, -1])}
+        if split > 1:
+            # splitloss: every rank ranks all queries against its gallery shard under the split score (global indices),
+            # the lists are merged as for the dot product; no background statistics, as on one GPU
+            local = ddist.split_local_topk(split, cross)
+            main_v, main_l = ddist.sharded_topk(qf, gf, k, vlo, local, ddist.cuda_merge, query_sizes=q_sizes)
+            out = {"values": main_v, "indices": main_l, "stats": retrieval.retrieval_stats(main_v[:, 0])}
+        else:
+            main_v, main_l = ddist.sharded_topk(qf, gf, k, vlo, ddist.cuda_local_topk, ddist.cuda_merge,
+                                                query_sizes=q_sizes)
+            bg, _ = ddist.sharded_topk(gf, gf, min(2, len(v_files)), vlo, ddist.cuda_local_topk, ddist.cuda_merge,
+                                       query_sizes=v_sizes)                                     # :403, :418
+            out = {"values": main_v, "indices": main_l, "bg_values": bg[:, -1],
+                   "stats": retrieval.retrieval_stats(main_v[:, 0], bg[:, -1])}
     fid_val = None
     if args.fid_weights and world > 1:
         # every rank embeds its shard of both folders; the fp64 statistics are merged over the ranks (dcr_b200/fid.py)

@@ -38,6 +38,19 @@ int dcr_sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, i
                        &g_last_stats);
 }
 
+size_t dcr_sim_topk_split_workspace_size(int nq, int ng, int d, int n_parts, int k) {
+  return dcr::sim_topk_split_workspace_size(nq, ng, d, n_parts, k);
+}
+
+int dcr_sim_topk_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, int k, int64_t g_index_base,
+                       int64_t g_index_stride, float* out_scores, int64_t* out_idx, void* workspace, size_t workspace_bytes,
+                       void* stream) {
+  DCR_REQUIRE(q && g && out_scores && out_idx, "dcr_sim_topk_split: null pointer argument");
+  return dcr::sim_topk_split(q, nq, g, ng, d, n_parts, k, g_index_base, g_index_stride, out_scores,
+                             reinterpret_cast<long long*>(out_idx), workspace, workspace_bytes, as_stream(stream),
+                             &g_last_stats);
+}
+
 int dcr_sim_topk_host(const float* q, int nq, const float* g, int ng, int d, int k, float* out_scores,
                       int64_t* out_idx) {
   DCR_REQUIRE(q && g && out_scores && out_idx, "dcr_sim_topk_host: null pointer argument");

@@ -28,6 +28,12 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
              long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
              cudaStream_t stream, SimStats* stats);
 
+// top-k under the split score: max over the n_parts equal parts of the per-part dot products (sim_topk.cu)
+size_t sim_topk_split_workspace_size(int nq, int ng, int d, int n_parts, int k);
+int sim_topk_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, int k, long long g_index_base,
+                   long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
+                   cudaStream_t stream, SimStats* stats);
+
 size_t sim_range_workspace_size(int nq, int ng, int d, long long max_pairs);
 int sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, long long g_index_base,
               long long g_index_stride, long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,

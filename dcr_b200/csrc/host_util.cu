@@ -71,7 +71,8 @@ int require_sm90a(const DeviceInfo* di, const char* who) {
 }
 
 int allow_dynamic_smem(const void* func, size_t bytes, const char* who) {
-  if (bytes <= 48 * 1024) return 0;
+  // within the default 48 KB even next to 16 KB of static shared memory (the default counts both; no kernel here has more)
+  if (bytes <= 32 * 1024) return 0;
   const DeviceInfo* di = device_info();
   if (!di) return -2;
   static std::map<std::pair<const void*, int>, size_t> limits;   // (kernel, device) -> dynamic shared memory allowed

@@ -53,8 +53,8 @@ const DeviceInfo* device_info();
 // 0 on an sm_90 device, else -1 with an error naming `who`: the tensor-core kernels are built for sm_90a only
 int require_sm90a(const DeviceInfo* di, const char* who);
 
-// Lets `func` be launched with `bytes` of dynamic shared memory on the current device.  Above the default 48 KB the
-// kernel's limit is raised to the most the device allows it (the opt-in maximum less its static shared memory), once per
+// Lets `func` be launched with `bytes` of dynamic shared memory on the current device.  Above 32 KB (the default 48 KB
+// counts static shared memory too) the kernel's limit is raised to the most the device allows it (the opt-in maximum less its static shared memory), once per
 // (kernel, device), so every later size is covered; more than that is refused (-1, naming `who`).
 int allow_dynamic_smem(const void* func, size_t bytes, const char* who);
 

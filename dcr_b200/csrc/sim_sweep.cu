@@ -197,7 +197,100 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// Stage 1 under the split score: part c of row r (p floats) -> bf16 at [r][c p_pad, c p_pad + p), zeros up to
+// (c + 1) p_pad, and the norms of that part (as to_bf16_rows_kernel) at norm_*[r n_parts + c]; gmax[2c], gmax[2c + 1] =
+// the maxima over the rows of part c.  A warp per (row, part), walked part-major: a warp's running maxima change part
+// rarely, so it issues one pair of atomics per part it leaves instead of one per row.
+__global__ void __launch_bounds__(256)
+    to_bf16_parts_kernel(const float* __restrict__ x, int n, int n_pad, int n_parts, int p, int p_pad,
+                         __nv_bfloat16* __restrict__ out, float* __restrict__ norm_hat, float* __restrict__ norm_res,
+                         float* __restrict__ norm_x, unsigned int* __restrict__ gmax) {
+  const int lane = threadIdx.x & 31;
+  const long long warps = static_cast<long long>(gridDim.x) * (blockDim.x >> 5);
+  const long long total = static_cast<long long>(n_parts) * n_pad;
+  const size_t d = static_cast<size_t>(n_parts) * p, d_pad = static_cast<size_t>(n_parts) * p_pad;
+  int cur = -1;
+  unsigned int w_nx = 0u, w_nr = 0u;   // running maxima of part `cur` (lane 0)
+  auto flush = [&]() {
+    if (gmax && cur >= 0 && lane == 0) {
+      atomicMax(gmax + 2 * cur, w_nx);
+      atomicMax(gmax + 2 * cur + 1, w_nr);
+    }
+  };
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x >> 5) + (threadIdx.x >> 5); i < total; i += warps) {
+    const int c = static_cast<int>(i / n_pad), row = static_cast<int>(i % n_pad);
+    if (c != cur) {
+      flush();
+      cur = c;
+      w_nx = w_nr = 0u;
+    }
+    const float* xr = x + static_cast<size_t>(row) * d + static_cast<size_t>(c) * p;
+    __nv_bfloat16* o = out + static_cast<size_t>(row) * d_pad + static_cast<size_t>(c) * p_pad;
+    float s_hat = 0.f, s_res = 0.f, s_x = 0.f;
+    for (int e = lane * 4; e < p_pad; e += 128) {
+      const float4 v = (row < n && e < p) ? *reinterpret_cast<const float4*>(xr + e) : make_float4(0.f, 0.f, 0.f, 0.f);   // p % 4 == 0
+      const __nv_bfloat16 h0 = __float2bfloat16_rn(v.x), h1 = __float2bfloat16_rn(v.y);
+      const __nv_bfloat16 h2 = __float2bfloat16_rn(v.z), h3 = __float2bfloat16_rn(v.w);
+      const float f0 = __bfloat162float(h0), f1 = __bfloat162float(h1), f2 = __bfloat162float(h2), f3 = __bfloat162float(h3);
+      s_hat += f0 * f0 + f1 * f1 + f2 * f2 + f3 * f3;
+      s_res += (v.x - f0) * (v.x - f0) + (v.y - f1) * (v.y - f1) + (v.z - f2) * (v.z - f2) + (v.w - f3) * (v.w - f3);
+      s_x += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+      uint2 pk;
+      pk.x = static_cast<uint32_t>(__bfloat16_as_ushort(h0)) | (static_cast<uint32_t>(__bfloat16_as_ushort(h1)) << 16);
+      pk.y = static_cast<uint32_t>(__bfloat16_as_ushort(h2)) | (static_cast<uint32_t>(__bfloat16_as_ushort(h3)) << 16);
+      *reinterpret_cast<uint2*>(o + e) = pk;
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      s_hat += __shfl_xor_sync(kFull, s_hat, off);
+      s_res += __shfl_xor_sync(kFull, s_res, off);
+      s_x += __shfl_xor_sync(kFull, s_x, off);
+    }
+    if (lane == 0 && row < n) {
+      const float nh = sqrtf(s_hat) * 1.0001f, nr = sqrtf(s_res) * 1.0001f, nx = sqrtf(s_x) * 1.0001f;
+      const size_t j = static_cast<size_t>(row) * n_parts + c;
+      if (norm_hat) norm_hat[j] = nh;
+      if (norm_res) norm_res[j] = nr;
+      if (norm_x) norm_x[j] = nx;
+      w_nx = max(w_nx, __float_as_uint(nx));
+      w_nr = max(w_nr, __float_as_uint(nr));
+    }
+  }
+  flush();
+}
+
 }  // namespace
+
+void plan_split_geometry(int ng, int n_parts, int p, SweepGeometry* geo) {
+  const int p_pad = (p + kBlockK - 1) / kBlockK * kBlockK;
+  plan_geometry(ng, n_parts * p_pad, geo);   // the chunks of the dot product over the part-padded rows
+  // always streamed: the consumer warpgroups need the shared memory of two column halves' lists (the running maximum of
+  // a 128-column tile does not fit a thread's registers), and d_pad is far above 512 for per-token descriptors
+  geo->stream_a = 1;
+}
+
+Operands carve_split_operands(Carve& w, int nq_pad, const SweepGeometry& geo, int n_parts) {
+  Operands o = {};
+  o.qb = w.take<__nv_bfloat16>(static_cast<size_t>(nq_pad) * geo.d_pad);
+  o.gb = w.take<__nv_bfloat16>(static_cast<size_t>(geo.ng_pad) * geo.d_pad);
+  o.qnh = w.take<float>(static_cast<size_t>(nq_pad) * n_parts);
+  o.qnr = w.take<float>(static_cast<size_t>(nq_pad) * n_parts);
+  o.qnx = w.take<float>(static_cast<size_t>(nq_pad) * n_parts);
+  o.gmax = w.take<unsigned int>(2 * static_cast<size_t>(n_parts));
+  return o;
+}
+
+int prepare_split_operands(const float* q, int nq, int nq_pad, const float* g, int ng, int n_parts, int p,
+                           const SweepGeometry& geo, const DeviceInfo* di, const Operands& o, cudaStream_t stream) {
+  DCR_CUDA_CHECK(cudaMemsetAsync(o.gmax, 0, 8 * static_cast<size_t>(n_parts), stream));
+  const int p_pad = geo.d_pad / n_parts;
+  const int blocks = di->num_sms * 8;
+  if (int rc = launch(to_bf16_parts_kernel, blocks, 256, 0, stream, "sim_sweep", q, nq, nq_pad, n_parts, p, p_pad, o.qb,
+                      o.qnh, o.qnr, o.qnx, nullptr))
+    return rc;
+  return launch(to_bf16_parts_kernel, blocks, 256, 0, stream, "sim_sweep", g, ng, geo.ng_pad, n_parts, p, p_pad, o.gb,
+                nullptr, nullptr, nullptr, o.gmax);
+}
 
 void plan_geometry(int ng, int d, SweepGeometry* geo) {
   geo->d_pad = (d + kBlockK - 1) / kBlockK * kBlockK;

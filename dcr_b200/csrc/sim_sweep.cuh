@@ -225,6 +225,54 @@ DCR_DEVICE void fused_tile_mma(WgAcc<kCols>& acc, PipeState& st, const FusedPipe
   }
 }
 
+// The same k-loop under the split score (descriptors cut into parts of kb_part k-blocks each, DESIGN.md section 3): each
+// part's first k-block overwrites the part accumulator, and after its last one the accumulator is folded into `best`,
+// the running element-wise maximum over the parts (fmaxf: a NaN part is ignored, as in the exact split score).  A part
+// boundary waits for every MMA in flight, because the fold reads the accumulator, and then releases both stages it held.
+template <int kCols>
+DCR_DEVICE void fused_tile_mma_split(WgAcc<kCols>& best, PipeState& st, const FusedPipe& pp, uint32_t a_base,
+                                     uint32_t b_base, int kb_part, bool last, uint32_t lane) {
+  const uint32_t a_step = pp.stream_a ? 0u : static_cast<uint32_t>(kATileBytes);
+  WgAcc<kCols> part;
+#pragma unroll
+  for (int s = 0; s < 2; ++s)
+#pragma unroll
+    for (int i = 0; i < kCols / 2; ++i) best.d[s][i] = -INFINITY;
+  uint32_t prev_s = 0;
+  bool held = false;   // stage prev_s is still read by an MMA that may be in flight
+  int kin = 0;         // k-block within the current part
+  for (int kb = 0; kb < pp.num_kb; ++kb, st.next()) {
+    const uint32_t s = st.s;
+    mbar_wait(&pp.b_full[s], st.ph);
+    const uint32_t a_addr = a_base + (pp.stream_a ? s * static_cast<uint32_t>(pp.stage_bytes) : static_cast<uint32_t>(kb) * a_step);
+    const uint32_t b_addr = b_base + s * static_cast<uint32_t>(pp.stage_bytes);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBlockK / 16; ++k) part.mma(a_addr + 32 * k, wgmma_desc_sw128(b_addr + 32 * k), (kin | k) != 0);
+    wgmma_commit();
+    if (++kin == kb_part) {
+      wgmma_wait<0>();
+      part.fence_regs();
+      if (lane == 0) {
+        if (held) mbar_arrive(&pp.b_empty[prev_s]);
+        mbar_arrive(&pp.b_empty[s]);
+      }
+      held = false;
+      kin = 0;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < kCols / 2; ++i) best.d[h][i] = fmaxf(best.d[h][i], part.d[h][i]);
+    } else {
+      wgmma_wait<1>();
+      if (held && lane == 0) mbar_arrive(&pp.b_empty[prev_s]);
+      held = true;
+      prev_s = s;
+    }
+  }
+  if (lane == 0 && !pp.stream_a && last) mbar_arrive(pp.a_empty);   // num_kb is a whole number of parts: nothing held
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // The exact dot product: fp64 accumulate with one fixed association.  Lane l owns the elements l*4 + 128*i (float4
 // granules), accumulates them in ascending order with fma, then a fixed xor butterfly from 16 down to 1.  Every exact
@@ -412,6 +460,37 @@ DCR_DEVICE RowBound row_bound(const TQ* __restrict__ q, int d, int d_pad, int qr
   return rb;
 }
 
+// The same bound under the split score, whose operands are not centred (qmu = 0).  Part c of a pair is a p-term dot
+// product accumulated over p_pad, bounded as above from the part's own norms (q_norm_*[qrow * n_parts + c], g_max[2c],
+// g_max[2c + 1]), and |max_c a_c - max_c s_c| <= max_c |a_c - s_c|: the bound is the largest over the parts.  A NaN
+// part norm makes eps NaN, so the certificate fails rather than leave that part unbounded.  Whole warp.
+DCR_DEVICE RowBound split_row_bound(int n_parts, int p, int p_pad, int qrow, const float* __restrict__ q_norm_hat,
+                                    const float* __restrict__ q_norm_res, const float* __restrict__ q_norm_x,
+                                    const unsigned int* __restrict__ g_max, uint32_t lane) {
+  float eps = 0.f;
+  double slack = 0.0;
+  bool nan = false;
+  for (int c = static_cast<int>(lane); c < n_parts; c += 32) {
+    const float g_norm = __uint_as_float(g_max[2 * c]), g_res = __uint_as_float(g_max[2 * c + 1]);
+    const size_t i = static_cast<size_t>(qrow) * n_parts + c;
+    const float qh = q_norm_hat[i], qr = q_norm_res[i], qx = q_norm_x[i];
+    const float e = 1.001f * (qh * g_res + qr * g_norm) + p_pad * 2.4e-7f * qh * (g_norm + g_res) + 3e-7f * qx * g_norm + 1e-30f;
+    nan |= (e != e);
+    eps = fmaxf(eps, e);
+    slack = fmax(slack, 4.6e-16 * (p + 8) * static_cast<double>(qx) * static_cast<double>(g_norm));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    eps = fmaxf(eps, __shfl_xor_sync(kFull, eps, o));
+    slack = fmax(slack, __shfl_xor_sync(kFull, slack, o));
+  }
+  RowBound rb;
+  rb.eps = __any_sync(kFull, nan) ? __int_as_float(0x7fc00000) : eps;
+  rb.qmu = 0.0;
+  rb.slack = slack;
+  return rb;
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // host side, defined in sim_sweep.cu
 
@@ -437,6 +516,14 @@ struct Operands {
 Operands carve_operands(Carve& w, int nq_pad, const SweepGeometry& geo, int d);
 int prepare_operands(const float* q, int nq, int nq_pad, const float* g, int ng, int d, const SweepGeometry& geo,
                      const DeviceInfo* di, const Operands& o, cudaStream_t stream);
+
+// Stage 1 under the split score: rows of n_parts parts of p values, each part zero-padded to p_pad = ceil64(p) so that a
+// part boundary is a k-block boundary (d_pad = n_parts * p_pad).  No centring.  Norms per part: qnh / qnr / qnx hold
+// [nq_pad][n_parts], gmax [n_parts][2] the gallery maxima of each part; mu, nu, bias, colsum and qflag stay unused.
+void plan_split_geometry(int ng, int n_parts, int p, SweepGeometry* geo);
+Operands carve_split_operands(Carve& w, int nq_pad, const SweepGeometry& geo, int n_parts);
+int prepare_split_operands(const float* q, int nq, int nq_pad, const float* g, int ng, int n_parts, int p,
+                           const SweepGeometry& geo, const DeviceInfo* di, const Operands& o, cudaStream_t stream);
 
 // The head of a sweep over the first n_qtiles query tiles of qb against gb, and the tensor maps of both operands
 int sweep_setup(const SweepGeometry& geo, int nq, int n_qtiles, int ng, int gchunk, int n_chunks, const __nv_bfloat16* qb,

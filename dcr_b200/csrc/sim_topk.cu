@@ -47,6 +47,7 @@ struct SimParams : SweepHead {
   unsigned int* gthr;      // [nq_pad] per query row: best threshold any unit has reached so far, as an order-preserving
                            // unsigned key (0 = none)
   unsigned long long* clk; // [4] clock64 / globaltimer at the start and end of CTA 0 (SM clock under this kernel); null = off
+  int kb_part;             // split score: k-blocks per descriptor part (kSplit kernels only)
 };
 
 // second-chance pass: copy the bf16 rows of the flagged queries into a compact matrix (zero rows up to n_pad)
@@ -243,10 +244,13 @@ DCR_DEVICE float seed_threshold(float (&slot)[32], int kp) {
 // replaying the first kWarmTiles tiles.  Segment (unit u, q-tile i) owns candidate slot u + i.
 // kBias: compiled with / without the per-column offset path of query centring.  Both variants are launched; the one
 // that does not match the device-side decision (p.bias_flag) exits at once -- no host synchronisation needed.
-template <bool kBias, int kSets>
+// kSplit: the split score (sim_topk_split): every tile's approximate score is the maximum over the descriptor parts
+// (fused_tile_mma_split); the filter and the lists see that maximum.  Built with kSets = 2 and without kBias only.
+template <bool kBias, int kSets, bool kSplit = false>
 __global__ void __launch_bounds__(32 + 128 * kSets, 1)
     sim_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_g,
                     const SimParams p) {
+  static_assert(!kSplit || (kSets == 2 && !kBias), "the split score runs on column halves, uncentred");
   if (((p.bias_flag != nullptr) && (*p.bias_flag != 0)) != kBias) return;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr int kSetCols = kBlockN / kSets;
@@ -326,7 +330,8 @@ __global__ void __launch_bounds__(32 + 128 * kSets, 1)
         unsigned int shared_key = 0;
         if (!kWarm && gslot) shared_key = *reinterpret_cast<volatile unsigned int*>(gslot);
         WgAcc<kSetCols> acc;
-        fused_tile_mma(acc, st, pp, a_base, b_base, last, lane);
+        if constexpr (kSplit) fused_tile_mma_split(acc, st, pp, a_base, b_base, p.kb_part, last, lane);
+        else fused_tile_mma(acc, st, pp, a_base, b_base, last, lane);
         if (!kWarm && gslot) {
           if (thr > published) {   // risen since the last publication (compaction): let the other units know
             atomicMax(gslot, thr_key(thr));
@@ -444,6 +449,9 @@ DCR_DEVICE void block_argbest(double& bs, long long& bi, int& bp, BlockBest<kWar
 //   3. exact fp64 scores of the survivors, selection by (score desc, index asc)
 //   4. certificate against the rows the fused kernel dropped; failures are appended to `flagged` together with
 //      a threshold for the second-chance pass (thr_next).
+// kSplit: the split score.  The exact score of a candidate is the maximum over the parts of exact_dot over that part, the
+// query staged in shared memory one part at a time (rows are far wider than shared memory), and the bound is
+// split_row_bound.
 struct RescoreParams {
   const float* q;                   // the caller's query rows [*][d]
   const float* g;                   // [ng][d]
@@ -468,6 +476,7 @@ struct RescoreParams {
   int* flagged;                     // caller rows whose certificate failed, counted by *n_flagged
   int* n_flagged;
   float* thr_next;                  // per flagged entry: start threshold of the second-chance pass; null = last pass
+  int n_parts;                      // split score (kSplit): descriptor parts of d / n_parts values; q_norm_* per part
 };
 
 // One query's shared memory: the query row widened to fp64, then four arrays of max_cand entries.  Every part is a
@@ -484,7 +493,7 @@ struct RescoreSmem {
   }
 };
 
-template <int kThreads>
+template <int kThreads, bool kSplit = false>
 __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const RescoreParams p) {
   constexpr int kWarps = kThreads / 32;
   extern __shared__ __align__(16) uint8_t sm[];
@@ -495,9 +504,9 @@ __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const R
   // crow indexes the (possibly compacted) query matrix the fused kernel saw; qrow is the caller's row
   const int crow = blockIdx.x * (kRescoreThreads / kThreads) + grp;
   if (crow >= p.nq) return;   // whole groups leave; nothing below synchronises across groups
-  const RescoreSmem L(p.d, p.max_cand);
+  const RescoreSmem L(kSplit ? p.d / p.n_parts : p.d, p.max_cand);
   uint8_t* base = sm + grp * L.bytes;
-  double* qs = reinterpret_cast<double*>(base);          // [d] the query row, widened once
+  double* qs = reinterpret_cast<double*>(base);          // [d] the query row, widened once ([d / n_parts]: one part)
   double* sc = reinterpret_cast<double*>(base + L.sc);   // exact scores of the survivors
   int* ci = reinterpret_cast<int*>(base + L.ci);         // gallery rows of all candidates
   float* ap = reinterpret_cast<float*>(base + L.ap);     // approximate scores
@@ -511,7 +520,7 @@ __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const R
 #pragma unroll
   for (int i = 0; i < kQv; ++i) {
     const int c = (i * kThreads + tid) * 4;
-    if (c < d) qv[i] = *reinterpret_cast<const float4*>(p.q + static_cast<size_t>(qrow) * d + c);   // d % 4 == 0
+    if (!kSplit && c < d) qv[i] = *reinterpret_cast<const float4*>(p.q + static_cast<size_t>(qrow) * d + c);   // d % 4 == 0
   }
 
   // ---- the (chunk, unit, set) slots that cover this q-tile, in rounds: lane c owns chunk c0 + c (every warp of the group
@@ -566,21 +575,28 @@ __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const R
   }
   if (overflow) n = 0;   // k >= 1: the certificate fails and the query is flagged
   thr = group_max<kThreads>(thr);
+  if constexpr (!kSplit) {
 #pragma unroll
-  for (int i = 0; i < kQv; ++i) {
-    const int c = (i * kThreads + tid) * 4;
-    if (c < d) {
-      *reinterpret_cast<double2*>(qs + c) = make_double2(static_cast<double>(qv[i].x), static_cast<double>(qv[i].y));
-      *reinterpret_cast<double2*>(qs + c + 2) = make_double2(static_cast<double>(qv[i].z), static_cast<double>(qv[i].w));
+    for (int i = 0; i < kQv; ++i) {
+      const int c = (i * kThreads + tid) * 4;
+      if (c < d) {
+        *reinterpret_cast<double2*>(qs + c) = make_double2(static_cast<double>(qv[i].x), static_cast<double>(qv[i].y));
+        *reinterpret_cast<double2*>(qs + c + 2) = make_double2(static_cast<double>(qv[i].z), static_cast<double>(qv[i].w));
+      }
     }
+    for (int c = 512 + tid; c < d; c += kThreads) qs[c] = static_cast<double>(p.q[static_cast<size_t>(qrow) * d + c]);
   }
-  for (int c = 512 + tid; c < d; c += kThreads) qs[c] = static_cast<double>(p.q[static_cast<size_t>(qrow) * d + c]);
   group_sync<kThreads>();
 
   // certificate: every gallery row that is not a candidate has approximate centred score <= thr, hence exact score
-  // q.g <= thr + eps + q.mu + slack (row_bound)
-  const RowBound rb = row_bound(qs, d, p.d_pad, qrow, p.q_norm_hat, p.q_norm_res, p.q_norm_x, p.g_max, p.mu, p.nu,
-                                p.nu_flag, lane);
+  // q.g <= thr + eps + q.mu + slack (row_bound; split_row_bound for the split score)
+  const RowBound rb = [&] {
+    if constexpr (kSplit)
+      return split_row_bound(p.n_parts, d / p.n_parts, p.d_pad / p.n_parts, qrow, p.q_norm_hat, p.q_norm_res, p.q_norm_x,
+                             p.g_max, lane);
+    else
+      return row_bound(qs, d, p.d_pad, qrow, p.q_norm_hat, p.q_norm_res, p.q_norm_x, p.g_max, p.mu, p.nu, p.nu_flag, lane);
+  }();
   const float eps = rb.eps;
   const double qmu = rb.qmu;
   const bool closed = thr > -INFINITY;   // some segment dropped rows
@@ -610,27 +626,60 @@ __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const R
     m += kept;
   }
   group_sync<kThreads>();
-  // every surviving row's cache lines are requested at once (L2 prefetch): the dot products below then wait for L2, not for
-  // one DRAM round trip per pair of rows
-  {
-    const int lines = (d * 4 + 127) / 128;
-    for (int t = tid; t < m * lines; t += kThreads) {
-      const float* ptr = p.g + static_cast<size_t>(kc[t / lines]) * d + (t % lines) * 32;
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
+  if constexpr (kSplit) {
+    // ---- exact split scores of the survivors: per part, stage the query part, prefetch that part of every survivor, then
+    // fold each part's dot product into the running maximum (the order of split_rescore_kernel: -inf, then parts 0, 1, ..)
+    const int pl = d / p.n_parts;
+    for (int c = tid; c < m; c += kThreads) sc[c] = -INFINITY;
+    for (int part = 0; part < p.n_parts; ++part) {
+      group_sync<kThreads>();   // the previous part's readers of qs are done
+      const float* qsrc = p.q + static_cast<size_t>(qrow) * d + static_cast<size_t>(part) * pl;
+      for (int c = tid * 4; c < pl; c += kThreads * 4) {
+        const float4 v = *reinterpret_cast<const float4*>(qsrc + c);
+        *reinterpret_cast<double2*>(qs + c) = make_double2(static_cast<double>(v.x), static_cast<double>(v.y));
+        *reinterpret_cast<double2*>(qs + c + 2) = make_double2(static_cast<double>(v.z), static_cast<double>(v.w));
+      }
+      const int lines = (pl * 4 + 127) / 128;
+      for (int t = tid; t < m * lines; t += kThreads) {
+        const float* ptr = p.g + static_cast<size_t>(kc[t / lines]) * d + static_cast<size_t>(part) * pl + (t % lines) * 32;
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
+      }
+      group_sync<kThreads>();
+      for (int c = 2 * warp; c < m; c += 2 * kWarps) {
+        const float* g0 = p.g + static_cast<size_t>(kc[c]) * d + static_cast<size_t>(part) * pl;
+        double v0, v1 = 0.0;
+        if (c + 1 < m) exact_dot<2>(qs, g0, p.g + static_cast<size_t>(kc[c + 1]) * d + static_cast<size_t>(part) * pl, pl, lane, v0, v1);
+        else exact_dot<1>(qs, g0, nullptr, pl, lane, v0, v1);
+        if (lane == 0) {
+          sc[c] = fmax(sc[c], v0);
+          if (c + 1 < m) sc[c + 1] = fmax(sc[c + 1], v1);
+        }
+      }
     }
-  }
+    group_sync<kThreads>();
+  } else {
+    // every surviving row's cache lines are requested at once (L2 prefetch): the dot products below then wait for L2, not
+    // for one DRAM round trip per pair of rows
+    {
+      const int lines = (d * 4 + 127) / 128;
+      for (int t = tid; t < m * lines; t += kThreads) {
+        const float* ptr = p.g + static_cast<size_t>(kc[t / lines]) * d + (t % lines) * 32;
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
+      }
+    }
 
-  // ---- exact scores of the survivors (two rows in flight per warp), then selection by (score desc, index asc) ----
-  for (int c = 2 * warp; c < m; c += 2 * kWarps) {
-    double v0, v1 = 0.0;
-    if (c + 1 < m) exact_dot<2>(qs, p.g + static_cast<size_t>(kc[c]) * d, p.g + static_cast<size_t>(kc[c + 1]) * d, d, lane, v0, v1);
-    else exact_dot<1>(qs, p.g + static_cast<size_t>(kc[c]) * d, nullptr, d, lane, v0, v1);
-    if (lane == 0) {
-      sc[c] = v0;
-      if (c + 1 < m) sc[c + 1] = v1;
+    // ---- exact scores of the survivors (two rows in flight per warp), then selection by (score desc, index asc) ----
+    for (int c = 2 * warp; c < m; c += 2 * kWarps) {
+      double v0, v1 = 0.0;
+      if (c + 1 < m) exact_dot<2>(qs, p.g + static_cast<size_t>(kc[c]) * d, p.g + static_cast<size_t>(kc[c + 1]) * d, d, lane, v0, v1);
+      else exact_dot<1>(qs, p.g + static_cast<size_t>(kc[c]) * d, nullptr, d, lane, v0, v1);
+      if (lane == 0) {
+        sc[c] = v0;
+        if (c + 1 < m) sc[c + 1] = v1;
+      }
     }
+    group_sync<kThreads>();
   }
-  group_sync<kThreads>();
   const int km = min(k, m);
   double kth = -INFINITY;
   for (int c = tid; c < m; c += kThreads) {
@@ -772,6 +821,40 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// the same under the split score: scores[f][g] = max over the parts of exact_dot over that part (the order of
+// split_rescore_kernel), the batch's query parts staged one part at a time
+__global__ void __launch_bounds__(256)
+    split_scan_kernel(const float* __restrict__ q, const float* __restrict__ g, int ng, int d, int n_parts,
+                      const int* __restrict__ flagged, int f_begin, const int* __restrict__ n_flagged,
+                      double* __restrict__ scores, int batch) {
+  extern __shared__ __align__(16) uint8_t sm[];
+  float* qs = reinterpret_cast<float*>(sm);  // [nb][pl]
+  const int nb = min(batch, *n_flagged - f_begin);
+  if (nb <= 0) return;
+  const int pl = d / n_parts;
+  const uint32_t lane = threadIdx.x & 31;
+  const int warps = (blockDim.x >> 5) * gridDim.x;
+  for (int part = 0; part < n_parts; ++part) {
+    __syncthreads();   // the previous part's readers are done
+    for (int i = threadIdx.x; i < nb * pl; i += blockDim.x) {
+      const int f = i / pl, c = i % pl;
+      qs[i] = q[static_cast<size_t>(flagged[f_begin + f]) * d + static_cast<size_t>(part) * pl + c];
+    }
+    __syncthreads();
+    for (int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < ng; row += warps) {
+      const float* gr = g + static_cast<size_t>(row) * d + static_cast<size_t>(part) * pl;
+      for (int f = 0; f < nb; ++f) {
+        double v;
+        exact_dot<1>(qs + f * pl, gr, nullptr, pl, lane, v, v);
+        if (lane == 0) {
+          double& s = scores[static_cast<size_t>(f) * ng + row];
+          s = fmax(part == 0 ? -INFINITY : s, v);
+        }
+      }
+    }
+  }
+}
+
 __global__ void __launch_bounds__(256)
     exact_select_kernel(double* __restrict__ scores, int ng, int k, const int* __restrict__ flagged, int f_begin,
                         const int* __restrict__ n_flagged, long long g_index_base, long long g_index_stride,
@@ -817,6 +900,7 @@ struct PassPlan {
 };
 
 struct SimPlan : SweepGeometry {
+  int n_parts;   // split score: descriptor parts (plan_split_geometry); 0 = dot product
   int max_sets;  // upper bound for PassPlan::n_sets (1 or 2)
   int kp0, kp1;           // candidates kept by the first pass / by the second-chance pass (0 = no second pass)
   PassPlan p0, p1;        // p1 is sized for the worst case (every query flagged)
@@ -837,6 +921,7 @@ int plan_pass(int nq, int kp, const SimPlan& sp, int num_sms, size_t max_smem, i
   auto fits = [&](int st, int cp, int sets) { return max_smem >= smem(st, cp, sets); };
   // two epilogue warp sets whenever their lists (at least kp + 8 entries per row and set) fit next to 3 B stages
   int sets = (sp.max_sets >= 2 && fits(3, kp + 8, 2)) ? 2 : 1;
+  DCR_REQUIRE(!sp.n_parts || sets == 2, "sim_topk_split: not enough shared memory (%zu B) for two column halves", max_smem);
   int cap = kp + (sets == 2 ? 8 : 16);
   if (!fits(2, cap, sets)) cap = kp + 8;   // d = 512 with k > 10: the resident query tile leaves room for 8 spare entries
   const int cap_max = std::max(cap, 64);
@@ -907,7 +992,7 @@ struct TopkBuffers {
 
 TopkBuffers carve_topk(const SimPlan& pl, int nq, int ng, int d, Carve& w) {
   TopkBuffers b;
-  b.ops = carve_operands(w, pl.p0.nq_pad, pl, d);
+  b.ops = pl.n_parts ? carve_split_operands(w, pl.p0.nq_pad, pl, pl.n_parts) : carve_operands(w, pl.p0.nq_pad, pl, d);
   b.qb1 = w.take<__nv_bfloat16>(pl.kp1 ? static_cast<size_t>(pl.p1.nq_pad) * pl.d_pad : 0);
   const size_t slot_rows = static_cast<size_t>(std::max(pl.p0.n_slots, pl.kp1 ? pl.p1.n_slots : 0)) * pl.rows_per_qtile;   // n_slots counts sets
   b.pb.cand = w.take<uint2>(slot_rows * kKPMax);
@@ -923,16 +1008,30 @@ TopkBuffers carve_topk(const SimPlan& pl, int nq, int ng, int d, Carve& w) {
   return b;
 }
 
-int make_plan(int nq, int ng, int d, int k, int num_sms, size_t max_smem, SimPlan* pl) {
-  DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "sim_topk: empty problem (nq=%d ng=%d d=%d)", nq, ng, d);
-  DCR_REQUIRE(d <= kMaxDim, "sim_topk: descriptor dim %d > %d not supported", d, kMaxDim);
-  DCR_REQUIRE(k >= 1 && k <= 16, "sim_topk: k=%d outside [1,16]", k);
-  DCR_REQUIRE(k <= ng, "sim_topk: k=%d > gallery size %d", k, ng);
-  plan_geometry(ng, d, pl);
+// n_parts = 0: the dot product; >= 1: the split score over n_parts parts (sim_topk_split)
+int make_plan(int nq, int ng, int d, int k, int n_parts, int num_sms, size_t max_smem, SimPlan* pl) {
+  const char* who = n_parts ? "sim_topk_split" : "sim_topk";
+  DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "%s: empty problem (nq=%d ng=%d d=%d)", who, nq, ng, d);
+  if (n_parts) {
+    DCR_REQUIRE(n_parts >= 1 && d % n_parts == 0 && (d / n_parts) % 4 == 0,
+                "sim_topk_split: d=%d must split into %d parts whose length is a multiple of 4", d, n_parts);
+    const int p = d / n_parts;
+    DCR_REQUIRE(p <= kMaxDim, "sim_topk_split: part length %d > %d not supported", p, kMaxDim);
+    DCR_REQUIRE(static_cast<long long>(n_parts) * ((p + kBlockK - 1) / kBlockK * kBlockK) <= (1ll << 30),
+                "sim_topk_split: %d parts of %d padded to 64 exceed 2^30 columns", n_parts, p);
+  } else {
+    DCR_REQUIRE(d <= kMaxDim, "sim_topk: descriptor dim %d > %d not supported", d, kMaxDim);
+  }
+  DCR_REQUIRE(k >= 1 && k <= 16, "%s: k=%d outside [1,16]", who, k);
+  DCR_REQUIRE(k <= ng, "%s: k=%d > gallery size %d", who, k, ng);
+  pl->n_parts = n_parts;
+  if (n_parts) plan_split_geometry(ng, n_parts, d / n_parts, pl);
+  else plan_geometry(ng, d, pl);
   // Two consumer warpgroups (two warps per 32-row block, each with its own lists for one column half) when few
   // candidates are kept (k <= 2: each segment keeps 2 x 4 candidates); with larger k the lists of two sets only fit with
-  // a small capacity.
-  pl->max_sets = k <= 2 ? 2 : 1;
+  // a small capacity.  The split score always runs on column halves: the running maximum of a 128-column tile next to its
+  // part accumulator would not fit a thread's registers.
+  pl->max_sets = (k <= 2 || n_parts) ? 2 : 1;
   // first pass keeps few candidates per (query, segment) -- enough unless many gallery rows sit within the error
   // bound of the k-th score; such queries get a second chance with 32 candidates before the brute-force path
   // k in 6..10 keeps 12 (two spare candidates per segment keep the second-chance pass rare)
@@ -967,53 +1066,42 @@ int launch_fused(const SimPlan& pl, const PassPlan& pp, const __nv_bfloat16* qb,
   p.thr_init = thr_init;
   p.clk = clk;
   p.gthr = gthr;
+  p.kb_part = pl.n_parts ? pl.num_kb / pl.n_parts : 0;
   DCR_CUDA_CHECK(cudaMemsetAsync(gthr, 0, static_cast<size_t>(pp.nq_pad) * 4, stream));
+  if (pl.n_parts)
+    return launch(sim_topk_kernel<false, 2, true>, pp.n_units, 32 + 128 * 2, pp.smem_bytes, stream, "sim_topk_split", tq, tg, p);
   const bool two = pp.n_sets == 2;
   return launch_sweep(two ? sim_topk_kernel<false, 2> : sim_topk_kernel<false, 1>,
                       two ? sim_topk_kernel<true, 2> : sim_topk_kernel<true, 1>, pp.n_units, 32 + 128 * pp.n_sets,
                       pp.smem_bytes, stream, "sim_topk", tq, tg, p);
 }
 
-}  // namespace
-
-int split_rescore(const float* q, const float* g, int nq, int d, int n_chunks, int cross, const long long* cand, int n_cand,
-                  int k, float* out_scores, long long* out_idx, cudaStream_t stream) {
-  DCR_REQUIRE(nq >= 1 && d >= 1 && n_chunks >= 1 && d % n_chunks == 0 && (d / n_chunks) % 4 == 0,
-              "split_rescore: d=%d must split into %d parts whose length is a multiple of 4", d, n_chunks);
-  DCR_REQUIRE(n_cand >= k && k >= 1 && n_cand <= 4096, "split_rescore: need k <= n_cand <= 4096 (k=%d n_cand=%d)", k, n_cand);
-  DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0,
-              "split_rescore: q/g must be 16-byte aligned");
-  const size_t smem = ((static_cast<size_t>(d / n_chunks) * 4 + 15) & ~size_t(15)) + static_cast<size_t>(n_cand) * 16;
-  return launch(split_rescore_kernel, nq, 128, smem, stream, "split_rescore", q, g, d, n_chunks, cross, cand, n_cand, k,
-                out_scores, out_idx);
-}
-
-size_t sim_topk_workspace_size(int nq, int ng, int d, int k) {
-  const DeviceInfo* di = device_info();
-  SimPlan pl;
-  if (make_plan(nq, ng, d, k, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &pl) != 0)
-    return 0;
-  return pl.total;
-}
-
-int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long long g_index_base,
-             long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
-             cudaStream_t stream, SimStats* stats) {
+// The whole search: stage 1, the fused pass, the exact re-score, the second-chance pass and the brute-force path.
+// n_parts = 0: the dot product (sim_topk); >= 1: the split score over n_parts parts (sim_topk_split).
+int topk_search(const float* q, int nq, const float* g, int ng, int d, int n_parts, int k, long long g_index_base,
+                long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
+                cudaStream_t stream, SimStats* stats) {
+  const char* who = n_parts ? "sim_topk_split" : "sim_topk";
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  if (int rc = require_sm90a(di, "sim_topk")) return rc;
+  if (int rc = require_sm90a(di, who)) return rc;
   SimPlan pl;
-  if (int rc = make_plan(nq, ng, d, k, di->num_sms, di->max_smem_optin, &pl)) return rc;
-  DCR_REQUIRE(ws != nullptr && ws_bytes >= pl.total, "sim_topk: workspace too small (%zu < %zu)", ws_bytes, pl.total);
-  DCR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "sim_topk: workspace must be 256-byte aligned");
+  if (int rc = make_plan(nq, ng, d, k, n_parts, di->num_sms, di->max_smem_optin, &pl)) return rc;
+  DCR_REQUIRE(ws != nullptr && ws_bytes >= pl.total, "%s: workspace too small (%zu < %zu)", who, ws_bytes, pl.total);
+  DCR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "%s: workspace must be 256-byte aligned", who);
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0 && d % 4 == 0,
-              "sim_topk: q/g must be 16-byte aligned with d %% 4 == 0 (d=%d)", d);
+              "%s: q/g must be 16-byte aligned with d %% 4 == 0 (d=%d)", who, d);
   Carve w{static_cast<uint8_t*>(ws)};
   TopkBuffers b = carve_topk(pl, nq, ng, d, w);
   DCR_CUDA_CHECK(cudaMemsetAsync(b.counts, 0, 16, stream));
-  b.ops.qflag = b.counts + 2;
+  const int pl_len = n_parts ? d / n_parts : d;   // the length of one exact dot product (a part, or the whole row)
+  if (n_parts) {
+    if (int rc = prepare_split_operands(q, nq, pl.p0.nq_pad, g, ng, n_parts, pl_len, pl, di, b.ops, stream)) return rc;
+  } else {
+    b.ops.qflag = b.counts + 2;
+    if (int rc = prepare_operands(q, nq, pl.p0.nq_pad, g, ng, d, pl, di, b.ops, stream)) return rc;
+  }
   const Operands& o = b.ops;
-  if (int rc = prepare_operands(q, nq, pl.p0.nq_pad, g, ng, d, pl, di, o, stream)) return rc;
 
   // CUDA events around the first fused pass only (thread-local, created once): bench.py's roofline numerator
   // (events belong to the device that was current when they were created: one pair per device)
@@ -1037,16 +1125,17 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     rp.mu = o.mu, rp.nu = o.nu, rp.nu_flag = o.qflag;
     rp.q_norm_hat = o.qnh, rp.q_norm_res = o.qnr, rp.q_norm_x = o.qnx, rp.g_max = o.gmax;
     rp.g_index_base = g_index_base, rp.g_index_stride = g_index_stride, rp.out_scores = out_scores, rp.out_idx = out_idx;
-    rp.flagged = flagged, rp.n_flagged = n_flagged, rp.thr_next = thr_next;
+    rp.flagged = flagged, rp.n_flagged = n_flagged, rp.thr_next = thr_next, rp.n_parts = n_parts;
     // one warp per query when a q-tile's candidate slots fit a lane each and four queries' rows fit a block's shared memory
     // (the block-wide form spends its time on barriers for such small candidate sets)
-    const size_t per_query = RescoreSmem(d, pp.max_cand).bytes;
+    const size_t per_query = RescoreSmem(pl_len, pp.max_cand).bytes;
     const bool warp_form = pp.kp > 0 && pp.max_cand / pp.kp <= 32 && pp.n_chunks <= 32 && 4 * per_query <= 56 * 1024 &&
                            !tuning_flag("DCR_SIM_RESCORE_BLOCK");
     const int per_block = warp_form ? kRescoreThreads / 32 : 1;
     const size_t smem = per_block * per_query;
-    auto kern = warp_form ? rescore_select_kernel<32> : rescore_select_kernel<kRescoreThreads>;
-    return launch(kern, (pp.nq + per_block - 1) / per_block, kRescoreThreads, smem, stream, "sim_topk", rp);
+    auto kern = n_parts ? (warp_form ? rescore_select_kernel<32, true> : rescore_select_kernel<kRescoreThreads, true>)
+                        : (warp_form ? rescore_select_kernel<32> : rescore_select_kernel<kRescoreThreads>);
+    return launch(kern, (pp.nq + per_block - 1) / per_block, kRescoreThreads, smem, stream, who, rp);
   };
   if (int rc = rescore(pl.p0, nullptr, b.flag0, b.counts + 0, b.thr1)) return rc;
 
@@ -1064,7 +1153,7 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     PassPlan p1;
     if (int rc = plan_pass(n_second, pl.kp1, pl, di->num_sms, di->max_smem_optin, d, k, &p1)) return rc;
     if (int rc = launch(gather_rows_kernel, std::min(di->num_sms * 8, (p1.nq_pad * (pl.d_pad / 8) + 255) / 256), 256, 0,
-                        stream, "sim_topk", o.qb, b.flag0, n_second, p1.nq_pad, pl.d_pad, b.qb1))
+                        stream, who, o.qb, b.flag0, n_second, p1.nq_pad, pl.d_pad, b.qb1))
       return rc;
     if (int rc = launch_fused(pl, p1, b.qb1, o.gb, ng, b.pb, o.bias, o.qflag, b.thr1, nullptr, b.gthr, stream)) return rc;
     if (int rc = rescore(p1, b.flag0, b.flag1, b.counts + 1, nullptr)) return rc;
@@ -1076,15 +1165,18 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
 
   // brute-force fp64 path for the queries whose certificate still fails (ties beyond 32 candidates, NaNs, ...)
   if (n_exact > 0) {
-    // queries per brute-force launch: as many as fit in shared memory next to each other (32 up to d = 1536)
-    const int ex_batch = std::max(1, std::min<int>(kExactBatch, static_cast<int>(192 * 1024 / (static_cast<size_t>(d) * 4))));
-    const size_t ex_smem = static_cast<size_t>(ex_batch) * d * 4;
+    // queries per brute-force launch: as many as fit in shared memory next to each other (32 up to d = 1536; under the
+    // split score the rows are staged one part at a time)
+    const int ex_batch = std::max(1, std::min<int>(kExactBatch, static_cast<int>(192 * 1024 / (static_cast<size_t>(pl_len) * 4))));
+    const size_t ex_smem = static_cast<size_t>(ex_batch) * pl_len * 4;
     const int* n_dev = (exact_list == b.flag0) ? b.counts + 0 : b.counts + 1;
     for (int done = 0; done < n_exact; done += ex_batch) {
-      if (int rc = launch(exact_scan_kernel, di->num_sms * 2, 256, ex_smem, stream, "sim_topk", q, g, ng, d, exact_list, done,
-                          n_dev, b.exact, ex_batch))
-        return rc;
-      if (int rc = launch(exact_select_kernel, ex_batch, 256, 0, stream, "sim_topk", b.exact, ng, k, exact_list, done, n_dev,
+      const int rc = n_parts ? launch(split_scan_kernel, di->num_sms * 2, 256, ex_smem, stream, who, q, g, ng, d, n_parts,
+                                      exact_list, done, n_dev, b.exact, ex_batch)
+                             : launch(exact_scan_kernel, di->num_sms * 2, 256, ex_smem, stream, who, q, g, ng, d, exact_list,
+                                      done, n_dev, b.exact, ex_batch);
+      if (rc) return rc;
+      if (int rc = launch(exact_select_kernel, ex_batch, 256, 0, stream, who, b.exact, ng, k, exact_list, done, n_dev,
                           g_index_base, g_index_stride, out_scores, out_idx))
         return rc;
     }
@@ -1110,6 +1202,56 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
     stats->d_pad = pl.d_pad;
   }
   return 0;
+}
+
+}  // namespace
+
+int split_rescore(const float* q, const float* g, int nq, int d, int n_chunks, int cross, const long long* cand, int n_cand,
+                  int k, float* out_scores, long long* out_idx, cudaStream_t stream) {
+  DCR_REQUIRE(nq >= 1 && d >= 1 && n_chunks >= 1 && d % n_chunks == 0 && (d / n_chunks) % 4 == 0,
+              "split_rescore: d=%d must split into %d parts whose length is a multiple of 4", d, n_chunks);
+  DCR_REQUIRE(n_cand >= k && k >= 1 && n_cand <= 4096, "split_rescore: need k <= n_cand <= 4096 (k=%d n_cand=%d)", k, n_cand);
+  DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0,
+              "split_rescore: q/g must be 16-byte aligned");
+  const size_t smem = ((static_cast<size_t>(d / n_chunks) * 4 + 15) & ~size_t(15)) + static_cast<size_t>(n_cand) * 16;
+  return launch(split_rescore_kernel, nq, 128, smem, stream, "split_rescore", q, g, d, n_chunks, cross, cand, n_cand, k,
+                out_scores, out_idx);
+}
+
+namespace {
+size_t workspace_size(int nq, int ng, int d, int n_parts, int k) {
+  const DeviceInfo* di = device_info();
+  SimPlan pl;
+  if (make_plan(nq, ng, d, k, n_parts, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &pl) != 0)
+    return 0;
+  return pl.total;
+}
+}  // namespace
+
+size_t sim_topk_workspace_size(int nq, int ng, int d, int k) { return workspace_size(nq, ng, d, 0, k); }
+
+int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long long g_index_base,
+             long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
+             cudaStream_t stream, SimStats* stats) {
+  return topk_search(q, nq, g, ng, d, 0, k, g_index_base, g_index_stride, out_scores, out_idx, ws, ws_bytes, stream, stats);
+}
+
+// one part is the dot product itself: the dot-product search, whose bits the split score must reproduce
+size_t sim_topk_split_workspace_size(int nq, int ng, int d, int n_parts, int k) {
+  if (n_parts == 1) return workspace_size(nq, ng, d, 0, k);
+  if (n_parts < 1) {
+    set_error(-1, "sim_topk_split: n_parts=%d < 1", n_parts);
+    return 0;
+  }
+  return workspace_size(nq, ng, d, n_parts, k);
+}
+
+int sim_topk_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, int k, long long g_index_base,
+                   long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
+                   cudaStream_t stream, SimStats* stats) {
+  DCR_REQUIRE(n_parts >= 1, "sim_topk_split: n_parts=%d < 1", n_parts);
+  return topk_search(q, nq, g, ng, d, n_parts == 1 ? 0 : n_parts, k, g_index_base, g_index_stride, out_scores, out_idx, ws,
+                     ws_bytes, stream, stats);
 }
 
 }  // namespace dcr

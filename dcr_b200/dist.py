@@ -103,6 +103,14 @@ def cuda_local_topk(q, g, k, index_base):
     return sim_topk(q, g, k, index_base=index_base)
 
 
+def split_local_topk(num_chunks: int, cross: bool = False) -> Callable:
+    """local_topk of sharded_topk under the 'splitloss' similarity (similarity.sim_topk_split, aligned or cross parts)."""
+    def local(q, g, k, index_base):
+        from .similarity import sim_topk_split
+        return sim_topk_split(q, g, k, num_chunks, cross=cross, index_base=index_base)
+    return local
+
+
 def cuda_merge(scores, idx, k):
     from .similarity import topk_merge
     return topk_merge(scores, idx, k)

@@ -132,42 +132,44 @@ def sim_range(query: torch.Tensor, gallery: torch.Tensor, threshold: float, *, i
     return offsets, out_i, out_s
 
 
-def sim_topk_split(q: torch.Tensor, g: torch.Tensor, k: int, num_chunks: int, cross: bool = False
-                   ) -> Tuple[torch.Tensor, torch.Tensor]:
+def sim_topk_split(q: torch.Tensor, g: torch.Tensor, k: int, num_chunks: int, cross: bool = False, *,
+                   index_base: int = 0, index_stride: int = 1) -> Tuple[torch.Tensor, torch.Tensor]:
     """Top-k under the 'splitloss' similarity of diff_retrieval.py:393-400 (--similarity_metric splitloss,
     --num_loss_chunks C): score(q, g) = max_c <q_c, g_c> over the C equal parts of the descriptors.
-    One fused similarity+top-k pass per part (the true top-k is contained in the union of the per-part top-k lists),
-    then dcr_split_rescore evaluates the exact split score of the <= C*k candidates per query and selects.
+    One fused tensor-core sweep whose epilogue sees the maximum over the parts, then the exact split score of the
+    candidates (dcr_sim_topk_split): any number of parts, part length p = D/C a multiple of 4 and at most 8192.
+    Reported gallery indices are index_base + index_stride * row (a rank's gallery shard).
     cross=True is `--stype cross` (einsum_in_chunks :643-662): score = max over every (gallery part, query part) pair.
     Candidates then come from ONE fused pass over the part matrices [Q*C, D/C] x [G*C, D/C] with
     k' = (k-1)*C + 1 rows per query part (fewer than k' part-rows can beat the best part-row of a true top-k gallery row)
     while k' <= 16, otherwise from one pass per gallery part with k' = k (no limit on the number of parts)."""
     lib = _lib.load()
-    if num_chunks == 1:
-        return sim_topk(q, g, k)
-    if cross:
-        return _sim_topk_cross(lib, q, g, k, num_chunks)
-    if not (q.is_cuda and g.is_cuda):
+    if cross and num_chunks > 1:
+        s, i = _sim_topk_cross(lib, q, g, k, num_chunks)
+        if index_base != 0 or index_stride != 1:
+            i = torch.where(i >= 0, index_base + index_stride * i, i)
+        return s, i
+    if not (isinstance(q, torch.Tensor) and isinstance(g, torch.Tensor) and q.is_cuda and g.is_cuda):
         raise _lib.DcrError("sim_topk_split needs CUDA tensors")
-    q = q.contiguous().float()
-    g = g.contiguous().float()
+    q = _check_cuda_f32("query", q.contiguous().float())
+    g = _check_cuda_f32("gallery", g.contiguous().float())
+    if q.device != g.device:
+        raise _lib.DcrError("query and gallery must be on the same device")
+    if q.shape[1] != g.shape[1]:
+        raise _lib.DcrError(f"descriptor dims differ: {q.shape[1]} vs {g.shape[1]}")
     nq, d = q.shape
-    if d % num_chunks or (d // num_chunks) % 4:
-        raise _lib.DcrError(f"splitloss: descriptor dim {d} must split into {num_chunks} parts of a multiple of 4 dims")
-    if num_chunks * k > 4096:
-        raise _lib.DcrError("splitloss: num_chunks * k must be <= 4096")
-    p = d // num_chunks
-    cand = torch.empty((nq, num_chunks * k), dtype=torch.int64, device=q.device)
-    for c in range(num_chunks):
-        _, idx = sim_topk(q[:, c * p:(c + 1) * p].contiguous(), g[:, c * p:(c + 1) * p].contiguous(), k)
-        cand[:, c * k:(c + 1) * k] = idx
-    out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
-    out_i = torch.empty((nq, k), dtype=torch.int64, device=q.device)
+    ng = g.shape[0]
     with torch.cuda.device(q.device):
+        nbytes = lib.dcr_sim_topk_split_workspace_size(nq, ng, d, num_chunks, k)
+        if nbytes == 0:
+            raise _lib.DcrError(f"dcr_sim_topk_split_workspace_size: {_lib.last_error()}")
+        ws = _workspace(nbytes, q.device)
+        out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
+        out_i = torch.empty((nq, k), dtype=torch.int64, device=q.device)
         st = torch.cuda.current_stream().cuda_stream
-        rc = lib.dcr_split_rescore(q.data_ptr(), g.data_ptr(), nq, d, num_chunks, 0, cand.data_ptr(), num_chunks * k, k,
-                                   out_s.data_ptr(), out_i.data_ptr(), st)
-        _lib.check(rc, "dcr_split_rescore")
+        rc = lib.dcr_sim_topk_split(q.data_ptr(), nq, g.data_ptr(), ng, d, num_chunks, k, index_base, index_stride,
+                                    out_s.data_ptr(), out_i.data_ptr(), _aligned_ptr(ws), nbytes, st)
+        _lib.check(rc, "dcr_sim_topk_split")
     return out_s, out_i
 
 

@@ -104,7 +104,21 @@ int dcr_sim_topk_sharded(const float* q, int nq, const float* g, int ng_local, i
                          int64_t g_index_stride, int world, dcr_allgather_fn allgather, void* allgather_ctx,
                          float* out_scores, int64_t* out_idx, void* workspace, size_t workspace_bytes, void* stream);
 
-/* Final step of the 'splitloss' similarity (diff_retrieval.py:393-400: descriptors cut into n_chunks equal parts, pair
+/* Top-k under the 'splitloss' similarity (diff_retrieval.py:393-400): the descriptors are cut into n_parts equal parts of
+ * p = d / n_parts values and a pair scores max over c of <q_c, g_c>.  One fused tensor-core sweep whose epilogue sees the
+ * maximum over the parts, then the exact re-score: score = max over the parts of the fp64-accumulated part dot products,
+ * bit for bit what dcr_split_rescore reports for the same pair (fmax: a NaN part is ignored).  Ranked on the fp64 value,
+ * reported as fp32, ordered by (score desc, gallery index asc); indices as dcr_sim_topk (g_index_base / _stride).
+ * q[nq,d], g[ng,d]: device, fp32, 16-byte aligned; d % n_parts == 0, p % 4 == 0, p <= 8192 (no limit on d or n_parts);
+ * 1 <= k <= 16, k <= ng.  n_parts = 1 returns the bits of dcr_sim_topk.  The workspace grows with (nq + ng) * d, never with
+ * nq * ng; dcr_sim_topk_last_stats and friends describe the call afterwards. */
+size_t dcr_sim_topk_split_workspace_size(int nq, int ng, int d, int n_parts, int k);
+int dcr_sim_topk_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, int k, int64_t g_index_base,
+                       int64_t g_index_stride, float* out_scores, int64_t* out_idx, void* workspace,
+                       size_t workspace_bytes, void* stream);
+
+/* Final step of the 'splitloss' similarity in its 'cross' form, and of the per-part composition the aligned form used
+ * before dcr_sim_topk_split (descriptors cut into n_chunks equal parts, pair
  * score = max over the parts of the per-part dot products).  The caller runs dcr_sim_topk once per part and passes
  * the union of the per-part top-k rows as cand [nq][n_cand] (duplicates allowed); this evaluates the exact split
  * score of every candidate (float64 accumulation, reported as fp32) and writes the k best per query ordered by
