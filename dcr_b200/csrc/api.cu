@@ -97,66 +97,16 @@ int dcr_sim_topk_host(const float* q, int nq, const float* g, int ng, int d, int
   return rc;
 }
 
-namespace {
-inline size_t up256(size_t x) { return (x + 255) / 256 * 256; }
-}  // namespace
-
 size_t dcr_sim_topk_sharded_workspace_size(int nq, int ng_local, int d, int k, int world) {
-  if (world < 1 || k < 1 || nq < 1) return 0;
-  const int kk = k < ng_local ? k : ng_local;
-  const size_t inner = dcr::sim_topk_workspace_size(nq, ng_local, d, kk < 1 ? 1 : kk);
-  if (inner == 0) return 0;
-  const size_t list = static_cast<size_t>(nq) * k;
-  // local scores + indices, gathered scores + indices (each rank's block: [scores f32 | indices i64])
-  return up256(inner) + up256(list * 12) + up256(list * 12 * world) + up256(list * 4 * world) + up256(list * 8 * world);
+  return dcr::sim_topk_sharded_workspace_size(nq, ng_local, d, k, world);
 }
 
 int dcr_sim_topk_sharded(const float* q, int nq, const float* g, int ng_local, int d, int k, int64_t g_index_base,
                          int64_t g_index_stride, int world, dcr_allgather_fn allgather, void* allgather_ctx,
                          float* out_scores, int64_t* out_idx, void* workspace, size_t workspace_bytes, void* stream) {
-  DCR_REQUIRE(q && g && out_scores && out_idx && workspace, "dcr_sim_topk_sharded: null pointer argument");
-  DCR_REQUIRE(world >= 1 && (world == 1 || allgather != nullptr), "dcr_sim_topk_sharded: world=%d needs an all-gather callback", world);
-  DCR_REQUIRE(static_cast<long long>(world) * k <= 1024, "dcr_sim_topk_sharded: world * k = %d > 1024", world * k);
-  const size_t need = dcr_sim_topk_sharded_workspace_size(nq, ng_local, d, k, world);
-  DCR_REQUIRE(need != 0 && workspace_bytes >= need, "dcr_sim_topk_sharded: workspace too small (%zu < %zu)", workspace_bytes, need);
-  DCR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "dcr_sim_topk_sharded: workspace must be 256-byte aligned");
-  cudaStream_t st = as_stream(stream);
-  const int kk = k < ng_local ? k : ng_local;       // a shard smaller than k contributes empty (-inf, -1) entries
-  const size_t list = static_cast<size_t>(nq) * k;
-  uint8_t* w = static_cast<uint8_t*>(workspace);
-  const size_t inner = dcr::sim_topk_workspace_size(nq, ng_local, d, kk);
-  uint8_t* send = w + up256(inner);                                  // [scores f32 [nq,k] | indices i64 [nq,k]]
-  uint8_t* recv = send + up256(list * 12);                           // world x the same block
-  float* all_s = reinterpret_cast<float*>(recv + up256(list * 12 * world));        // [world][nq][k]
-  long long* all_i = reinterpret_cast<long long*>(reinterpret_cast<uint8_t*>(all_s) + up256(list * 4 * world));
-  float* loc_s = reinterpret_cast<float*>(send);
-  long long* loc_i = reinterpret_cast<long long*>(send + list * 4);
-  if (kk == k) {
-    if (int rc = dcr::sim_topk(q, nq, g, ng_local, d, k, g_index_base, g_index_stride, loc_s, loc_i, w, inner, st, &g_last_stats))
-      return rc;
-  } else {
-    // fewer gallery rows than k on this rank: top-kk into a compact list, spread into the k-wide slots, the rest empty
-    float* tmp_s = all_s;                      // scratch (not yet in use)
-    long long* tmp_i = all_i;
-    if (int rc = dcr::sim_topk(q, nq, g, ng_local, d, kk, g_index_base, g_index_stride, tmp_s, tmp_i, w, inner, st, &g_last_stats))
-      return rc;
-    if (int rc = dcr::pad_topk_lists(tmp_s, tmp_i, nq, kk, k, loc_s, loc_i, st)) return rc;
-  }
-  if (world == 1) {
-    DCR_CUDA_CHECK(cudaMemcpyAsync(out_scores, loc_s, list * 4, cudaMemcpyDeviceToDevice, st));
-    DCR_CUDA_CHECK(cudaMemcpyAsync(out_idx, loc_i, list * 8, cudaMemcpyDeviceToDevice, st));
-    return 0;
-  }
-  const int arc = allgather(send, recv, list * 12, allgather_ctx, stream);
-  DCR_REQUIRE(arc == 0, "dcr_sim_topk_sharded: the all-gather callback failed (%d)", arc);
-  // un-interleave the gathered blocks into [world][nq][k] score and index arrays, then merge
-  for (int r = 0; r < world; ++r) {
-    DCR_CUDA_CHECK(cudaMemcpyAsync(all_s + static_cast<size_t>(r) * list, recv + static_cast<size_t>(r) * list * 12, list * 4,
-                                   cudaMemcpyDeviceToDevice, st));
-    DCR_CUDA_CHECK(cudaMemcpyAsync(all_i + static_cast<size_t>(r) * list, recv + static_cast<size_t>(r) * list * 12 + list * 4, list * 8,
-                                   cudaMemcpyDeviceToDevice, st));
-  }
-  return dcr::topk_merge(all_s, all_i, nq, world, k, k, out_scores, reinterpret_cast<long long*>(out_idx), st);
+  return dcr::sim_topk_sharded(q, nq, g, ng_local, d, k, g_index_base, g_index_stride, world, allgather, allgather_ctx,
+                               out_scores, reinterpret_cast<long long*>(out_idx), workspace, workspace_bytes,
+                               as_stream(stream), &g_last_stats);
 }
 
 size_t dcr_sim_range_workspace_size(int nq, int ng, int d, int64_t max_pairs) {

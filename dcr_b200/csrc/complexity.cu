@@ -512,8 +512,6 @@ __global__ void __launch_bounds__(kStatsThreads)
   }
 }
 
-inline size_t up256(size_t x) { return (x + 255) / 256 * 256; }
-
 int check_jpeg_size(const char* what, int h, int w) {
   DCR_REQUIRE(h >= 16 && w >= 16 && h <= 4096 && w <= 4096 && h % 16 == 0 && w % 16 == 0,
               "%s: %d x %d images: height and width must be multiples of 16 in 16..4096 (the edge replication libjpeg "
@@ -521,22 +519,28 @@ int check_jpeg_size(const char* what, int h, int w) {
   return 0;
 }
 
+// The workspace.  With a null base only nb, words_per_image and bytes are meaningful.
 struct JpegLayout {
   int nb;                    // blocks per image
   size_t words_per_image;    // bit-buffer words per image
-  size_t dc_off, bits_off, total_off, header_off, buf_off, bytes;
+  short* dc;
+  unsigned *bits, *total, *buf;
+  unsigned char* header;
+  size_t bytes;
 };
 
-JpegLayout jpeg_layout(int n, int h, int w) {
+JpegLayout jpeg_layout(int n, int h, int w, void* base = nullptr) {
   JpegLayout l;
   l.nb = 6 * (h / 16) * (w / 16);
   l.words_per_image = (static_cast<size_t>(l.nb) * kMaxBlockBits + 31) / 32;
-  l.dc_off = 0;
-  l.bits_off = l.dc_off + up256(sizeof(short) * static_cast<size_t>(n) * l.nb);
-  l.total_off = l.bits_off + up256(sizeof(unsigned) * static_cast<size_t>(n) * l.nb);
-  l.header_off = l.total_off + up256(sizeof(unsigned) * static_cast<size_t>(n));
-  l.buf_off = l.header_off + up256(kJpegHeaderBytes);
-  l.bytes = l.buf_off + sizeof(unsigned) * l.words_per_image * static_cast<size_t>(n);
+  Carve c{static_cast<uint8_t*>(base)};
+  l.dc = c.take<short>(static_cast<size_t>(n) * l.nb);
+  l.bits = c.take<unsigned>(static_cast<size_t>(n) * l.nb);
+  l.total = c.take<unsigned>(n);
+  l.header = c.take<unsigned char>(kJpegHeaderBytes);
+  // the bit buffer comes last and is not rounded up: take(0) only places it
+  l.buf = c.take<unsigned>(0);
+  l.bytes = c.bytes + sizeof(unsigned) * l.words_per_image * static_cast<size_t>(n);
   return l;
 }
 
@@ -550,10 +554,7 @@ int image_stats(const unsigned char* images, int n, int h, int w, double* out_en
   if (n == 0) return 0;
   DCR_REQUIRE(images && out_entropy && out_tv, "dcr_image_stats: null pointer argument");
   if (!device_info()) return -2;
-  image_stats_kernel<<<n, kStatsThreads, 0, stream>>>(images, h, w, out_entropy, out_tv);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(image_stats_kernel, n, kStatsThreads, 0, stream, "dcr_image_stats", images, h, w, out_entropy, out_tv);
 }
 
 size_t jpeg_workspace_size(int n, int h, int w) {
@@ -579,32 +580,27 @@ int jpeg_encode(const unsigned char* images, int n, int h, int w, int quality, l
   DCR_REQUIRE(quality >= 1 && quality <= 100, "dcr_jpeg_encode: quality %d outside 1..100", quality);
   if (n == 0) return 0;
   DCR_REQUIRE(images && out_sizes && workspace, "dcr_jpeg_encode: null pointer argument");
-  const JpegLayout l = jpeg_layout(n, h, w);
+  const JpegLayout l = jpeg_layout(n, h, w, workspace);
   DCR_REQUIRE(workspace_bytes >= l.bytes, "dcr_jpeg_encode: workspace too small (%zu < %zu)", workspace_bytes, l.bytes);
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "dcr_jpeg_encode: workspace must be 256-byte aligned");
   if (!device_info()) return -2;
   const JpegTables t = make_tables(quality);
   const std::vector<unsigned char> header = make_header(h, w, quality);
   DCR_REQUIRE(header.size() == kJpegHeaderBytes, "dcr_jpeg_encode: internal header size %zu", header.size());
-  unsigned char* ws = static_cast<unsigned char*>(workspace);
-  short* dc = reinterpret_cast<short*>(ws + l.dc_off);
-  unsigned* bits = reinterpret_cast<unsigned*>(ws + l.bits_off);
-  unsigned* total = reinterpret_cast<unsigned*>(ws + l.total_off);
-  unsigned char* hdr = ws + l.header_off;
-  unsigned* buf = reinterpret_cast<unsigned*>(ws + l.buf_off);
   // pageable source: staged before the call returns, so `header` may go out of scope
-  DCR_CUDA_CHECK(cudaMemcpyAsync(hdr, header.data(), kJpegHeaderBytes, cudaMemcpyHostToDevice, stream));
-  DCR_CUDA_CHECK(cudaMemsetAsync(buf, 0, sizeof(unsigned) * l.words_per_image * static_cast<size_t>(n), stream));
+  DCR_CUDA_CHECK(cudaMemcpyAsync(l.header, header.data(), kJpegHeaderBytes, cudaMemcpyHostToDevice, stream));
+  DCR_CUDA_CHECK(cudaMemsetAsync(l.buf, 0, sizeof(unsigned) * l.words_per_image * static_cast<size_t>(n), stream));
   const long long blocks = static_cast<long long>(n) * l.nb;
   const unsigned grid = static_cast<unsigned>((blocks + kBlockThreads - 1) / kBlockThreads);
-  jpeg_block_kernel<<<grid, kBlockThreads, 0, stream>>>(images, n, h, w, t, dc, bits);
-  jpeg_scan_kernel<<<n, kScanThreads, 0, stream>>>(l.nb, t, dc, bits, total);
-  jpeg_emit_kernel<<<grid, kBlockThreads, 0, stream>>>(images, n, h, w, t, dc, bits, buf, l.words_per_image);
-  jpeg_finish_kernel<<<n, kFinishThreads, 0, stream>>>(buf, l.words_per_image, total, hdr, out_sizes, out_bytes,
-                                                       out_bytes ? jpeg_max_bytes(h, w) : 0);
-  count_launch(4);
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  if (int rc = launch(jpeg_block_kernel, grid, kBlockThreads, 0, stream, "dcr_jpeg_encode", images, n, h, w, t, l.dc, l.bits))
+    return rc;
+  if (int rc = launch(jpeg_scan_kernel, n, kScanThreads, 0, stream, "dcr_jpeg_encode", l.nb, t, l.dc, l.bits, l.total))
+    return rc;
+  if (int rc = launch(jpeg_emit_kernel, grid, kBlockThreads, 0, stream, "dcr_jpeg_encode", images, n, h, w, t, l.dc, l.bits,
+                      l.buf, l.words_per_image))
+    return rc;
+  return launch(jpeg_finish_kernel, n, kFinishThreads, 0, stream, "dcr_jpeg_encode", l.buf, l.words_per_image, l.total,
+                l.header, out_sizes, out_bytes, out_bytes ? jpeg_max_bytes(h, w) : 0);
 }
 
 }  // namespace dcr

@@ -214,10 +214,7 @@ int conv_exact(const ConvGemmDesc& d, cudaStream_t stream) {
   p.ld_out_f32 = d.ld_out_f32;
   p.act = d.act;
   const dim3 grid(static_cast<unsigned>((p.M + kTM - 1) / kTM), static_cast<unsigned>((d.N + kTN - 1) / kTN));
-  conv_exact_kernel<<<grid, kThreadsExact, 0, stream>>>(p);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(conv_exact_kernel, grid, kThreadsExact, 0, stream, "conv_exact", p);
 }
 
 }  // namespace dcr

@@ -41,8 +41,12 @@ int sim_range(const float* q, int nq, const float* g, int ng, int d, float thres
 // out[0..n] = exclusive prefix sums of in[0..n-1], out[n] = total: one block, a fixed association (sim_range's row scan)
 int exclusive_scan_i64(const long long* in, long long n, long long* out, cudaStream_t stream);
 
-// gallery-sharded threshold search (sim_range_sharded.cu); the all-gather callback has the dcr_allgather_fn signature
+// gallery-sharded top-k and threshold search (sim_sharded.cu); the all-gather callback has the dcr_allgather_fn signature
 typedef int (*AllgatherFn)(const void* send, void* recv, size_t bytes_per_rank, void* ctx, void* stream);
+size_t sim_topk_sharded_workspace_size(int nq, int ng_local, int d, int k, int world);
+int sim_topk_sharded(const float* q, int nq, const float* g, int ng_local, int d, int k, long long g_index_base,
+                     long long g_index_stride, int world, AllgatherFn allgather, void* allgather_ctx, float* out_scores,
+                     long long* out_idx, void* ws, size_t ws_bytes, cudaStream_t stream, SimStats* stats);
 size_t sim_range_sharded_workspace_size(int nq, int ng_local, int d, int world, long long max_local_pairs);
 int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int d, float threshold, long long g_index_base,
                       long long g_index_stride, int world, AllgatherFn allgather, void* allgather_ctx, long long* row_offsets,

@@ -176,10 +176,9 @@ int fid_merge(FidState* s, const void* packed, int count, cudaStream_t stream) {
   }
   if (n == s->n) return 0;   // only empty states
   const size_t elems = static_cast<size_t>(d) * d;
-  fid_merge_kernel<<<static_cast<unsigned>((elems + 255) / 256), 256, 0, stream>>>(
-      static_cast<const unsigned char*>(packed), stride, count, d, s->n, s->shift, s->sum, s->xtx);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
+  if (int rc = launch(fid_merge_kernel, static_cast<unsigned>((elems + 255) / 256), 256, 0, stream, "fid_merge",
+                      static_cast<const unsigned char*>(packed), stride, count, d, s->n, s->shift, s->sum, s->xtx))
+    return rc;
   s->n = n;
   return 0;
 }
@@ -210,13 +209,13 @@ int fid_accumulate(FidState* s, const float* act, int n, cudaStream_t stream) {
   DCR_REQUIRE(s && act, "fid_accumulate: null argument");
   if (n <= 0) return 0;
   if (s->n == 0) {
-    fid_shift_kernel<<<(s->d + 127) / 128, 128, 0, stream>>>(act, n, s->d, s->shift);
-    count_launch();
+    if (int rc = launch(fid_shift_kernel, (s->d + 127) / 128, 128, 0, stream, "fid_accumulate", act, n, s->d, s->shift))
+      return rc;
   }
   const int t = (s->d + kTile - 1) / kTile;
-  fid_accumulate_kernel<<<dim3(t, t), 256, 0, stream>>>(act, n, s->d, s->shift, s->sum, s->xtx);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
+  if (int rc = launch(fid_accumulate_kernel, dim3(t, t), 256, 0, stream, "fid_accumulate", act, n, s->d, s->shift, s->sum,
+                      s->xtx))
+    return rc;
   s->n += n;
   return 0;
 }

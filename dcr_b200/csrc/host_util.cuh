@@ -58,14 +58,15 @@ int require_sm90a(const DeviceInfo* di, const char* who);
 // (kernel, device), so every later size is covered; more than that is refused (-1, naming `who`).
 int allow_dynamic_smem(const void* func, size_t bytes, const char* who);
 
-// kern<<<grid, block, smem, stream>>>(args...) after allow_dynamic_smem, counted, with the launch error checked
+// kern<<<grid, block, smem, stream>>>(args...) after allow_dynamic_smem, counted, with a launch error named after `who`
 template <class... Params, class... Args>
 int launch(void (*kern)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, const char* who,
            Args&&... args) {
   if (int rc = allow_dynamic_smem(reinterpret_cast<const void*>(kern), smem, who)) return rc;
   kern<<<grid, block, smem, stream>>>(std::forward<Args>(args)...);
   count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(-2, "%s: kernel launch failed: %s", who, cudaGetErrorString(e));
   return 0;
 }
 

@@ -153,21 +153,22 @@ __global__ void __launch_bounds__(256) stem_rows_kernel(const StemRowsParams p) 
   }
 }
 
-// Calls launch(kF32, kResize), both std::bool_constant, for the form of the source.
-template <class Launch>
-void with_source_form(const ImageSource& s, Launch&& launch) {
+// Returns body(kF32, kResize), both std::bool_constant, for the form of the source.
+template <class Body>
+int with_source_form(const ImageSource& s, Body&& body) {
   if (s.img_f32) {
-    if (s.rscale == 0.f) launch(std::true_type{}, std::false_type{});
-    else launch(std::true_type{}, std::true_type{});
-  } else {
-    if (s.rscale == 0.f) launch(std::false_type{}, std::false_type{});
-    else launch(std::false_type{}, std::true_type{});
+    if (s.rscale == 0.f) return body(std::true_type{}, std::false_type{});
+    return body(std::true_type{}, std::true_type{});
   }
+  if (s.rscale == 0.f) return body(std::false_type{}, std::false_type{});
+  return body(std::false_type{}, std::true_type{});
 }
 
 template <int KW>
-void launch_im2col(const Im2colParams& p, int grid, cudaStream_t stream) {
-  with_source_form(p.src, [&](auto f32, auto resize) { im2col_u8_kernel<KW, f32, resize><<<grid, 256, 0, stream>>>(p); });
+int launch_im2col(const Im2colParams& p, int grid, cudaStream_t stream) {
+  return with_source_form(p.src, [&](auto f32, auto resize) {
+    return launch(im2col_u8_kernel<KW, f32, resize>, grid, 256, 0, stream, "im2col_u8", p);
+  });
 }
 
 }  // namespace
@@ -187,14 +188,11 @@ int im2col_u8(const ImageSource& src, int B, int kh, int kw, int stride, int pad
   p.OW = (src.RW + 2 * pad - kw) / stride + 1;
   p.out = out; p.out_plane_stride = out_plane_stride; p.planes = planes;
   const int grid = grid_for(static_cast<long long>(B) * p.OH * p.OW * ((k_pad + rp - 1) / rp), 256, di->num_sms);
-  if (kw == 7) launch_im2col<7>(p, grid, stream);
-  else if (kw == 3) launch_im2col<3>(p, grid, stream);
-  else if (kw == 8) launch_im2col<8>(p, grid, stream);
-  else if (kw == 14) launch_im2col<14>(p, grid, stream);
-  else launch_im2col<16>(p, grid, stream);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  if (kw == 7) return launch_im2col<7>(p, grid, stream);
+  if (kw == 3) return launch_im2col<3>(p, grid, stream);
+  if (kw == 8) return launch_im2col<8>(p, grid, stream);
+  if (kw == 14) return launch_im2col<14>(p, grid, stream);
+  return launch_im2col<16>(p, grid, stream);
 }
 
 int stem_s2d_u8(const ImageSource& src, int B, __nv_bfloat16* out, long long out_plane_stride, int planes,
@@ -209,10 +207,9 @@ int stem_s2d_u8(const ImageSource& src, int B, __nv_bfloat16* out, long long out
   p.U = (src.RH + 6) / 2; p.V = (src.RW + 6) / 2;
   p.out = out; p.out_plane_stride = out_plane_stride; p.planes = planes;
   const int grid = grid_for(static_cast<long long>(B) * p.U * p.V, 256, di->num_sms);
-  with_source_form(src, [&](auto f32, auto resize) { stem_s2d_u8_kernel<f32, resize><<<grid, 256, 0, stream>>>(p); });
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return with_source_form(src, [&](auto f32, auto resize) {
+    return launch(stem_s2d_u8_kernel<f32, resize>, grid, 256, 0, stream, "stem_s2d_u8", p);
+  });
 }
 
 int stem_rows(const ImageSource& src, int B, __nv_bfloat16* out, cudaStream_t stream) {
@@ -229,10 +226,9 @@ int stem_rows(const ImageSource& src, int B, __nv_bfloat16* out, cudaStream_t st
   p.plane_stride = stem_fused_plane_units(OH, OW) * 8;
   p.img_stride = 2 * p.plane_stride;
   const int grid = grid_for(2ll * p.rows * p.PW * B, 256, di->num_sms);
-  with_source_form(src, [&](auto f32, auto resize) { stem_rows_kernel<f32, resize><<<grid, 256, 0, stream>>>(p); });
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return with_source_form(src, [&](auto f32, auto resize) {
+    return launch(stem_rows_kernel<f32, resize>, grid, 256, 0, stream, "stem_rows", p);
+  });
 }
 
 }  // namespace dcr

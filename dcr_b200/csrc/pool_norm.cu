@@ -461,10 +461,8 @@ int embed_tokens(const int* ids, int B, int T, int C, const float* table, int vo
   EmbedParams p;
   p.ids = ids; p.table = table; p.pos = pos; p.out = out; p.out_plane_stride = out_plane_stride;
   p.planes = planes; p.B = B; p.T = T; p.C = C; p.vocab = vocab;
-  embed_tokens_kernel<<<grid_for(static_cast<long long>(B) * T * (C / 8), 256, di->num_sms), 256, 0, stream>>>(p);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(embed_tokens_kernel, grid_for(static_cast<long long>(B) * T * (C / 8), 256, di->num_sms), 256, 0, stream,
+                "embed_tokens", p);
 }
 
 int pool2d(bool is_max, const __nv_bfloat16* in, long long in_plane_stride, __nv_bfloat16* out,
@@ -483,14 +481,12 @@ int pool2d(bool is_max, const __nv_bfloat16* in, long long in_plane_stride, __nv
   const long long total = static_cast<long long>(B) * p.OH * p.OW * (C / 8);
   if (is_max && planes == 1 && k == 3 && stride <= 2 && !tuning_flag("DCR_POOL_GENERIC")) {
     const long long total2 = static_cast<long long>(B) * p.OH * ((p.OW + 1) / 2) * (C / 8);
-    maxpool3_bf16_kernel<<<grid_for(total2, 256, di->num_sms), 256, 0, stream>>>(p);
-  } else if (!is_max && planes == 1 && k == 3 && !tuning_flag("DCR_POOL_GENERIC")) {
-    avgpool3_bf16_kernel<<<grid_for(total, 256, di->num_sms), 256, 0, stream>>>(p);
-  } else if (is_max) pool_kernel<true><<<grid_for(total, 256, di->num_sms), 256, 0, stream>>>(p);
-  else pool_kernel<false><<<grid_for(total, 256, di->num_sms), 256, 0, stream>>>(p);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+    return launch(maxpool3_bf16_kernel, grid_for(total2, 256, di->num_sms), 256, 0, stream, "pool2d", p);
+  }
+  if (!is_max && planes == 1 && k == 3 && !tuning_flag("DCR_POOL_GENERIC"))
+    return launch(avgpool3_bf16_kernel, grid_for(total, 256, di->num_sms), 256, 0, stream, "pool2d", p);
+  if (is_max) return launch(pool_kernel<true>, grid_for(total, 256, di->num_sms), 256, 0, stream, "pool2d", p);
+  return launch(pool_kernel<false>, grid_for(total, 256, di->num_sms), 256, 0, stream, "pool2d", p);
 }
 
 int reduce_hw(bool gem, const __nv_bfloat16* in, long long in_plane_stride, int planes, int B, int HW, int C,
@@ -503,12 +499,9 @@ int reduce_hw(bool gem, const __nv_bfloat16* in, long long in_plane_stride, int 
   if (B == 0) return 0;
   const int cg = C / 8;
   dim3 grid(B, (cg + 63) / 64);
-  if (gem && p_exp == 3.f) reduce_hw_kernel<true, true><<<grid, 64 * kRedSlices, 0, stream>>>(p);
-  else if (gem) reduce_hw_kernel<true, false><<<grid, 64 * kRedSlices, 0, stream>>>(p);
-  else reduce_hw_kernel<false, false><<<grid, 64 * kRedSlices, 0, stream>>>(p);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  if (gem && p_exp == 3.f) return launch(reduce_hw_kernel<true, true>, grid, 64 * kRedSlices, 0, stream, "reduce_hw", p);
+  if (gem) return launch(reduce_hw_kernel<true, false>, grid, 64 * kRedSlices, 0, stream, "reduce_hw", p);
+  return launch(reduce_hw_kernel<false, false>, grid, 64 * kRedSlices, 0, stream, "reduce_hw", p);
 }
 
 int layernorm(const __nv_bfloat16* in, long long in_plane_stride, int planes, int rows, int C, long long in_row_stride,
@@ -525,20 +518,13 @@ int layernorm(const __nv_bfloat16* in, long long in_plane_stride, int planes, in
   if (planes == 1 && C % 128 == 0 && C / 128 >= 3 && C / 128 <= 8 && in_row_stride % 8 == 0 && !tuning_flag("DCR_LN_GENERIC")) {
     const int blocks = std::min((rows + 15) / 16, di->num_sms * 8);        // 16 half-warps per 256-thread block
     switch (C / 128) {
-      case 3: layernorm_fast_kernel<3><<<blocks, 256, 0, stream>>>(p); break;
-      case 4: layernorm_fast_kernel<4><<<blocks, 256, 0, stream>>>(p); break;
-      case 6: layernorm_fast_kernel<6><<<blocks, 256, 0, stream>>>(p); break;
-      case 8: layernorm_fast_kernel<8><<<blocks, 256, 0, stream>>>(p); break;
-      default: layernorm_kernel<<<std::min((rows + 3) / 4, di->num_sms * 32), 128, 0, stream>>>(p); break;
+      case 3: return launch(layernorm_fast_kernel<3>, blocks, 256, 0, stream, "layernorm", p);
+      case 4: return launch(layernorm_fast_kernel<4>, blocks, 256, 0, stream, "layernorm", p);
+      case 6: return launch(layernorm_fast_kernel<6>, blocks, 256, 0, stream, "layernorm", p);
+      case 8: return launch(layernorm_fast_kernel<8>, blocks, 256, 0, stream, "layernorm", p);
     }
-    count_launch();
-    DCR_CUDA_CHECK(cudaGetLastError());
-    return 0;
   }
-  layernorm_kernel<<<std::min((rows + 3) / 4, di->num_sms * 32), 128, 0, stream>>>(p);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(layernorm_kernel, std::min((rows + 3) / 4, di->num_sms * 32), 128, 0, stream, "layernorm", p);
 }
 
 int vit_tokens(const __nv_bfloat16* patch, long long patch_plane_stride, const float* cls, const float* pos,
@@ -551,10 +537,7 @@ int vit_tokens(const __nv_bfloat16* patch, long long patch_plane_stride, const f
   p.out_plane_stride = out_plane_stride; p.planes = planes; p.B = B; p.NP = NP; p.C = C;
   if (B == 0) return 0;
   const long long total = static_cast<long long>(B) * (NP + 1) * (C / 8);
-  vit_tokens_kernel<<<grid_for(total, 256, di->num_sms), 256, 0, stream>>>(p);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(vit_tokens_kernel, grid_for(total, 256, di->num_sms), 256, 0, stream, "vit_tokens", p);
 }
 
 }  // namespace dcr

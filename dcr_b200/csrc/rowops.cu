@@ -105,11 +105,8 @@ int pad_topk_lists(const float* s_in, const long long* i_in, int nq, int k_in, i
                    cudaStream_t stream) {
   DCR_REQUIRE(nq >= 1 && k_in >= 1 && k_out >= k_in, "pad_topk_lists: bad arguments");
   const long long total = static_cast<long long>(nq) * k_out;
-  pad_topk_lists_kernel<<<static_cast<int>(std::min<long long>((total + 255) / 256, 1184)), 256, 0, stream>>>(s_in, i_in, nq, k_in, k_out,
-                                                                                                       s_out, i_out);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(pad_topk_lists_kernel, static_cast<int>(std::min<long long>((total + 255) / 256, 1184)), 256, 0, stream,
+                "pad_topk_lists", s_in, i_in, nq, k_in, k_out, s_out, i_out);
 }
 
 int l2_normalize(float* x, int n, int d, float eps, cudaStream_t stream) {
@@ -118,10 +115,7 @@ int l2_normalize(float* x, int n, int d, float eps, cudaStream_t stream) {
   const DeviceInfo* di = device_info();
   if (!di) return -2;
   const int blocks = std::min((n + 7) / 8, di->num_sms * 8);
-  l2_normalize_kernel<<<blocks, 256, 0, stream>>>(x, n, d, eps);
-  count_launch();
-  DCR_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  return launch(l2_normalize_kernel, blocks, 256, 0, stream, "l2_normalize", x, n, d, eps);
 }
 
 int topk_merge(const float* scores, const long long* idx, int nq, int nlists, int k_in, int k_out, float* out_scores,

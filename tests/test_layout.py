@@ -66,13 +66,18 @@ def test_similarity_planner_accepts_the_supported_shape_range():
 
 
 def test_hopper_scaffolding_has_one_definition():
-    """The opt-in to large dynamic shared memory, the TMA bulk-store group and the 1024-byte alignment of dynamic shared
-    memory are each written once (host_util.cu, ptx.cuh); kernels and launch sites use those instead of a private copy."""
+    """The opt-in to large dynamic shared memory, the kernel launch, the TMA bulk-store group and the 1024-byte alignment
+    of dynamic shared memory are each written once (host_util, ptx.cuh); kernels and launch sites use those instead of a
+    private copy."""
     csrc = os.path.join(ROOT, "dcr_b200", "csrc")
     texts = {f: open(os.path.join(csrc, f)).read() for f in sorted(os.listdir(csrc)) if f.endswith((".cu", ".cuh", ".h"))}
     for needle, home in [("cudaFuncSetAttribute", "host_util.cu"), ("cp.async.bulk.commit_group", "ptx.cuh"),
                          ("cp.async.bulk.wait_group", "ptx.cuh"), ("~uintptr_t(1023)", "ptx.cuh")]:
         assert [f for f, t in texts.items() if needle in t] == [home], needle
-    # the similarity engine launches every kernel through host_util's launch(): counted, error-checked, smem opted in
-    for f in ("sim_sweep.cu", "sim_topk.cu", "sim_range.cu"):
-        assert "<<<" not in texts[f], f
+    # every kernel is launched through host_util's launch(): counted, error-checked under its caller's name, smem opted in
+    sources = [f for f in texts if f.endswith((".cu", ".cuh"))]
+    assert "sim_sweep.cu" in sources and "pool_norm.cu" in sources
+    assert [f for f in sources if "<<<" in texts[f]] == ["host_util.cuh"]
+    assert [f for f in texts if "count_launch(" in texts[f]] == ["host_util.cu", "host_util.cuh"]
+    # workspaces are laid out with Carve, not with private round-up helpers
+    assert [f for f in texts if "up256" in texts[f]] == []
