@@ -14,7 +14,7 @@ class DcrError(RuntimeError):
     pass
 
 
-ERR_CAPACITY = -3   # DCR_ERR_CAPACITY: dcr_sim_range(_sharded) found more candidate pairs than its capacities
+ERR_CAPACITY = -3   # DCR_ERR_CAPACITY: dcr_sim_range(_split)(_sharded) found more candidate pairs than its capacities
 
 
 # name -> (restype, argtypes); mirrors include/dcr_b200.h one to one (tests check the header against this table)
@@ -43,6 +43,15 @@ SIGNATURES = {
                                         C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_int64, C.c_int64, C.POINTER(C.c_int64), C.c_void_p, C.c_size_t,
                                         C.c_void_p]),
+    "dcr_sim_range_split_workspace_size": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64]),
+    "dcr_sim_range_split": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int64,
+                                      C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
+                                      C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dcr_sim_range_split_sharded_workspace_size": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64]),
+    "dcr_sim_range_split_sharded": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float,
+                                              C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.POINTER(C.c_int64),
+                                              C.c_void_p, C.c_size_t, C.c_void_p]),
     "dcr_sim_topk_last_stats": (C.c_int, [C.POINTER(C.c_int)]),
     "dcr_sim_topk_last_kernel_ms": (C.c_float, []),
     "dcr_sim_topk_last_sm_mhz": (C.c_float, []),

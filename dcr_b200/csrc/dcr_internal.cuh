@@ -38,6 +38,12 @@ size_t sim_range_workspace_size(int nq, int ng, int d, long long max_pairs);
 int sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, long long g_index_base,
               long long g_index_stride, long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,
               long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream);
+// threshold search under the split score (sim_range.cu); n_parts = 1 is sim_range
+size_t sim_range_split_workspace_size(int nq, int ng, int d, int n_parts, long long max_pairs);
+int sim_range_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, float threshold,
+                    long long g_index_base, long long g_index_stride, long long* row_offsets, long long* out_idx,
+                    float* out_scores, long long max_pairs, long long* counts, void* ws, size_t ws_bytes,
+                    cudaStream_t stream);
 // out[0..n] = exclusive prefix sums of in[0..n-1], out[n] = total: one block, a fixed association (sim_range's row scan)
 int exclusive_scan_i64(const long long* in, long long n, long long* out, cudaStream_t stream);
 
@@ -52,6 +58,12 @@ int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int 
                       long long g_index_stride, int world, AllgatherFn allgather, void* allgather_ctx, long long* row_offsets,
                       long long* out_idx, float* out_scores, long long max_pairs, long long max_local_pairs,
                       long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream);
+size_t sim_range_split_sharded_workspace_size(int nq, int ng_local, int d, int n_parts, int world, long long max_local_pairs);
+int sim_range_split_sharded(const float* q, int nq, const float* g, int ng_local, int d, int n_parts, float threshold,
+                            long long g_index_base, long long g_index_stride, int world, AllgatherFn allgather,
+                            void* allgather_ctx, long long* row_offsets, long long* out_idx, float* out_scores,
+                            long long max_pairs, long long max_local_pairs, long long* counts, void* ws, size_t ws_bytes,
+                            cudaStream_t stream);
 
 int split_rescore(const float* q, const float* g, int nq, int d, int n_chunks, int cross, const long long* cand, int n_cand,
                   int k, float* out_scores, long long* out_idx, cudaStream_t stream);

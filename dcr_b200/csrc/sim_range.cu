@@ -24,6 +24,9 @@ namespace {
 //                              pairs that reach tau
 //   6. exclusive_scan_kernel over the pieces, range_output_kernel / range_row_offsets_kernel: the CSR arrays
 // Everything is a fixed function of the inputs (no atomics decide an order), so every call returns the same bits.
+// Under the split score (sim_range_split, n_parts > 0) the same steps run on the split operands: the sweep folds the
+// parts into a running maximum (fused_tile_mma_split), the bound is split_row_bound and the re-score takes the maximum
+// of the per-part exact dot products (DESIGN.md section 3).
 constexpr int kRangePiece = 512;   // candidates of one row re-scored by one block
 
 struct RangeParams : SweepHead {
@@ -34,6 +37,7 @@ struct RangeParams : SweepHead {
   int* seg;                    // [n_slots][128] count sweep: candidates; emit sweep: offset inside the row
   const long long* row_cand;   // [nq + 1] emit sweep: first candidate of each row
   int* cand_idx;               // emit sweep: local gallery rows
+  int kb_part;                 // split score: k-blocks per descriptor part (kSplit kernels only)
 };
 
 // Candidate columns of one 32-column chunk of an accumulator row: bit c is set when the approximate score of column
@@ -62,28 +66,42 @@ DCR_DEVICE uint32_t range_hits(const uint32_t (&r)[32], const float* sb, float t
 // consumer warpgroup, an epilogue that compares every accumulator column against its row's threshold, and no warm-up.
 // kEmit = 0 counts the candidates of every (segment slot, row); kEmit = 1 writes them at the offsets the scan derived
 // from those counts.  Both make the same decisions: same tiles, same wgmma sequence, same thresholds.
-template <bool kBias, bool kEmit>
-__global__ void __launch_bounds__(32 + 128, 1)
+// kSplit: the split score.  A tile's approximate score is the maximum over the descriptor parts (fused_tile_mma_split),
+// and range_hits sees that maximum.  The running maximum and the part accumulator of a 128-column tile would take 256
+// registers per thread, so two consumer warpgroups each own one 64-column half of every tile, as in the split top-k.
+// After each tile the halves trade their per-row hit counts through shared memory: the lower half's columns come first
+// in the row, so both halves count the same total and the emit sweep writes the row in ascending column order.
+template <bool kBias, bool kEmit, bool kSplit = false>
+__global__ void __launch_bounds__(32 + 128 * (kSplit ? 2 : 1), 1)
     sim_range_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_g,
                      const RangeParams p) {
+  static_assert(!kSplit || !kBias, "the split score is not centred");
+  constexpr int kSets = kSplit ? 2 : 1;
+  constexpr int kSetCols = kBlockN / kSets;
   if (((p.bias_flag != nullptr) && (*p.bias_flag != 0)) != kBias) return;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const FusedPipe pp(smem_raw, p.num_kb, p.stream_a, p.stages, 0);   // then barriers, then 4 transpose buffers
+  // the pipeline, then barriers, then 4 kSets transpose buffers (split: then the halves' hit counts [2][2][128])
+  const FusedPipe pp(smem_raw, p.num_kb, p.stream_a, p.stages, 0);
   const uint32_t warp = threadIdx.x >> 5;
   const uint32_t lane = threadIdx.x & 31;
-  pp.init(&tmap_q, &tmap_g, p.stages, 4);
+  pp.init(&tmap_q, &tmap_g, p.stages, 4 * kSets);
   const long long n_units = gridDim.x;
   const long long unit = blockIdx.x;
   SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
-  if (warp == 4) {
+  if (warp == 4 * kSets) {
     fused_producer(pp, &tmap_q, &tmap_g, p.stages, w, [](const SegWalker&) { return 0; });
   } else {
-    const uint32_t row = warp * 32 + lane;   // query row inside the tile
+    const uint32_t set = kSplit ? warp >> 2 : 0;                    // column half of every tile (split)
+    const uint32_t row = (kSplit ? warp & 3 : warp) * 32 + lane;   // query row inside the tile
     const uint32_t xacc = smem_u32(pp.tail) + warp * kAccXposeWarpBytes;
+    // [tile parity][set][row]: tile n writes buffer n & 1, so a half that runs ahead never overwrites a count the
+    // other half has yet to read (it first passes the barrier of tile n + 1)
+    int* half_cnt = reinterpret_cast<int*>(pp.tail + 4 * kSets * kAccXposeWarpBytes);
     const uint32_t a_base = smem_u32(pp.stream_a ? pp.smem_b + kBTileBytes : pp.smem_a);
-    const uint32_t b_base = smem_u32(pp.smem_b);
+    const uint32_t b_base = smem_u32(pp.smem_b) + set * kSetCols * 128;
     PipeState st(p.stages);
     uint32_t seg = 0;
+    uint32_t tile_no = 0;   // tiles swept so far (split: the parity of the hit-count buffer)
     while (w.next()) {
       const int qrow = w.qi * kBlockM + static_cast<int>(row);
       const bool row_ok = qrow < p.nq;
@@ -96,24 +114,56 @@ __global__ void __launch_bounds__(32 + 128, 1)
       if (!pp.stream_a) mbar_wait(pp.a_full, seg & 1);
 #pragma unroll 1
       for (int j = 0; j < w.ntiles; ++j) {
-        WgAcc<kBlockN> acc;
-        fused_tile_mma(acc, st, pp, a_base, b_base, j == w.ntiles - 1, lane);
-        const int gcol0 = (w.g_begin + j) * kBlockN;
+        if constexpr (kSplit) {
+          WgAcc<kSetCols> acc;
+          fused_tile_mma_split(acc, st, pp, a_base, b_base, p.kb_part, j == w.ntiles - 1, lane);
+          const int gcol0 = (w.g_begin + j) * kBlockN + static_cast<int>(set) * kSetCols;
+          uint32_t hits[kSetCols / 32];
+          int mine = 0;
 #pragma unroll
-        for (int ch = 0; ch < kBlockN / 32; ++ch) {
-          uint32_t r[32];
-          acc.rows32(ch, r, xacc, lane);
-          const int col0 = gcol0 + ch * 32;
-          const uint32_t hits = range_hits<kBias>(r, kBias ? p.col_bias + col0 : nullptr, t, row_ok ? p.ng - col0 : 0);
+          for (int ch = 0; ch < kSetCols / 32; ++ch) {
+            uint32_t r[32];
+            acc.rows32(ch, r, xacc, lane);
+            const int col0 = gcol0 + ch * 32;
+            hits[ch] = range_hits<false>(r, nullptr, t, row_ok ? p.ng - col0 : 0);
+            mine += __popc(hits[ch]);
+          }
+          int* hc = half_cnt + (tile_no & 1) * 2 * kBlockM;
+          hc[set * kBlockM + row] = mine;
+          named_bar_sync(1, 128 * kSets);
+          const int lower = hc[row], both = lower + hc[kBlockM + row];
+          ++tile_no;
           if constexpr (kEmit) {
-            for (uint32_t h = hits; h; h &= h - 1) *out++ = col0 + __ffs(h) - 1;   // ascending columns
+            if (mine) {
+              int* o = out + (set ? lower : 0);
+#pragma unroll
+              for (int ch = 0; ch < kSetCols / 32; ++ch)
+                for (uint32_t h = hits[ch]; h; h &= h - 1) *o++ = gcol0 + ch * 32 + __ffs(h) - 1;   // ascending columns
+            }
+            if (both) out += both;
           } else {
-            cnt += __popc(hits);
+            cnt += both;
+          }
+        } else {
+          WgAcc<kBlockN> acc;
+          fused_tile_mma(acc, st, pp, a_base, b_base, j == w.ntiles - 1, lane);
+          const int gcol0 = (w.g_begin + j) * kBlockN;
+#pragma unroll
+          for (int ch = 0; ch < kBlockN / 32; ++ch) {
+            uint32_t r[32];
+            acc.rows32(ch, r, xacc, lane);
+            const int col0 = gcol0 + ch * 32;
+            const uint32_t hits = range_hits<kBias>(r, kBias ? p.col_bias + col0 : nullptr, t, row_ok ? p.ng - col0 : 0);
+            if constexpr (kEmit) {
+              for (uint32_t h = hits; h; h &= h - 1) *out++ = col0 + __ffs(h) - 1;   // ascending columns
+            } else {
+              cnt += __popc(hits);
+            }
           }
         }
       }
       ++seg;
-      if (!kEmit) p.seg[sr] = cnt;
+      if (!kEmit && set == 0) p.seg[sr] = cnt;   // split: both halves hold the row's total
     }
   }
   __syncthreads();
@@ -121,8 +171,11 @@ __global__ void __launch_bounds__(32 + 128, 1)
 
 // t_i = tau - q.mu - eps - slack - margin, rounded down at every step.  fp32(s) >= tau needs s >= tau - half an fp32 ulp
 // (margin), hence approximate score >= t_i (row_bound).  A warp per query row.
+// kSplit: the split score, with eps and slack from split_row_bound (q.mu = 0; d_pad = n_parts * p_pad).  A NaN part norm
+// makes eps and t_i NaN, and !(a < NaN) keeps every column of that row: the exact re-score decides them all.
+template <bool kSplit>
 __global__ void __launch_bounds__(128)
-    range_threshold_kernel(const float* __restrict__ q, int nq, int d, int d_pad, float tau,
+    range_threshold_kernel(const float* __restrict__ q, int nq, int d, int d_pad, int n_parts, float tau,
                            const float* __restrict__ q_norm_hat, const float* __restrict__ q_norm_res,
                            const float* __restrict__ q_norm_x, const unsigned int* __restrict__ g_max,
                            const float* __restrict__ mu, const float* __restrict__ nu, const int* __restrict__ nu_flag,
@@ -130,8 +183,13 @@ __global__ void __launch_bounds__(128)
   const int row = blockIdx.x * 4 + static_cast<int>(threadIdx.x >> 5);
   const uint32_t lane = threadIdx.x & 31;
   if (row >= nq) return;
-  const RowBound rb = row_bound(q + static_cast<size_t>(row) * d, d, d_pad, row, q_norm_hat, q_norm_res, q_norm_x, g_max,
-                                mu, nu, nu_flag, lane);
+  const RowBound rb = [&] {
+    if constexpr (kSplit)
+      return split_row_bound(n_parts, d / n_parts, d_pad / n_parts, row, q_norm_hat, q_norm_res, q_norm_x, g_max, lane);
+    else
+      return row_bound(q + static_cast<size_t>(row) * d, d, d_pad, row, q_norm_hat, q_norm_res, q_norm_x, g_max, mu, nu,
+                       nu_flag, lane);
+  }();
   if (lane == 0) {
     const double margin = isfinite(tau) ? fabs(static_cast<double>(tau)) * 1.2e-7 + 1e-45 : 0.0;
     double t = __dsub_rd(static_cast<double>(tau), rb.qmu);
@@ -219,29 +277,68 @@ DCR_DEVICE void range_piece(long long w, const long long* __restrict__ row_cand,
 
 // Exact scores of one piece (exact_dot: the values dcr_sim_topk reports), then a stable in-place
 // compaction of the pairs with fp32 score >= tau.  piece_kept[w] = pairs kept.
+// kSplit: the split score, bit for bit what dcr_split_rescore reports.  A split row is far wider than shared memory, so the
+// query is staged one part at a time: per part, stage the query part, prefetch that part of the piece's candidates, and
+// fold the part's exact_dot into the candidate's fp64 running maximum (-inf, then parts 0, 1, ..: the order of
+// split_rescore_kernel); the maximum is rounded to fp32 once.
+template <bool kSplit>
 __global__ void __launch_bounds__(kRescoreThreads)
-    range_rescore_kernel(const float* __restrict__ q, const float* __restrict__ g, int nq, int d, float tau,
+    range_rescore_kernel(const float* __restrict__ q, const float* __restrict__ g, int nq, int d, int n_parts, float tau,
                          const long long* __restrict__ row_cand, const long long* __restrict__ row_piece,
                          int* __restrict__ cand_idx, float* __restrict__ cand_score, int* __restrict__ piece_kept) {
   extern __shared__ __align__(16) uint8_t sm[];
-  double* qs = reinterpret_cast<double*>(sm);   // [d] the query row, widened once
   const int tid = threadIdx.x;
   const uint32_t lane = threadIdx.x & 31;
   const int warp = tid >> 5;
   int row, n;
   long long start;
   range_piece(blockIdx.x, row_cand, row_piece, nq, row, start, n);
-  for (int c = tid; c < d; c += kRescoreThreads) qs[c] = static_cast<double>(q[static_cast<size_t>(row) * d + c]);
-  __syncthreads();
   int* ci = cand_idx + start;
   float* cs = cand_score + start;
-  for (int c = 2 * warp; c < n; c += 2 * (kRescoreThreads / 32)) {
-    double v0, v1 = 0.0;
-    if (c + 1 < n) exact_dot<2>(qs, g + static_cast<size_t>(ci[c]) * d, g + static_cast<size_t>(ci[c + 1]) * d, d, lane, v0, v1);
-    else exact_dot<1>(qs, g + static_cast<size_t>(ci[c]) * d, nullptr, d, lane, v0, v1);
-    if (lane == 0) {
-      cs[c] = static_cast<float>(v0);
-      if (c + 1 < n) cs[c + 1] = static_cast<float>(v1);
+  if constexpr (kSplit) {
+    double* best = reinterpret_cast<double*>(sm);   // [kRangePiece] running maxima of the piece's candidates
+    double* qs = best + kRangePiece;                // [d / n_parts] the query part, widened
+    const int pl = d / n_parts;
+    for (int c = tid; c < n; c += kRescoreThreads) best[c] = -INFINITY;
+    const float* qsrc = q + static_cast<size_t>(row) * d;
+    const float* gp = g;   // part `part` of gallery row 0
+    for (int part = 0; part < n_parts; ++part, qsrc += pl, gp += pl) {
+      __syncthreads();   // the previous part's readers of qs are done (and the maxima initialised)
+      for (int c = tid * 4; c < pl; c += kRescoreThreads * 4) {
+        const float4 v = *reinterpret_cast<const float4*>(qsrc + c);
+        *reinterpret_cast<double2*>(qs + c) = make_double2(static_cast<double>(v.x), static_cast<double>(v.y));
+        *reinterpret_cast<double2*>(qs + c + 2) = make_double2(static_cast<double>(v.z), static_cast<double>(v.w));
+      }
+      for (int c = warp; c < n; c += kRescoreThreads / 32) {   // a warp per candidate, a lane per 128-byte line
+        const float* gr = gp + static_cast<size_t>(ci[c]) * d;
+        for (int l = static_cast<int>(lane) * 32; l < pl; l += 32 * 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(gr + l));
+      }
+      __syncthreads();
+      for (int c = 2 * warp; c < n; c += 2 * (kRescoreThreads / 32)) {
+        const float* g0 = gp + static_cast<size_t>(ci[c]) * d;
+        double v0, v1 = 0.0;
+        if (c + 1 < n) exact_dot<2>(qs, g0, gp + static_cast<size_t>(ci[c + 1]) * d, pl, lane, v0, v1);
+        else exact_dot<1>(qs, g0, nullptr, pl, lane, v0, v1);
+        if (lane == 0) {
+          best[c] = fmax(best[c], v0);
+          if (c + 1 < n) best[c + 1] = fmax(best[c + 1], v1);
+        }
+      }
+    }
+    __syncthreads();
+    for (int c = tid; c < n; c += kRescoreThreads) cs[c] = static_cast<float>(best[c]);
+  } else {
+    double* qs = reinterpret_cast<double*>(sm);   // [d] the query row, widened once
+    for (int c = tid; c < d; c += kRescoreThreads) qs[c] = static_cast<double>(q[static_cast<size_t>(row) * d + c]);
+    __syncthreads();
+    for (int c = 2 * warp; c < n; c += 2 * (kRescoreThreads / 32)) {
+      double v0, v1 = 0.0;
+      if (c + 1 < n) exact_dot<2>(qs, g + static_cast<size_t>(ci[c]) * d, g + static_cast<size_t>(ci[c + 1]) * d, d, lane, v0, v1);
+      else exact_dot<1>(qs, g + static_cast<size_t>(ci[c]) * d, nullptr, d, lane, v0, v1);
+      if (lane == 0) {
+        cs[c] = static_cast<float>(v0);
+        if (c + 1 < n) cs[c + 1] = static_cast<float>(v1);
+      }
     }
   }
   __syncthreads();
@@ -297,6 +394,7 @@ constexpr long long kMaxRangePairs = 1ll << 40;   // capacity accepted by the pl
 
 struct RangePlan {
   SweepGeometry geo;
+  int n_parts;   // split score: descriptor parts; 0 = dot product
   int nq_pad, n_qtiles, n_units, n_slots, stages;
   size_t smem_bytes;
   long long max_pieces;   // pieces of kRangePiece candidates when max_pairs candidates fill the rows worst
@@ -318,8 +416,12 @@ struct RangeBuffers {
 
 RangeBuffers carve_range(const RangePlan& rp, int nq, int d, long long max_pairs, Carve& w) {
   RangeBuffers b;
-  b.ops = carve_operands(w, rp.nq_pad, rp.geo, d);
-  b.ops.qflag = w.take<int>(4);
+  if (rp.n_parts) {
+    b.ops = carve_split_operands(w, rp.nq_pad, rp.geo, rp.n_parts);   // no centring: no flag
+  } else {
+    b.ops = carve_operands(w, rp.nq_pad, rp.geo, d);
+    b.ops.qflag = w.take<int>(4);
+  }
   b.thr = w.take<float>(nq);
   b.seg = w.take<int>(static_cast<size_t>(rp.n_slots) * kBlockM);
   b.row_cnt = w.take<long long>(nq);
@@ -333,19 +435,40 @@ RangeBuffers carve_range(const RangePlan& rp, int nq, int d, long long max_pairs
   return b;
 }
 
-int make_range_plan(int nq, int ng, int d, long long max_pairs, int num_sms, size_t max_smem, RangePlan* rp) {
-  DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "sim_range: empty problem (nq=%d ng=%d d=%d)", nq, ng, d);
-  DCR_REQUIRE(d <= kMaxDim, "sim_range: descriptor dim %d > %d not supported", d, kMaxDim);
-  DCR_REQUIRE(d % 4 == 0, "sim_range: descriptor dim %d is not a multiple of 4", d);
-  DCR_REQUIRE(max_pairs >= 0 && max_pairs <= kMaxRangePairs, "sim_range: max_pairs=%lld outside [0, 2^40]", max_pairs);
-  plan_geometry(ng, d, &rp->geo);
+// n_parts = 0: the dot product (sim_range); >= 2: the split score over n_parts parts (sim_range_split)
+int make_range_plan(int nq, int ng, int d, int n_parts, long long max_pairs, int num_sms, size_t max_smem, RangePlan* rp) {
+  const char* who = n_parts ? "sim_range_split" : "sim_range";
+  DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "%s: empty problem (nq=%d ng=%d d=%d)", who, nq, ng, d);
+  if (n_parts) {
+    DCR_REQUIRE(n_parts >= 1 && d % n_parts == 0 && (d / n_parts) % 4 == 0,
+                "sim_range_split: d=%d must split into %d parts whose length is a multiple of 4", d, n_parts);
+    const int p = d / n_parts;
+    DCR_REQUIRE(p <= kMaxDim, "sim_range_split: part length %d > %d not supported", p, kMaxDim);
+    DCR_REQUIRE(static_cast<long long>(n_parts) * ((p + kBlockK - 1) / kBlockK * kBlockK) <= (1ll << 30),
+                "sim_range_split: %d parts of %d padded to 64 exceed 2^30 columns", n_parts, p);
+  } else {
+    DCR_REQUIRE(d <= kMaxDim, "sim_range: descriptor dim %d > %d not supported", d, kMaxDim);
+    DCR_REQUIRE(d % 4 == 0, "sim_range: descriptor dim %d is not a multiple of 4", d);
+  }
+  DCR_REQUIRE(max_pairs >= 0 && max_pairs <= kMaxRangePairs, "%s: max_pairs=%lld outside [0, 2^40]", who, max_pairs);
+  rp->n_parts = n_parts;
+  if (n_parts) {
+    plan_split_geometry(ng, n_parts, d / n_parts, &rp->geo);
+    // the threshold sweep keeps no candidate lists in shared memory, so a query tile of up to 512 part-padded columns
+    // stays resident as in the dot product (the split top-k always streams it)
+    rp->geo.stream_a = rp->geo.num_kb > kMaxKB ? 1 : 0;
+  } else {
+    plan_geometry(ng, d, &rp->geo);
+  }
   const SweepGeometry& g = rp->geo;
   rp->n_qtiles = (nq + kBlockM - 1) / kBlockM;
   rp->nq_pad = rp->n_qtiles * kBlockM;
-  // shared memory: the pipeline, then the accumulator transposes of 4 warps
-  auto smem = [&](int st) { return FusedPipe::smem_bytes(g.num_kb, g.stream_a, st, 0, 4 * kAccXposeWarpBytes); };
+  // shared memory: the pipeline, then the accumulator transposes of 4 warps per consumer warpgroup (split: two
+  // warpgroups, then their per-tile hit counts)
+  const size_t tail = n_parts ? 8 * kAccXposeWarpBytes + 2 * 2 * kBlockM * sizeof(int) : 4 * kAccXposeWarpBytes;
+  auto smem = [&](int st) { return FusedPipe::smem_bytes(g.num_kb, g.stream_a, st, 0, tail); };
   int stages = 2;
-  DCR_REQUIRE(max_smem >= smem(stages), "sim_range: not enough shared memory (%zu B) for d=%d", max_smem, d);
+  DCR_REQUIRE(max_smem >= smem(stages), "%s: not enough shared memory (%zu B) for d=%d", who, max_smem, d);
   while (stages < 8 && max_smem >= smem(stages + 1)) ++stages;
   rp->stages = stages;
   rp->smem_bytes = smem(stages);
@@ -360,36 +483,43 @@ int make_range_plan(int nq, int ng, int d, long long max_pairs, int num_sms, siz
   return 0;
 }
 
-}  // namespace
-
-size_t sim_range_workspace_size(int nq, int ng, int d, long long max_pairs) {
+size_t range_workspace_size(int nq, int ng, int d, int n_parts, long long max_pairs) {
   const DeviceInfo* di = device_info();
   RangePlan rp;
-  if (make_range_plan(nq, ng, d, max_pairs, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &rp) != 0) return 0;
+  if (make_range_plan(nq, ng, d, n_parts, max_pairs, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &rp) != 0)
+    return 0;
   return rp.total;
 }
 
-int sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, long long g_index_base,
-              long long g_index_stride, long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,
-              long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
+// The whole search.  n_parts = 0: the dot product (sim_range); >= 2: the split score (sim_range_split).
+int range_search(const float* q, int nq, const float* g, int ng, int d, int n_parts, float threshold,
+                 long long g_index_base, long long g_index_stride, long long* row_offsets, long long* out_idx,
+                 float* out_scores, long long max_pairs, long long* counts, void* ws, size_t ws_bytes,
+                 cudaStream_t stream) {
+  const char* who = n_parts ? "sim_range_split" : "sim_range";
   const DeviceInfo* di = device_info();
   if (!di) return -2;
-  if (int rc = require_sm90a(di, "sim_range")) return rc;
-  DCR_REQUIRE(!std::isnan(threshold), "sim_range: threshold is NaN");
-  DCR_REQUIRE(g_index_stride >= 1, "sim_range: g_index_stride=%lld < 1", g_index_stride);
+  if (int rc = require_sm90a(di, who)) return rc;
+  DCR_REQUIRE(!std::isnan(threshold), "%s: threshold is NaN", who);
+  DCR_REQUIRE(g_index_stride >= 1, "%s: g_index_stride=%lld < 1", who, g_index_stride);
   RangePlan rp;
-  if (int rc = make_range_plan(nq, ng, d, max_pairs, di->num_sms, di->max_smem_optin, &rp)) return rc;
-  DCR_REQUIRE(ws != nullptr && ws_bytes >= rp.total, "sim_range: workspace too small (%zu < %zu)", ws_bytes, rp.total);
-  DCR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "sim_range: workspace must be 256-byte aligned");
+  if (int rc = make_range_plan(nq, ng, d, n_parts, max_pairs, di->num_sms, di->max_smem_optin, &rp)) return rc;
+  DCR_REQUIRE(ws != nullptr && ws_bytes >= rp.total, "%s: workspace too small (%zu < %zu)", who, ws_bytes, rp.total);
+  DCR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "%s: workspace must be 256-byte aligned", who);
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0,
-              "sim_range: q/g must be 16-byte aligned");
+              "%s: q/g must be 16-byte aligned", who);
   const SweepGeometry& geo = rp.geo;
   Carve w{static_cast<uint8_t*>(ws)};
   const RangeBuffers b = carve_range(rp, nq, d, max_pairs, w);
   const Operands& o = b.ops;
-  if (int rc = prepare_operands(q, nq, rp.nq_pad, g, ng, d, geo, di, o, stream)) return rc;
-  if (int rc = launch(range_threshold_kernel, (nq + 3) / 4, 128, 0, stream, "sim_range", q, nq, d, geo.d_pad, threshold,
-                      o.qnh, o.qnr, o.qnx, o.gmax, o.mu, o.nu, o.qflag, b.thr))
+  const int pl = n_parts ? d / n_parts : d;   // the length of one exact dot product (a part, or the whole row)
+  if (n_parts) {
+    if (int rc = prepare_split_operands(q, nq, rp.nq_pad, g, ng, n_parts, pl, geo, di, o, stream)) return rc;
+  } else {
+    if (int rc = prepare_operands(q, nq, rp.nq_pad, g, ng, d, geo, di, o, stream)) return rc;
+  }
+  if (int rc = launch(n_parts ? range_threshold_kernel<true> : range_threshold_kernel<false>, (nq + 3) / 4, 128, 0, stream,
+                      who, q, nq, d, geo.d_pad, n_parts, threshold, o.qnh, o.qnr, o.qnx, o.gmax, o.mu, o.nu, o.qflag, b.thr))
     return rc;
 
   CUtensorMap tq, tg;
@@ -402,11 +532,14 @@ int sim_range(const float* q, int nq, const float* g, int ng, int d, float thres
   p.seg = b.seg;
   p.row_cand = b.row_cand;
   p.cand_idx = b.cand_idx;
-  auto sweep = [&](auto off, auto on) {
-    return launch_sweep(off, on, rp.n_units, 32 + 128, rp.smem_bytes, stream, "sim_range", tq, tg, p);
+  p.kb_part = n_parts ? geo.num_kb / n_parts : 0;
+  auto sweep = [&](auto off, auto on, auto split) {
+    if (n_parts) return launch(split, rp.n_units, 32 + 128 * 2, rp.smem_bytes, stream, who, tq, tg, p);
+    return launch_sweep(off, on, rp.n_units, 32 + 128, rp.smem_bytes, stream, who, tq, tg, p);
   };
-  if (int rc = sweep(sim_range_kernel<false, false>, sim_range_kernel<true, false>)) return rc;
-  if (int rc = launch(range_slot_scan_kernel, (nq + 255) / 256, 256, 0, stream, "sim_range", b.seg, nq, rp.n_qtiles,
+  if (int rc = sweep(sim_range_kernel<false, false>, sim_range_kernel<true, false>, sim_range_kernel<false, false, true>))
+    return rc;
+  if (int rc = launch(range_slot_scan_kernel, (nq + 255) / 256, 256, 0, stream, who, b.seg, nq, rp.n_qtiles,
                       geo.n_gtiles, geo.gchunk, geo.n_chunks, rp.n_units, b.row_cnt, b.row_pcnt))
     return rc;
   if (int rc = exclusive_scan_i64(b.row_cnt, nq, b.row_cand, stream)) return rc;
@@ -419,25 +552,28 @@ int sim_range(const float* q, int nq, const float* g, int ng, int d, float thres
   counts[0] = 0;
   counts[1] = n_cand;
   if (n_cand > max_pairs)
-    return set_error(DCR_ERR_CAPACITY, "sim_range: %lld candidate pairs exceed max_pairs=%lld (call again with that capacity)",
-                     n_cand, max_pairs);
+    return set_error(DCR_ERR_CAPACITY, "%s: %lld candidate pairs exceed max_pairs=%lld (call again with that capacity)",
+                     who, n_cand, max_pairs);
 
   if (n_pieces > 0) {
-    if (int rc = sweep(sim_range_kernel<false, true>, sim_range_kernel<true, true>)) return rc;
-    if (int rc = launch(range_rescore_kernel, static_cast<unsigned>(n_pieces), kRescoreThreads, static_cast<size_t>(d) * 8,
-                        stream, "sim_range", q, g, nq, d, threshold, b.row_cand, b.row_piece, b.cand_idx, b.cand_score,
-                        b.piece_kept))
+    if (int rc = sweep(sim_range_kernel<false, true>, sim_range_kernel<true, true>, sim_range_kernel<false, true, true>))
+      return rc;
+    // split: the piece's running maxima, then one query part; dot product: the whole query row
+    const size_t rescore_smem = (n_parts ? static_cast<size_t>(kRangePiece) + pl : static_cast<size_t>(d)) * 8;
+    if (int rc = launch(n_parts ? range_rescore_kernel<true> : range_rescore_kernel<false>, static_cast<unsigned>(n_pieces),
+                        kRescoreThreads, rescore_smem, stream, who, q, g, nq, d, n_parts, threshold, b.row_cand,
+                        b.row_piece, b.cand_idx, b.cand_score, b.piece_kept))
       return rc;
   }
-  if (int rc = launch(exclusive_scan_kernel<int>, 1, 1024, 0, stream, "sim_range", b.piece_kept, n_pieces, b.piece_excl))
+  if (int rc = launch(exclusive_scan_kernel<int>, 1, 1024, 0, stream, who, b.piece_kept, n_pieces, b.piece_excl))
     return rc;
   if (n_pieces > 0) {
-    if (int rc = launch(range_output_kernel, static_cast<unsigned>(n_pieces), 256, 0, stream, "sim_range", b.row_cand,
+    if (int rc = launch(range_output_kernel, static_cast<unsigned>(n_pieces), 256, 0, stream, who, b.row_cand,
                         b.row_piece, nq, b.piece_excl, b.cand_idx, b.cand_score, g_index_base, g_index_stride, out_idx,
                         out_scores))
       return rc;
   }
-  if (int rc = launch(range_row_offsets_kernel, grid_for(nq + 1, 256, di->num_sms), 256, 0, stream, "sim_range", b.row_piece,
+  if (int rc = launch(range_row_offsets_kernel, grid_for(nq + 1, 256, di->num_sms), 256, 0, stream, who, b.row_piece,
                       b.piece_excl, nq, row_offsets))
     return rc;
   long long h_pairs = 0;
@@ -445,6 +581,37 @@ int sim_range(const float* q, int nq, const float* g, int ng, int d, float thres
   DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
   counts[0] = h_pairs;
   return 0;
+}
+
+}  // namespace
+
+size_t sim_range_workspace_size(int nq, int ng, int d, long long max_pairs) {
+  return range_workspace_size(nq, ng, d, 0, max_pairs);
+}
+
+int sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, long long g_index_base,
+              long long g_index_stride, long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,
+              long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  return range_search(q, nq, g, ng, d, 0, threshold, g_index_base, g_index_stride, row_offsets, out_idx, out_scores,
+                      max_pairs, counts, ws, ws_bytes, stream);
+}
+
+// one part is the dot product itself: the dot-product search, whose bits the split score must reproduce
+size_t sim_range_split_workspace_size(int nq, int ng, int d, int n_parts, long long max_pairs) {
+  if (n_parts < 1) {
+    set_error(-1, "sim_range_split: n_parts=%d < 1", n_parts);
+    return 0;
+  }
+  return range_workspace_size(nq, ng, d, n_parts == 1 ? 0 : n_parts, max_pairs);
+}
+
+int sim_range_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, float threshold,
+                    long long g_index_base, long long g_index_stride, long long* row_offsets, long long* out_idx,
+                    float* out_scores, long long max_pairs, long long* counts, void* ws, size_t ws_bytes,
+                    cudaStream_t stream) {
+  DCR_REQUIRE(n_parts >= 1, "sim_range_split: n_parts=%d < 1", n_parts);
+  return range_search(q, nq, g, ng, d, n_parts == 1 ? 0 : n_parts, threshold, g_index_base, g_index_stride, row_offsets,
+                      out_idx, out_scores, max_pairs, counts, ws, ws_bytes, stream);
 }
 
 int exclusive_scan_i64(const long long* in, long long n, long long* out, cudaStream_t stream) {

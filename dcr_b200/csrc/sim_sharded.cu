@@ -15,7 +15,9 @@
 //                       place in its row by binary search in the other ranks' pieces of that row.  No atomic decides an
 //                       order; a check pass before it refuses overlapping shards and malformed messages.
 // Every score is a function of its pair alone and the pieces are complete, so the merged rows are the rows sim_range
-// returns for the union of the shards.
+// returns for the union of the shards.  The split form (dcr_sim_range_split_sharded) runs sim_range_split as the local
+// search; the exchange and the merge are the same, and header word [9] carries n_parts so that ranks running different
+// searches disagree instead of merging.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -35,7 +37,7 @@ constexpr int kHdrWords = 10;                               // int64 words of a 
 constexpr long long kHdrMagic = 0x31474E52524344ll;         // "DCRRNG1" in memory
 constexpr int kMaxWorld = 65535;                            // ranks: the merge grid's y extent
 constexpr long long kMaxLocalPairs = 1ll << 40;             // as sim_range's max_pairs
-enum { H_MAGIC, H_STATUS, H_PAIRS, H_CAND, H_CAND_CAP, H_MAX_PAIRS, H_NQ, H_D, H_THR, H_RESERVED };
+enum { H_MAGIC, H_STATUS, H_PAIRS, H_CAND, H_CAND_CAP, H_MAX_PAIRS, H_NQ, H_D, H_THR, H_PARTS };
 
 // bytes of a message holding `pairs` pairs: int64 offsets[nq + 1], int64 idx[pairs], fp32 scores[pairs], 16-byte multiple
 inline size_t msg_bytes(int nq, long long pairs) {
@@ -55,12 +57,15 @@ struct ShardLayout {
   size_t total;
 };
 
-int shard_layout(int nq, int ng_local, int d, int world, long long cap, void* base, ShardLayout* L) {
-  DCR_REQUIRE(world >= 1 && world <= kMaxWorld, "sim_range_sharded: world=%d outside [1, %d]", world, kMaxWorld);
-  DCR_REQUIRE(nq >= 1 && ng_local >= 0, "sim_range_sharded: bad problem (nq=%d ng_local=%d)", nq, ng_local);
-  DCR_REQUIRE(cap >= 0 && cap <= kMaxLocalPairs, "sim_range_sharded: max_local_pairs=%lld outside [0, 2^40]", cap);
+// n_parts = 0: the dot product; >= 1: the split score (the local search is sim_range_split)
+int shard_layout(int nq, int ng_local, int d, int n_parts, int world, long long cap, void* base, ShardLayout* L) {
+  const char* who = n_parts ? "sim_range_split_sharded" : "sim_range_sharded";
+  DCR_REQUIRE(world >= 1 && world <= kMaxWorld, "%s: world=%d outside [1, %d]", who, world, kMaxWorld);
+  DCR_REQUIRE(nq >= 1 && ng_local >= 0, "%s: bad problem (nq=%d ng_local=%d)", who, nq, ng_local);
+  DCR_REQUIRE(cap >= 0 && cap <= kMaxLocalPairs, "%s: max_local_pairs=%lld outside [0, 2^40]", who, cap);
   // an empty shard runs no search, but its d is still checked by the same planner
-  L->inner = sim_range_workspace_size(nq, ng_local > 0 ? ng_local : 1, d, cap);
+  const int ng_plan = ng_local > 0 ? ng_local : 1;
+  L->inner = n_parts ? sim_range_split_workspace_size(nq, ng_plan, d, n_parts, cap) : sim_range_workspace_size(nq, ng_plan, d, cap);
   if (L->inner == 0) return -1;
   if (ng_local == 0) L->inner = 0;
   const size_t msg = msg_bytes(nq, cap);
@@ -250,35 +255,36 @@ int sim_topk_sharded(const float* q, int nq, const float* g, int ng_local, int d
   return topk_merge(L.all_s, L.all_i, nq, world, k, k, out_scores, out_idx, stream);
 }
 
-size_t sim_range_sharded_workspace_size(int nq, int ng_local, int d, int world, long long max_local_pairs) {
-  ShardLayout L;
-  if (shard_layout(nq, ng_local, d, world, max_local_pairs, nullptr, &L) != 0) return 0;
-  return L.total;
-}
+namespace {
 
-int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int d, float threshold, long long g_index_base,
-                      long long g_index_stride, int world, AllgatherFn allgather, void* allgather_ctx, long long* row_offsets,
-                      long long* out_idx, float* out_scores, long long max_pairs, long long max_local_pairs,
-                      long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
+// The sharded threshold search.  split = false: the dot product (n_parts unused, header word [9] = 0); true: the split
+// score over n_parts parts, one part being the dot product itself (word [9] = 0 then too).
+int range_sharded(const float* q, int nq, const float* g, int ng_local, int d, bool split, int n_parts, float threshold,
+                  long long g_index_base, long long g_index_stride, int world, AllgatherFn allgather, void* allgather_ctx,
+                  long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,
+                  long long max_local_pairs, long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  const char* who = split ? "sim_range_split_sharded" : "sim_range_sharded";
+  const int parts = split && n_parts > 1 ? n_parts : 0;
   // the only outcomes decided before the first exchange: without these there is nobody to agree with
-  DCR_REQUIRE(world >= 1 && world <= kMaxWorld, "sim_range_sharded: world=%d outside [1, %d]", world, kMaxWorld);
-  DCR_REQUIRE(world == 1 || allgather != nullptr, "sim_range_sharded: world=%d needs an all-gather callback", world);
+  DCR_REQUIRE(world >= 1 && world <= kMaxWorld, "%s: world=%d outside [1, %d]", who, world, kMaxWorld);
+  DCR_REQUIRE(world == 1 || allgather != nullptr, "%s: world=%d needs an all-gather callback", who, world);
 
   // 1. the local search; its outcome goes into the header, whatever it is
   uint32_t thr_bits;
   std::memcpy(&thr_bits, &threshold, 4);
-  long long hdr[kHdrWords] = {kHdrMagic, 0, 0, 0, max_local_pairs, max_pairs, nq, d, static_cast<long long>(thr_bits), 0};
+  long long hdr[kHdrWords] = {kHdrMagic, 0, 0, 0, max_local_pairs, max_pairs, nq, d, static_cast<long long>(thr_bits), parts};
   ShardLayout L{};
   uint8_t* w = static_cast<uint8_t*>(ws);
   auto local = [&]() -> int {
     DCR_REQUIRE(q && (g || ng_local == 0) && row_offsets && counts && (max_pairs == 0 || (out_idx && out_scores)),
-                "sim_range_sharded: null pointer argument");
-    DCR_REQUIRE(!std::isnan(threshold), "sim_range_sharded: threshold is NaN");
-    DCR_REQUIRE(g_index_stride >= 1, "sim_range_sharded: g_index_stride=%lld < 1", g_index_stride);
-    DCR_REQUIRE(max_pairs >= 0, "sim_range_sharded: max_pairs=%lld < 0", max_pairs);
-    if (int rc = shard_layout(nq, ng_local, d, world, max_local_pairs, w, &L)) return rc;
-    DCR_REQUIRE(w != nullptr && ws_bytes >= L.total, "sim_range_sharded: workspace too small (%zu < %zu)", ws_bytes, L.total);
-    DCR_REQUIRE((reinterpret_cast<uintptr_t>(w) & 255) == 0, "sim_range_sharded: workspace must be 256-byte aligned");
+                "%s: null pointer argument", who);
+    DCR_REQUIRE(!split || n_parts >= 1, "%s: n_parts=%d < 1", who, n_parts);
+    DCR_REQUIRE(!std::isnan(threshold), "%s: threshold is NaN", who);
+    DCR_REQUIRE(g_index_stride >= 1, "%s: g_index_stride=%lld < 1", who, g_index_stride);
+    DCR_REQUIRE(max_pairs >= 0, "%s: max_pairs=%lld < 0", who, max_pairs);
+    if (int rc = shard_layout(nq, ng_local, d, parts, world, max_local_pairs, w, &L)) return rc;
+    DCR_REQUIRE(w != nullptr && ws_bytes >= L.total, "%s: workspace too small (%zu < %zu)", who, ws_bytes, L.total);
+    DCR_REQUIRE((reinterpret_cast<uintptr_t>(w) & 255) == 0, "%s: workspace must be 256-byte aligned", who);
     long long* send_off = reinterpret_cast<long long*>(L.send);
     if (ng_local == 0) {
       DCR_CUDA_CHECK(cudaMemsetAsync(send_off, 0, 8 * (static_cast<size_t>(nq) + 1), stream));
@@ -289,8 +295,10 @@ int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int 
     long long* send_idx = send_off + nq + 1;
     float* tmp_scores = reinterpret_cast<float*>(L.recv);
     long long c[2] = {0, 0};
-    const int rc = sim_range(q, nq, g, ng_local, d, threshold, g_index_base, g_index_stride, send_off, send_idx, tmp_scores,
-                             max_local_pairs, c, L.inner_ws, L.inner, stream);
+    const int rc = parts ? sim_range_split(q, nq, g, ng_local, d, parts, threshold, g_index_base, g_index_stride, send_off,
+                                           send_idx, tmp_scores, max_local_pairs, c, L.inner_ws, L.inner, stream)
+                         : sim_range(q, nq, g, ng_local, d, threshold, g_index_base, g_index_stride, send_off, send_idx,
+                                     tmp_scores, max_local_pairs, c, L.inner_ws, L.inner, stream);
     hdr[H_CAND] = c[1];
     if (rc) return rc;
     hdr[H_PAIRS] = c[0];
@@ -315,25 +323,29 @@ int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int 
   long long* h_send = hb.p;
   long long* h_recv = hb.p + kHdrWords;
   DCR_CUDA_CHECK(cudaMemcpyAsync(h_send, hdr, hbytes, cudaMemcpyHostToDevice, stream));
-  if (int rc = allgather_step("sim_range_sharded", world, allgather, allgather_ctx, h_send, h_recv, hbytes, stream)) return rc;
+  if (int rc = allgather_step(who, world, allgather, allgather_ctx, h_send, h_recv, hbytes, stream)) return rc;
   std::vector<long long> H(static_cast<size_t>(world) * kHdrWords);
   DCR_CUDA_CHECK(cudaMemcpyAsync(H.data(), h_recv, hbytes * world, cudaMemcpyDeviceToHost, stream));
   DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
   auto h = [&](int r, int f) { return H[static_cast<size_t>(r) * kHdrWords + f]; };
   if (counts) counts[0] = counts[1] = counts[2] = 0;
   for (int r = 0; r < world; ++r)
-    DCR_REQUIRE(h(r, H_MAGIC) == kHdrMagic, "sim_range_sharded: rank %d sent a malformed header", r);
+    DCR_REQUIRE(h(r, H_MAGIC) == kHdrMagic, "%s: rank %d sent a malformed header", who, r);
   for (int r = 0; r < world; ++r) {
     const long long st = h(r, H_STATUS);
     if (st != 0 && st != DCR_ERR_CAPACITY)
-      return set_error(static_cast<int>(st), "sim_range_sharded: rank %d failed (%lld)%s%s", r, st,
+      return set_error(static_cast<int>(st), "%s: rank %d failed (%lld)%s%s", who, r, st,
                        local_rc ? "; this rank: " : "", local_msg.c_str());
   }
   for (int r = 1; r < world; ++r)
     DCR_REQUIRE(h(r, H_NQ) == h(0, H_NQ) && h(r, H_D) == h(0, H_D) && h(r, H_THR) == h(0, H_THR),
-                "sim_range_sharded: ranks disagree on the problem: rank 0 has nq=%lld d=%lld threshold bits 0x%llx, rank %d "
+                "%s: ranks disagree on the problem: rank 0 has nq=%lld d=%lld threshold bits 0x%llx, rank %d "
                 "has nq=%lld d=%lld threshold bits 0x%llx",
-                h(0, H_NQ), h(0, H_D), h(0, H_THR), r, h(r, H_NQ), h(r, H_D), h(r, H_THR));
+                who, h(0, H_NQ), h(0, H_D), h(0, H_THR), r, h(r, H_NQ), h(r, H_D), h(r, H_THR));
+  for (int r = 1; r < world; ++r)
+    DCR_REQUIRE(h(r, H_PARTS) == h(0, H_PARTS),
+                "%s: ranks disagree on the score: rank 0 has n_parts=%lld, rank %d has n_parts=%lld (0: the dot product)",
+                who, h(0, H_PARTS), r, h(r, H_PARTS));
   // capacities: every local search finished, every receive buffer holds the largest message, every output the total
   bool finished = true;
   long long cand_need = 0, p_max = 0, total = 0, min_cap = h(0, H_CAND_CAP), min_out = h(0, H_MAX_PAIRS);
@@ -350,12 +362,12 @@ int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int 
   counts[2] = total;
   if (!finished || p_max > min_cap || total > min_out)
     return set_error(DCR_ERR_CAPACITY,
-                     "sim_range_sharded: capacity too small on some rank (call again with max_local_pairs=%lld, "
-                     "max_pairs=%lld on every rank)", cand_need, total);
+                     "%s: capacity too small on some rank (call again with max_local_pairs=%lld, "
+                     "max_pairs=%lld on every rank)", who, cand_need, total);
 
   // 3. the messages, each padded to the largest
   const size_t msg = msg_bytes(nq, p_max);
-  if (int rc = allgather_step("sim_range_sharded", world, allgather, allgather_ctx, L.send, L.recv, msg, stream)) return rc;
+  if (int rc = allgather_step(who, world, allgather, allgather_ctx, L.send, L.recv, msg, stream)) return rc;
 
   // 4. the merge
   const DeviceInfo* di = device_info();
@@ -366,28 +378,63 @@ int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int 
   const dim3 grid(static_cast<unsigned>(std::max(1, grid_for(std::max(p_max, 1ll), 256, di->num_sms) / world)),
                   static_cast<unsigned>(world));
   DCR_CUDA_CHECK(cudaMemsetAsync(bad, 0, 4, stream));
-  if (int rc = launch(shard_row_count_kernel, grid_for(nq, 256, di->num_sms), 256, 0, stream, "sim_range_sharded", m, row_cnt,
-                      bad))
+  if (int rc = launch(shard_row_count_kernel, grid_for(nq, 256, di->num_sms), 256, 0, stream, who, m, row_cnt, bad))
     return rc;
   if (p_max > 0) {
-    if (int rc = launch(shard_merge_kernel<false>, grid, 256, 0, stream, "sim_range_sharded", m, nullptr, nullptr, nullptr, bad))
+    if (int rc = launch(shard_merge_kernel<false>, grid, 256, 0, stream, who, m, nullptr, nullptr, nullptr, bad))
       return rc;
   }
   int h_bad = 0;
   DCR_CUDA_CHECK(cudaMemcpyAsync(&h_bad, bad, 4, cudaMemcpyDeviceToHost, stream));
   DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
   DCR_REQUIRE(h_bad == 0,
-              "sim_range_sharded: two ranks report the same gallery index (the shards overlap), or a rank's message is "
-              "not an ascending CSR of its pairs");
+              "%s: two ranks report the same gallery index (the shards overlap), or a rank's message is "
+              "not an ascending CSR of its pairs", who);
   if (int rc = exclusive_scan_i64(row_cnt, nq, row_offsets, stream)) return rc;
   if (p_max > 0) {
-    if (int rc = launch(shard_merge_kernel<true>, grid, 256, 0, stream, "sim_range_sharded", m, row_offsets, out_idx, out_scores,
-                        bad))
+    if (int rc = launch(shard_merge_kernel<true>, grid, 256, 0, stream, who, m, row_offsets, out_idx, out_scores, bad))
       return rc;
   }
   DCR_CUDA_CHECK(cudaStreamSynchronize(stream));
   counts[0] = total;
   return 0;
+}
+
+}  // namespace
+
+size_t sim_range_sharded_workspace_size(int nq, int ng_local, int d, int world, long long max_local_pairs) {
+  ShardLayout L;
+  if (shard_layout(nq, ng_local, d, 0, world, max_local_pairs, nullptr, &L) != 0) return 0;
+  return L.total;
+}
+
+int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int d, float threshold, long long g_index_base,
+                      long long g_index_stride, int world, AllgatherFn allgather, void* allgather_ctx, long long* row_offsets,
+                      long long* out_idx, float* out_scores, long long max_pairs, long long max_local_pairs,
+                      long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  return range_sharded(q, nq, g, ng_local, d, false, 0, threshold, g_index_base, g_index_stride, world, allgather,
+                       allgather_ctx, row_offsets, out_idx, out_scores, max_pairs, max_local_pairs, counts, ws, ws_bytes,
+                       stream);
+}
+
+size_t sim_range_split_sharded_workspace_size(int nq, int ng_local, int d, int n_parts, int world, long long max_local_pairs) {
+  if (n_parts < 1) {
+    set_error(-1, "sim_range_split_sharded: n_parts=%d < 1", n_parts);
+    return 0;
+  }
+  ShardLayout L;
+  if (shard_layout(nq, ng_local, d, n_parts == 1 ? 0 : n_parts, world, max_local_pairs, nullptr, &L) != 0) return 0;
+  return L.total;
+}
+
+int sim_range_split_sharded(const float* q, int nq, const float* g, int ng_local, int d, int n_parts, float threshold,
+                            long long g_index_base, long long g_index_stride, int world, AllgatherFn allgather,
+                            void* allgather_ctx, long long* row_offsets, long long* out_idx, float* out_scores,
+                            long long max_pairs, long long max_local_pairs, long long* counts, void* ws, size_t ws_bytes,
+                            cudaStream_t stream) {
+  return range_sharded(q, nq, g, ng_local, d, true, n_parts, threshold, g_index_base, g_index_stride, world, allgather,
+                       allgather_ctx, row_offsets, out_idx, out_scores, max_pairs, max_local_pairs, counts, ws, ws_bytes,
+                       stream);
 }
 
 }  // namespace dcr

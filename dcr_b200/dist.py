@@ -177,8 +177,8 @@ def _allgather_callback(allgather: Optional[Callable], world: int, device: torch
 
 
 def sharded_range(query_all: torch.Tensor, gallery_local: torch.Tensor, threshold: float, gallery_base: int, *,
-                  allgather: Optional[Callable] = None, world: Optional[int] = None, index_stride: int = 1
-                  ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                  allgather: Optional[Callable] = None, world: Optional[int] = None, index_stride: int = 1,
+                  num_chunks: int = 1) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """Threshold search over a gallery sharded across ranks, through the C entry `dcr_sim_range_sharded`
     (include/dcr_b200.h): every rank searches ALL queries against its shard (global index of local row j =
     gallery_base + index_stride * j), the CSR pieces are exchanged and merged on the device, and every rank returns
@@ -186,7 +186,9 @@ def sharded_range(query_all: torch.Tensor, gallery_local: torch.Tensor, threshol
     the shards.  `query_all`: every query descriptor (a query-sharded caller all-gathers them first with
     all_gather_rows).  `gallery_local` may have 0 rows; that rank still takes part in the exchanges.  `allgather` as in
     sharded_topk_c (default: torch.distributed.all_gather_into_tensor).  The capacities start where sim_range's do; when
-    some rank needs more, every rank gets DCR_ERR_CAPACITY with the needs and retries once, together."""
+    some rank needs more, every rank gets DCR_ERR_CAPACITY with the needs and retries once, together.
+    num_chunks > 1: the 'splitloss' score over that many aligned parts (`dcr_sim_range_split_sharded`), bit for bit
+    what similarity.sim_range_split returns for the union of the shards."""
     import ctypes as C
     from . import _lib
     from .similarity import _aligned_ptr, _check_cuda_f32
@@ -202,29 +204,38 @@ def sharded_range(query_all: torch.Tensor, gallery_local: torch.Tensor, threshol
     g_ok = g.shape[1] == d and g.device == q.device
     g_ptr = (g.data_ptr() if ng > 0 else None) if g_ok else None
     cb = _allgather_callback(allgather, world, q.device, "sharded_range")
+    split = num_chunks > 1
+    what = "dcr_sim_range_split_sharded" if split else "dcr_sim_range_sharded"
     counts = (C.c_int64 * 3)()
     local_cap = out_cap = max(1 << 20, 16 * nq)   # sim_range's start; the exact needs come back with ERR_CAPACITY
     with torch.cuda.device(q.device):
         offsets = torch.empty(nq + 1, dtype=torch.int64, device=q.device)
         for attempt in range(2):
             # 0 (invalid arguments) is passed on: the library reports the reason on every rank
-            nbytes = lib.dcr_sim_range_sharded_workspace_size(nq, ng if g_ok else 1, d, world, local_cap)
+            if split:
+                nbytes = lib.dcr_sim_range_split_sharded_workspace_size(nq, ng if g_ok else 1, d, num_chunks, world,
+                                                                        local_cap)
+            else:
+                nbytes = lib.dcr_sim_range_sharded_workspace_size(nq, ng if g_ok else 1, d, world, local_cap)
             ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=q.device) if nbytes else None
             out_i = torch.empty(out_cap, dtype=torch.int64, device=q.device)
             out_s = torch.empty(out_cap, dtype=torch.float32, device=q.device)
             st = torch.cuda.current_stream().cuda_stream
-            rc = lib.dcr_sim_range_sharded(q.data_ptr(), nq, g_ptr, ng if g_ok else 1, d, float(threshold),
-                                           gallery_base, index_stride, world, C.cast(cb, C.c_void_p), None,
-                                           offsets.data_ptr(), out_i.data_ptr() or None, out_s.data_ptr() or None,
-                                           out_cap, local_cap, counts, _aligned_ptr(ws) if ws is not None else None,
-                                           nbytes, st)
+            args = (gallery_base, index_stride, world, C.cast(cb, C.c_void_p), None, offsets.data_ptr(),
+                    out_i.data_ptr() or None, out_s.data_ptr() or None, out_cap, local_cap, counts,
+                    _aligned_ptr(ws) if ws is not None else None, nbytes, st)
+            if split:
+                rc = lib.dcr_sim_range_split_sharded(q.data_ptr(), nq, g_ptr, ng if g_ok else 1, d, num_chunks,
+                                                     float(threshold), *args)
+            else:
+                rc = lib.dcr_sim_range_sharded(q.data_ptr(), nq, g_ptr, ng if g_ok else 1, d, float(threshold), *args)
             if rc == _lib.ERR_CAPACITY and attempt == 0:
                 local_cap, out_cap = int(counts[1]), int(counts[2])   # agreed by every rank: all retry together
                 continue
             if rc != 0 and not g_ok:
-                raise _lib.DcrError(f"dcr_sim_range_sharded: gallery_local {tuple(g.shape)} on {g.device} does not "
+                raise _lib.DcrError(f"{what}: gallery_local {tuple(g.shape)} on {g.device} does not "
                                     f"match query_all {tuple(q.shape)} on {q.device} ({_lib.last_error()})")
-            _lib.check(rc, "dcr_sim_range_sharded")
+            _lib.check(rc, what)
             break
     n = int(counts[0])
     if n < out_cap:   # do not keep the whole capacity alive behind the result

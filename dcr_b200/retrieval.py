@@ -19,7 +19,7 @@ import torch
 
 from . import _lib
 from .nets import DcrNet
-from .similarity import l2_normalize_, sim_range, sim_topk, sim_topk_split
+from .similarity import l2_normalize_, sim_range, sim_range_split, sim_topk, sim_topk_split
 
 
 @torch.no_grad()
@@ -148,9 +148,11 @@ def run_retrieval(net: DcrNet, query_images: torch.Tensor, gallery_images: torch
     """Embed both image sets and match them (the rank-0 block of diff_retrieval.py:386-419).  With a threshold, also
     every pair scoring at least that much (sim_range, CSR): out["matches"] (query x gallery, the entries of the
     reference's similarity.pth, :402, :414) and, with the background, out["bg_matches"] (the gallery self-join, diagonal
-    included, as similarity_wtrain.pth, :403, :415).  Dot-product metric only."""
-    if threshold is not None and num_loss_chunks > 1:
-        raise NotImplementedError("a similarity threshold is implemented for the dot-product metric only")
+    included, as similarity_wtrain.pth, :403, :415).  With num_loss_chunks = C > 1 (the aligned 'splitloss' score)
+    out["matches"] comes from sim_range_split, the entries of the splitloss similarity.pth (:393-400, :411, :414); the
+    cross form has no threshold search."""
+    if threshold is not None and num_loss_chunks > 1 and cross:
+        raise NotImplementedError("a similarity threshold is not implemented for the cross form of the split score")
     if isinstance(net, (list, tuple)):                                      # multiscale=args.multiscale (:386-387)
         values_features = extract_features_multiscale(net, gallery_images, batch_size)
         query_features = extract_features_multiscale(net, query_images, batch_size)
@@ -171,7 +173,10 @@ def run_retrieval(net: DcrNet, query_images: torch.Tensor, gallery_images: torch
         bg_v = bg[:, -1]                                                      # :419
         out["bg_values"] = bg_v
     if threshold is not None:
-        out["matches"] = sim_range(query_features, values_features, threshold)
+        if num_loss_chunks > 1:
+            out["matches"] = sim_range_split(query_features, values_features, threshold, num_loss_chunks)
+        else:
+            out["matches"] = sim_range(query_features, values_features, threshold)
         if with_background:
             out["bg_matches"] = sim_range(values_features, values_features, threshold)
     out["stats"] = retrieval_stats(main_v[:, 0], bg_v)

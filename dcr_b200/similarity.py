@@ -11,6 +11,7 @@ The reference has no function boundary here -- it is inline tensor code in `main
 `sim_topk(query, gallery, k)` returns exactly what `torch.mm(gallery, query.T).T.topk(k, dim=1)` would (values,
 indices), with a defined tie rule (lowest gallery index first) and without materialising the [Q,G] matrix.
 `sim_range(query, gallery, threshold)` returns the entries of that matrix that reach a threshold, as CSR.
+`sim_topk_split` and `sim_range_split` do the same under the 'splitloss' score (the best of the descriptor parts).
 All compute happens in libdcr_b200.so on the tensors' CUDA device.
 """
 from __future__ import annotations
@@ -125,6 +126,52 @@ def sim_range(query: torch.Tensor, gallery: torch.Tensor, threshold: float, *, i
                 cap = int(counts[1])   # the candidate count is a fixed function of the inputs: this capacity fits
                 continue
             _lib.check(rc, "dcr_sim_range")
+            break
+    n = int(counts[0])
+    if n < cap:   # do not keep the whole capacity alive behind the result
+        out_i, out_s = out_i[:n].clone(), out_s[:n].clone()
+    return offsets, out_i, out_s
+
+
+def sim_range_split(query: torch.Tensor, gallery: torch.Tensor, threshold: float, num_chunks: int, *,
+                    index_base: int = 0, index_stride: int = 1) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Every (query i, gallery j) pair whose 'splitloss' score (diff_retrieval.py:393-400, aligned parts) reaches the
+    threshold, in sim_range's CSR form: (offsets i64[Q+1], indices i64[P], scores f32[P]).  The score is
+    max_c <q_c, g_c> over the C = num_chunks equal parts, bit for bit what sim_topk_split reports for the same pair; a
+    NaN part is ignored, a pair whose parts are all NaN scores -inf, threshold = -inf reports every pair.  Part length
+    p = D/C a multiple of 4 and at most 8192; num_chunks = 1 is sim_range.  Replaces the splitloss similarity.pth
+    (:411, :414) without the [G, Q, C] tensor of its einsum (dcr_sim_range_split)."""
+    lib = _lib.load()
+    q = _check_cuda_f32("query", query)
+    g = _check_cuda_f32("gallery", gallery)
+    if q.device != g.device:
+        raise _lib.DcrError("query and gallery must be on the same device")
+    if q.shape[1] != g.shape[1]:
+        raise _lib.DcrError(f"descriptor dims differ: {q.shape[1]} vs {g.shape[1]}")
+    threshold = float(threshold)
+    if math.isnan(threshold):
+        raise _lib.DcrError("sim_range_split: threshold is NaN")
+    nq, d = q.shape
+    ng = g.shape[0]
+    counts = (C.c_int64 * 2)()
+    cap = max(1 << 20, 16 * nq)   # sim_range's start; the exact need is known after the counting pass
+    with torch.cuda.device(q.device):
+        offsets = torch.empty(nq + 1, dtype=torch.int64, device=q.device)
+        for attempt in range(2):
+            nbytes = lib.dcr_sim_range_split_workspace_size(nq, ng, d, num_chunks, cap)
+            if nbytes == 0:
+                raise _lib.DcrError(f"dcr_sim_range_split_workspace_size: {_lib.last_error()}")
+            ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=q.device)
+            out_i = torch.empty(cap, dtype=torch.int64, device=q.device)
+            out_s = torch.empty(cap, dtype=torch.float32, device=q.device)
+            st = torch.cuda.current_stream().cuda_stream
+            rc = lib.dcr_sim_range_split(q.data_ptr(), nq, g.data_ptr(), ng, d, num_chunks, threshold, index_base,
+                                         index_stride, offsets.data_ptr(), out_i.data_ptr(), out_s.data_ptr(), cap,
+                                         counts, _aligned_ptr(ws), nbytes, st)
+            if rc == _lib.ERR_CAPACITY and attempt == 0:
+                cap = int(counts[1])   # the candidate count is a fixed function of the inputs: this capacity fits
+                continue
+            _lib.check(rc, "dcr_sim_range_split")
             break
     n = int(counts[0])
     if n < cap:   # do not keep the whole capacity alive behind the result

@@ -168,7 +168,7 @@ int dcr_sim_range(const float* q, int nq, const float* g, int ng, int d, float t
  * int64 words):
  *     [0] 0x31474E52524344 ("DCRRNG1" in memory)   [1] status: 0, DCR_ERR_CAPACITY or the code of a local failure
  *     [2] local pairs   [3] local candidates (the max_local_pairs its search needs)   [4] max_local_pairs   [5] max_pairs
- *     [6] nq   [7] d   [8] the threshold's fp32 bits   [9] 0
+ *     [6] nq   [7] d   [8] the threshold's fp32 bits   [9] n_parts: 0 here (dcr_sim_range_split_sharded writes its own)
  * so every rank returns the same code:
  *   - a local failure on any rank (bad argument, workspace too small, CUDA error): that rank's code on every rank
  *   - headers that disagree on nq, d or the threshold: -1
@@ -198,6 +198,41 @@ int dcr_sim_range_sharded(const float* q, int nq, const float* g, int ng_local, 
                           int64_t g_index_base, int64_t g_index_stride, int world, dcr_allgather_fn allgather,
                           void* allgather_ctx, int64_t* row_offsets, int64_t* out_idx, float* out_scores, int64_t max_pairs,
                           int64_t max_local_pairs, int64_t* counts, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Threshold search under the 'splitloss' similarity (diff_retrieval.py:393-400): for every query row i, every gallery row
+ * j whose split score s_ij >= threshold.  The descriptors are cut into n_parts equal parts of p = d / n_parts values and
+ * s_ij is max over c of the fp64-accumulated part dot products, folded with fmax from -inf in part order and rounded to
+ * fp32: bit for bit what dcr_split_rescore and dcr_sim_topk_split report for the same pair.  A NaN part is ignored; a pair
+ * whose parts are all NaN scores -inf.  threshold = -inf reports all nq * ng pairs; a NaN threshold is an error.  Exact and
+ * the same bits on every call.  One fused tensor-core sweep whose epilogue compares the maximum over the parts with a
+ * per-row threshold no qualifying pair falls below, then the exact re-score of the candidates, one part at a time.
+ * q[nq,d], g[ng,d]: device, fp32, 16-byte aligned; d % n_parts == 0, p % 4 == 0, p <= 8192 (no limit on d or n_parts).
+ * Output, counts, capacity and DCR_ERR_CAPACITY as dcr_sim_range.  n_parts = 1 returns the bits of dcr_sim_range.  The
+ * workspace (dcr_sim_range_split_workspace_size) grows with (nq + ng) * d and max_pairs, never with nq * ng.
+ * Replaces   sim = einsum('ncp,mcp->nmc', values, query).max(dim=2)        diff_retrieval.py:393-400 (splitloss branch)
+ *            torch.save(sim, 'similarity.pth')                             diff_retrieval.py:411, 414
+ * without the [G, Q, C] tensor the einsum materialises. */
+size_t dcr_sim_range_split_workspace_size(int nq, int ng, int d, int n_parts, int64_t max_pairs);
+int dcr_sim_range_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, float threshold,
+                        int64_t g_index_base, int64_t g_index_stride, int64_t* row_offsets, int64_t* out_idx,
+                        float* out_scores, int64_t max_pairs, int64_t* counts, void* workspace, size_t workspace_bytes,
+                        void* stream);
+
+/* Gallery-sharded form of dcr_sim_range_split: dcr_sim_range_sharded with dcr_sim_range_split as the local search.  The
+ * exchange, the agreement rules, the messages and the merge are those of dcr_sim_range_sharded, with header word [9] =
+ * n_parts (0 for n_parts = 1, the dot product, so such a rank agrees with a dcr_sim_range_sharded peer); headers that
+ * disagree on it return -1 on every rank, like nq, d and the threshold.  On success every rank holds the CSR
+ * dcr_sim_range_split returns for the same queries against the union of the shards, bit for bit.  The split form of the
+ * reference's splitloss similarity.pth (diff_retrieval.py:393-400, 411, 414) for a gallery spread over ranks.
+ * workspace: dcr_sim_range_split_sharded_workspace_size(nq, ng_local, d, n_parts, world, max_local_pairs) bytes, laid out
+ * as dcr_sim_range_sharded's around the split local search. */
+size_t dcr_sim_range_split_sharded_workspace_size(int nq, int ng_local, int d, int n_parts, int world,
+                                                  int64_t max_local_pairs);
+int dcr_sim_range_split_sharded(const float* q, int nq, const float* g, int ng_local, int d, int n_parts, float threshold,
+                                int64_t g_index_base, int64_t g_index_stride, int world, dcr_allgather_fn allgather,
+                                void* allgather_ctx, int64_t* row_offsets, int64_t* out_idx, float* out_scores,
+                                int64_t max_pairs, int64_t max_local_pairs, int64_t* counts, void* workspace,
+                                size_t workspace_bytes, void* stream);
 
 /* ---- dense contraction of the descriptor networks ------------------------------------------------------------- */
 /* y = act(scale[n] * conv2d(x, w)[.., n] + bias[n] (+ residual)) as a wgmma implicit GEMM.
