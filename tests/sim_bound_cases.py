@@ -27,7 +27,6 @@ from __future__ import annotations
 from dataclasses import dataclass, field
 
 import numpy as np
-import torch
 
 U = 2.0 ** -11          # the gallery's quantum
 SEG = 64                # the target and its competitors sit in the first 64 columns of a 128-row tile: one segment
@@ -37,8 +36,11 @@ KP1 = 32                             # candidates of the second-chance pass
 
 
 def bf16(x: np.ndarray) -> np.ndarray:
-    """Round-to-nearest-even fp32 -> bf16, back in fp32 (torch's conversion is RNE, as __float2bfloat16_rn)."""
-    return torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).to(torch.bfloat16).float().numpy()
+    """Round-to-nearest-even fp32 -> bf16, back in fp32, as __float2bfloat16_rn (finite values): add half a bf16 ulp
+    less one, plus the kept lsb, to the bits and cut the low 16."""
+    b = np.ascontiguousarray(x, dtype=np.float32).view(np.uint32)
+    assert np.isfinite(x).all()
+    return ((b + np.uint32(0x7FFF) + ((b >> 16) & np.uint32(1))) & np.uint32(0xFFFF0000)).view(np.float32)
 
 
 def _levels(d: int):
@@ -271,3 +273,156 @@ TOPK_CASES = [
 def topk_case(name: str, d: int, centred: bool) -> Case:
     _, k, n_b, shared, tie, _ = next(c for c in TOPK_CASES if c[0] == name)
     return build(d, n_b, centred=centred, shared=shared, tie=tie)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# The split score: an instance in one descriptor part
+#
+# sim_topk_split and sim_range_split rank on the maximum over the parts of per-part bf16 scores and trust split_row_bound
+# (sim_sweep.cuh): the largest over the parts of row_bound's expression, from each part's own query norms
+# (q_norm_*[qrow * n_parts + c]) and gallery maxima (g_max[2c], g_max[2c + 1]).  The instances below put a build()
+# instance (uncentred, its d becoming the part length p) into one part of n_parts:
+#
+# - quiet: every other part of the query is zero and every other part of the gallery holds tiny values x*2^-11
+#   (|x| <= 3, bf16-exact).  Those parts score exactly 0 and contribute nothing to eps, so eps comes from the instance
+#   part alone: a bound read from another part's norms or gallery maxima, or one that never visits the instance part,
+#   collapses below A's realized error and lets the bf16 order through.
+# - cross: A (and its twin) reach their scores in part `part`, the competitors in part `other`; the query holds +-w in
+#   both, and a row's part that does not hold its instance holds a +-1 filler.  The running maximum over the parts then
+#   decides every pair from a different part for A than for its competitors.
+
+SPLIT_SHAPES = ((2, 64), (4, 516), (3, 1024), (40, 64), (197, 64))   # (n_parts, p); 516 pads to 576
+RANGE_SPLIT_SHAPES = SPLIT_SHAPES + ((2, 256), (4, 64))              # d_pad <= 512: resident query tile
+
+
+def split_placements(n_parts: int):
+    """(layout, part, other) of every placement a shape is tested at.  quiet: the first part, the second, the last, and
+    33 (the second lane round of split_row_bound's part loop) when there is one; cross: A in the first part and the
+    competitors in the last, the reverse, and A in part 33 against competitors in part 1."""
+    quiet = sorted({0, 1, n_parts - 1} | ({33} if n_parts > 33 else set()))
+    cross = [(0, n_parts - 1), (n_parts - 1, 0)] + ([(33, 1)] if n_parts > 33 else [])
+    return [("quiet", c, -1) for c in quiet] + [("cross", c, o) for c, o in cross]
+
+
+def _mirror_set(g: np.ndarray, cols: slice, rows, rng):
+    """Fresh +-1 fillers in part `cols` of rows `rows` of X and, negated, of their mirrors in -X."""
+    n_x = g.shape[0] // 2
+    for r in sorted({int(r) % n_x for r in rows}):
+        f = _filler(cols.stop - cols.start, rng)
+        g[r, cols], g[r + n_x, cols] = f, -f
+
+
+def split_embed(case: Case, n_parts: int, part: int, layout: str = "quiet", other: int = -1, seed: int = 0) -> Case:
+    """`case` (uncentred, of dimension p) put into part `part` of n_parts; see above for the layouts."""
+    assert not case.centred and 0 <= part < n_parts
+    nq, p = case.q.shape
+    ng = case.g.shape[0]
+    rng = np.random.default_rng(seed + 1009 * n_parts + 17 * part)
+    q = np.zeros((nq, n_parts * p), np.float32)
+    g = (rng.integers(-3, 4, size=(ng, n_parts * p)) * U).astype(np.float32)
+    at = slice(part * p, (part + 1) * p)
+    q[:, at] = case.q
+    g[:, at] = case.g
+    if layout == "cross":
+        assert 0 <= other < n_parts and other != part
+        to = slice(other * p, (other + 1) * p)
+        q[:, to] = case.q
+        g[:, to] = case.g
+        _mirror_set(g, at, np.concatenate(case.comps), rng)                                    # B scores in `other` only
+        _mirror_set(g, to, np.concatenate([case.target, case.twin[case.twin >= 0]]), rng)     # A, twin in `part` only
+    else:
+        assert layout == "quiet"
+    return Case(q=q, g=g, centred=False, target=case.target, comps=case.comps, twin=case.twin,
+                info=dict(case.info, n_parts=n_parts, p=p, part=part, layout=layout, other=other))
+
+
+def split_case(name: str, p: int, n_parts: int, part: int, layout: str = "quiet", other: int = -1, **build_kw) -> Case:
+    """A TOPK_CASES instance (by name), or with name "range" the threshold-search instance build(p, 20, **build_kw)
+    (tie=, scales=), in part `part` of n_parts."""
+    base = build(p, 20, centred=False, **build_kw) if name == "range" else topk_case(name, p, False)
+    return split_embed(base, n_parts, part, layout, other)
+
+
+def second_half(case: Case) -> Case:
+    """The competitors moved from columns 0-63 of their 128-row tile to columns 64-127 (swapped with fillers), in X and
+    -X alike: the two column halves of a tile are swept by different consumer warpgroups."""
+    ng = case.g.shape[0]
+    n_x = ng // 2
+    perm = np.arange(ng)
+    for b in sorted({int(b) % n_x for b in np.concatenate(case.comps)}):
+        assert b % 128 < 64
+        for off in (0, n_x):
+            perm[off + b], perm[off + b + 64] = off + b + 64, off + b
+    inv = np.argsort(perm)   # new position of old row j: inv[j]
+    return Case(q=case.q, g=case.g[perm], centred=False, target=inv[case.target], comps=[inv[c] for c in case.comps],
+                twin=np.where(case.twin >= 0, inv[np.maximum(case.twin, 0)], -1), info=dict(case.info, second_half=True))
+
+
+@dataclass
+class SplitOperands:
+    qh: np.ndarray          # bf16(q), fp32 values [nq, d]
+    gh: np.ndarray          # bf16(g)
+    qnh: np.ndarray         # to_bf16_parts_kernel's norms of the query parts [nq, n_parts]
+    qnr: np.ndarray
+    qnx: np.ndarray
+    g_norm: np.ndarray      # gmax[2c], gmax[2c + 1]: the gallery maxima of every part [n_parts]
+    g_res: np.ndarray
+
+
+def _part_norm(v: np.ndarray, n_parts: int) -> np.ndarray:
+    """_norm of every part of every row: [n, n_parts]."""
+    v3 = v.astype(np.float64).reshape(v.shape[0], n_parts, -1)
+    s = np.sum(v3 ** 2, axis=2).astype(np.float32)
+    return (np.sqrt(s) * np.float32(1.0001)).astype(np.float32)
+
+
+def split_operands(q: np.ndarray, g: np.ndarray, n_parts: int) -> SplitOperands:
+    """to_bf16_parts_kernel per part: no centring, bf16 RNE, norms x 1.0001f, gallery maxima per part (the zero padding
+    of a part to p_pad adds nothing to any of them)."""
+    qh, gh = bf16(q), bf16(g)
+    return SplitOperands(qh=qh, gh=gh, qnh=_part_norm(qh, n_parts), qnr=_part_norm(q - qh, n_parts),
+                         qnx=_part_norm(q, n_parts), g_norm=_part_norm(g, n_parts).max(axis=0),
+                         g_res=_part_norm(g - gh, n_parts).max(axis=0))
+
+
+def split_part_eps(op: SplitOperands, p_pad: int) -> np.ndarray:
+    """split_row_bound's term of every part, in the kernel's fp32 order of operations: [nq, n_parts]."""
+    f = np.float32
+    qh, qr, qx, gn, gr = op.qnh, op.qnr, op.qnx, op.g_norm[None, :], op.g_res[None, :]
+    e = f(1.001) * (qh * gr + qr * gn) + f(p_pad) * f(2.4e-7) * qh * (gn + gr) + f(3e-7) * qx * gn + f(1e-30)
+    return e.astype(np.float32)
+
+
+def split_eps(op: SplitOperands, p_pad: int) -> np.ndarray:
+    """split_row_bound's eps per query row: the largest part term."""
+    return split_part_eps(op, p_pad).max(axis=1)
+
+
+def split_bf16_terms(op: SplitOperands) -> np.ndarray:
+    """The bf16 part of every part's term, qh g_res + qr g_norm: [nq, n_parts]."""
+    return (op.qnh * op.g_res[None, :] + op.qnr * op.g_norm[None, :]).astype(np.float32)
+
+
+def part_products(q: np.ndarray, g: np.ndarray, n_parts: int) -> np.ndarray:
+    """The fp64 dot products of every part: [n_parts, nq, ng]."""
+    qp = q.astype(np.float64).reshape(q.shape[0], n_parts, -1).transpose(1, 0, 2)
+    gp = g.astype(np.float64).reshape(g.shape[0], n_parts, -1).transpose(1, 2, 0)
+    return np.matmul(qp, gp)
+
+
+def split_approx(op: SplitOperands, n_parts: int) -> np.ndarray:
+    """The fused sweep's split score: per part the tensor-core product of the bf16 operands (exact here) as fp32, then
+    the maximum over the parts."""
+    return part_products(op.qh, op.gh, n_parts).astype(np.float32).max(axis=0)
+
+
+def split_exact(q: np.ndarray, g: np.ndarray, n_parts: int) -> np.ndarray:
+    """The fp64 split score: the maximum over the parts of the fp64 part dot products."""
+    return part_products(q, g, n_parts).max(axis=0)
+
+
+def split_realized(case: Case, op: SplitOperands) -> np.ndarray:
+    """Per query: how far the target's approximate split score lies below its exact split score."""
+    c = case.info["n_parts"]
+    rows = np.arange(case.q.shape[0])
+    return split_exact(case.q, case.g, c)[rows, case.target] - split_approx(op, c)[rows, case.target].astype(np.float64)
