@@ -51,6 +51,19 @@ int dcr_sim_topk_split(const float* q, int nq, const float* g, int ng, int d, in
                              &g_last_stats);
 }
 
+size_t dcr_sim_topk_cross_workspace_size(int nq, int ng, int d, int n_parts, int k) {
+  return dcr::sim_topk_split_workspace_size(nq, ng, d, n_parts, k, true);
+}
+
+int dcr_sim_topk_cross(const float* q, int nq, const float* g, int ng, int d, int n_parts, int k, int64_t g_index_base,
+                       int64_t g_index_stride, float* out_scores, int64_t* out_idx, void* workspace, size_t workspace_bytes,
+                       void* stream) {
+  DCR_REQUIRE(q && g && out_scores && out_idx, "dcr_sim_topk_cross: null pointer argument");
+  return dcr::sim_topk_split(q, nq, g, ng, d, n_parts, k, g_index_base, g_index_stride, out_scores,
+                             reinterpret_cast<long long*>(out_idx), workspace, workspace_bytes, as_stream(stream),
+                             &g_last_stats, true);
+}
+
 int dcr_sim_topk_host(const float* q, int nq, const float* g, int ng, int d, int k, float* out_scores,
                       int64_t* out_idx) {
   DCR_REQUIRE(q && g && out_scores && out_idx, "dcr_sim_topk_host: null pointer argument");
@@ -151,6 +164,22 @@ int dcr_sim_range_split(const float* q, int nq, const float* g, int ng, int d, i
   return dcr::sim_range_split(q, nq, g, ng, d, n_parts, threshold, g_index_base, g_index_stride,
                               reinterpret_cast<long long*>(row_offsets), reinterpret_cast<long long*>(out_idx), out_scores,
                               max_pairs, reinterpret_cast<long long*>(counts), workspace, workspace_bytes, as_stream(stream));
+}
+
+size_t dcr_sim_range_cross_workspace_size(int nq, int ng, int d, int n_parts, int64_t max_pairs) {
+  return dcr::sim_range_split_workspace_size(nq, ng, d, n_parts, max_pairs, true);
+}
+
+int dcr_sim_range_cross(const float* q, int nq, const float* g, int ng, int d, int n_parts, float threshold,
+                        int64_t g_index_base, int64_t g_index_stride, int64_t* row_offsets, int64_t* out_idx,
+                        float* out_scores, int64_t max_pairs, int64_t* counts, void* workspace, size_t workspace_bytes,
+                        void* stream) {
+  DCR_REQUIRE(q && g && row_offsets && counts && (max_pairs == 0 || (out_idx && out_scores)),
+              "dcr_sim_range_cross: null pointer argument");
+  return dcr::sim_range_split(q, nq, g, ng, d, n_parts, threshold, g_index_base, g_index_stride,
+                              reinterpret_cast<long long*>(row_offsets), reinterpret_cast<long long*>(out_idx), out_scores,
+                              max_pairs, reinterpret_cast<long long*>(counts), workspace, workspace_bytes, as_stream(stream),
+                              true);
 }
 
 size_t dcr_sim_range_split_sharded_workspace_size(int nq, int ng_local, int d, int n_parts, int world,

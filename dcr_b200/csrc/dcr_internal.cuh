@@ -28,22 +28,23 @@ int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long 
              long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
              cudaStream_t stream, SimStats* stats);
 
-// top-k under the split score: max over the n_parts equal parts of the per-part dot products (sim_topk.cu)
-size_t sim_topk_split_workspace_size(int nq, int ng, int d, int n_parts, int k);
+// top-k under the split score: max over the n_parts equal parts of the per-part dot products (sim_topk.cu); cross: max
+// over every (query part, gallery part) pair
+size_t sim_topk_split_workspace_size(int nq, int ng, int d, int n_parts, int k, bool cross = false);
 int sim_topk_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, int k, long long g_index_base,
                    long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
-                   cudaStream_t stream, SimStats* stats);
+                   cudaStream_t stream, SimStats* stats, bool cross = false);
 
 size_t sim_range_workspace_size(int nq, int ng, int d, long long max_pairs);
 int sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, long long g_index_base,
               long long g_index_stride, long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,
               long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream);
-// threshold search under the split score (sim_range.cu); n_parts = 1 is sim_range
-size_t sim_range_split_workspace_size(int nq, int ng, int d, int n_parts, long long max_pairs);
+// threshold search under the split score (sim_range.cu); n_parts = 1 is sim_range; cross: the cross split score
+size_t sim_range_split_workspace_size(int nq, int ng, int d, int n_parts, long long max_pairs, bool cross = false);
 int sim_range_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, float threshold,
                     long long g_index_base, long long g_index_stride, long long* row_offsets, long long* out_idx,
                     float* out_scores, long long max_pairs, long long* counts, void* ws, size_t ws_bytes,
-                    cudaStream_t stream);
+                    cudaStream_t stream, bool cross = false);
 // out[0..n] = exclusive prefix sums of in[0..n-1], out[n] = total: one block, a fixed association (sim_range's row scan)
 int exclusive_scan_i64(const long long* in, long long n, long long* out, cudaStream_t stream);
 

@@ -26,7 +26,9 @@ namespace {
 // Everything is a fixed function of the inputs (no atomics decide an order), so every call returns the same bits.
 // Under the split score (sim_range_split, n_parts > 0) the same steps run on the split operands: the sweep folds the
 // parts into a running maximum (fused_tile_mma_split), the bound is split_row_bound and the re-score takes the maximum
-// of the per-part exact dot products (DESIGN.md section 3).
+// of the per-part exact dot products (DESIGN.md section 3).  Under the cross split score (sim_range_cross) the sweep walks
+// every (query part, gallery part) pair (fused_tile_mma_split<., true>), the bound is cross_row_bound and the re-score
+// folds every pair (cross_exact_scores).
 constexpr int kRangePiece = 512;   // candidates of one row re-scored by one block
 
 struct RangeParams : SweepHead {
@@ -71,11 +73,13 @@ DCR_DEVICE uint32_t range_hits(const uint32_t (&r)[32], const float* sb, float t
 // registers per thread, so two consumer warpgroups each own one 64-column half of every tile, as in the split top-k.
 // After each tile the halves trade their per-row hit counts through shared memory: the lower half's columns come first
 // in the row, so both halves count the same total and the emit sweep writes the row in ascending column order.
-template <bool kBias, bool kEmit, bool kSplit = false>
+// kCross: the cross split score, the same kernel with the cross schedule of the part pairs.
+template <bool kBias, bool kEmit, bool kSplit = false, bool kCross = false>
 __global__ void __launch_bounds__(32 + 128 * (kSplit ? 2 : 1), 1)
     sim_range_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_g,
                      const RangeParams p) {
   static_assert(!kSplit || !kBias, "the split score is not centred");
+  static_assert(!kCross || kSplit, "the cross score is a split score");
   constexpr int kSets = kSplit ? 2 : 1;
   constexpr int kSetCols = kBlockN / kSets;
   if (((p.bias_flag != nullptr) && (*p.bias_flag != 0)) != kBias) return;
@@ -89,7 +93,7 @@ __global__ void __launch_bounds__(32 + 128 * (kSplit ? 2 : 1), 1)
   const long long unit = blockIdx.x;
   SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
   if (warp == 4 * kSets) {
-    fused_producer(pp, &tmap_q, &tmap_g, p.stages, w, [](const SegWalker&) { return 0; });
+    fused_producer<kCross>(pp, &tmap_q, &tmap_g, p.stages, w, [](const SegWalker&) { return 0; }, p.kb_part);
   } else {
     const uint32_t set = kSplit ? warp >> 2 : 0;                    // column half of every tile (split)
     const uint32_t row = (kSplit ? warp & 3 : warp) * 32 + lane;   // query row inside the tile
@@ -116,7 +120,7 @@ __global__ void __launch_bounds__(32 + 128 * (kSplit ? 2 : 1), 1)
       for (int j = 0; j < w.ntiles; ++j) {
         if constexpr (kSplit) {
           WgAcc<kSetCols> acc;
-          fused_tile_mma_split(acc, st, pp, a_base, b_base, p.kb_part, j == w.ntiles - 1, lane);
+          fused_tile_mma_split<kSetCols, kCross>(acc, st, pp, a_base, b_base, p.kb_part, j == w.ntiles - 1, lane);
           const int gcol0 = (w.g_begin + j) * kBlockN + static_cast<int>(set) * kSetCols;
           uint32_t hits[kSetCols / 32];
           int mine = 0;
@@ -173,7 +177,8 @@ __global__ void __launch_bounds__(32 + 128 * (kSplit ? 2 : 1), 1)
 // (margin), hence approximate score >= t_i (row_bound).  A warp per query row.
 // kSplit: the split score, with eps and slack from split_row_bound (q.mu = 0; d_pad = n_parts * p_pad).  A NaN part norm
 // makes eps and t_i NaN, and !(a < NaN) keeps every column of that row: the exact re-score decides them all.
-template <bool kSplit>
+// kCross: the cross split score, eps and slack from cross_row_bound.
+template <bool kSplit, bool kCross = false>
 __global__ void __launch_bounds__(128)
     range_threshold_kernel(const float* __restrict__ q, int nq, int d, int d_pad, int n_parts, float tau,
                            const float* __restrict__ q_norm_hat, const float* __restrict__ q_norm_res,
@@ -184,7 +189,9 @@ __global__ void __launch_bounds__(128)
   const uint32_t lane = threadIdx.x & 31;
   if (row >= nq) return;
   const RowBound rb = [&] {
-    if constexpr (kSplit)
+    if constexpr (kCross)
+      return cross_row_bound(n_parts, d / n_parts, d_pad / n_parts, row, q_norm_hat, q_norm_res, q_norm_x, g_max, lane);
+    else if constexpr (kSplit)
       return split_row_bound(n_parts, d / n_parts, d_pad / n_parts, row, q_norm_hat, q_norm_res, q_norm_x, g_max, lane);
     else
       return row_bound(q + static_cast<size_t>(row) * d, d, d_pad, row, q_norm_hat, q_norm_res, q_norm_x, g_max, mu, nu,
@@ -281,11 +288,15 @@ DCR_DEVICE void range_piece(long long w, const long long* __restrict__ row_cand,
 // query is staged one part at a time: per part, stage the query part, prefetch that part of the piece's candidates, and
 // fold the part's exact_dot into the candidate's fp64 running maximum (-inf, then parts 0, 1, ..: the order of
 // split_rescore_kernel); the maximum is rounded to fp32 once.
-template <bool kSplit>
+// kCross: the cross split score, every (query part, gallery part) pair folded by cross_exact_scores, `staged` query parts
+// in shared memory at a time.
+template <bool kSplit, bool kCross = false>
 __global__ void __launch_bounds__(kRescoreThreads)
     range_rescore_kernel(const float* __restrict__ q, const float* __restrict__ g, int nq, int d, int n_parts, float tau,
                          const long long* __restrict__ row_cand, const long long* __restrict__ row_piece,
-                         int* __restrict__ cand_idx, float* __restrict__ cand_score, int* __restrict__ piece_kept) {
+                         int* __restrict__ cand_idx, float* __restrict__ cand_score, int* __restrict__ piece_kept,
+                         int staged) {
+  static_assert(!kCross || kSplit, "the cross score is a split score");
   extern __shared__ __align__(16) uint8_t sm[];
   const int tid = threadIdx.x;
   const uint32_t lane = threadIdx.x & 31;
@@ -295,7 +306,13 @@ __global__ void __launch_bounds__(kRescoreThreads)
   range_piece(blockIdx.x, row_cand, row_piece, nq, row, start, n);
   int* ci = cand_idx + start;
   float* cs = cand_score + start;
-  if constexpr (kSplit) {
+  if constexpr (kCross) {
+    double* best = reinterpret_cast<double*>(sm);   // [kRangePiece] the piece's exact scores
+    double* qs = best + kRangePiece;                // the staged query parts, then the warps' running maxima
+    cross_exact_scores<kRescoreThreads>(q + static_cast<size_t>(row) * d, g, d, n_parts, staged, ci, n, best, qs,
+                                        qs + static_cast<size_t>(staged) * (d / n_parts));
+    for (int c = tid; c < n; c += kRescoreThreads) cs[c] = static_cast<float>(best[c]);
+  } else if constexpr (kSplit) {
     double* best = reinterpret_cast<double*>(sm);   // [kRangePiece] running maxima of the piece's candidates
     double* qs = best + kRangePiece;                // [d / n_parts] the query part, widened
     const int pl = d / n_parts;
@@ -395,6 +412,7 @@ constexpr long long kMaxRangePairs = 1ll << 40;   // capacity accepted by the pl
 struct RangePlan {
   SweepGeometry geo;
   int n_parts;   // split score: descriptor parts; 0 = dot product
+  bool cross;    // the cross split score (n_parts >= 2)
   int nq_pad, n_qtiles, n_units, n_slots, stages;
   size_t smem_bytes;
   long long max_pieces;   // pieces of kRangePiece candidates when max_pairs candidates fill the rows worst
@@ -435,23 +453,30 @@ RangeBuffers carve_range(const RangePlan& rp, int nq, int d, long long max_pairs
   return b;
 }
 
-// n_parts = 0: the dot product (sim_range); >= 2: the split score over n_parts parts (sim_range_split)
-int make_range_plan(int nq, int ng, int d, int n_parts, long long max_pairs, int num_sms, size_t max_smem, RangePlan* rp) {
-  const char* who = n_parts ? "sim_range_split" : "sim_range";
+// n_parts = 0: the dot product (sim_range); >= 2: the split score over n_parts parts (sim_range_split; cross:
+// sim_range_cross)
+const char* range_name(int n_parts, bool cross) {
+  return n_parts ? (cross ? "sim_range_cross" : "sim_range_split") : "sim_range";
+}
+
+int make_range_plan(int nq, int ng, int d, int n_parts, bool cross, long long max_pairs, int num_sms, size_t max_smem,
+                    RangePlan* rp) {
+  const char* who = range_name(n_parts, cross);
   DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "%s: empty problem (nq=%d ng=%d d=%d)", who, nq, ng, d);
   if (n_parts) {
     DCR_REQUIRE(n_parts >= 1 && d % n_parts == 0 && (d / n_parts) % 4 == 0,
-                "sim_range_split: d=%d must split into %d parts whose length is a multiple of 4", d, n_parts);
+                "%s: d=%d must split into %d parts whose length is a multiple of 4", who, d, n_parts);
     const int p = d / n_parts;
-    DCR_REQUIRE(p <= kMaxDim, "sim_range_split: part length %d > %d not supported", p, kMaxDim);
+    DCR_REQUIRE(p <= kMaxDim, "%s: part length %d > %d not supported", who, p, kMaxDim);
     DCR_REQUIRE(static_cast<long long>(n_parts) * ((p + kBlockK - 1) / kBlockK * kBlockK) <= (1ll << 30),
-                "sim_range_split: %d parts of %d padded to 64 exceed 2^30 columns", n_parts, p);
+                "%s: %d parts of %d padded to 64 exceed 2^30 columns", who, n_parts, p);
   } else {
     DCR_REQUIRE(d <= kMaxDim, "sim_range: descriptor dim %d > %d not supported", d, kMaxDim);
     DCR_REQUIRE(d % 4 == 0, "sim_range: descriptor dim %d is not a multiple of 4", d);
   }
   DCR_REQUIRE(max_pairs >= 0 && max_pairs <= kMaxRangePairs, "%s: max_pairs=%lld outside [0, 2^40]", who, max_pairs);
   rp->n_parts = n_parts;
+  rp->cross = n_parts && cross;
   if (n_parts) {
     plan_split_geometry(ng, n_parts, d / n_parts, &rp->geo);
     // the threshold sweep keeps no candidate lists in shared memory, so a query tile of up to 512 part-padded columns
@@ -483,27 +508,28 @@ int make_range_plan(int nq, int ng, int d, int n_parts, long long max_pairs, int
   return 0;
 }
 
-size_t range_workspace_size(int nq, int ng, int d, int n_parts, long long max_pairs) {
+size_t range_workspace_size(int nq, int ng, int d, int n_parts, bool cross, long long max_pairs) {
   const DeviceInfo* di = device_info();
   RangePlan rp;
-  if (make_range_plan(nq, ng, d, n_parts, max_pairs, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &rp) != 0)
+  if (make_range_plan(nq, ng, d, n_parts, cross, max_pairs, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &rp) != 0)
     return 0;
   return rp.total;
 }
 
-// The whole search.  n_parts = 0: the dot product (sim_range); >= 2: the split score (sim_range_split).
-int range_search(const float* q, int nq, const float* g, int ng, int d, int n_parts, float threshold,
+// The whole search.  n_parts = 0: the dot product (sim_range); >= 2: the split score (sim_range_split; cross:
+// sim_range_cross).
+int range_search(const float* q, int nq, const float* g, int ng, int d, int n_parts, bool cross, float threshold,
                  long long g_index_base, long long g_index_stride, long long* row_offsets, long long* out_idx,
                  float* out_scores, long long max_pairs, long long* counts, void* ws, size_t ws_bytes,
                  cudaStream_t stream) {
-  const char* who = n_parts ? "sim_range_split" : "sim_range";
+  const char* who = range_name(n_parts, cross);
   const DeviceInfo* di = device_info();
   if (!di) return -2;
   if (int rc = require_sm90a(di, who)) return rc;
   DCR_REQUIRE(!std::isnan(threshold), "%s: threshold is NaN", who);
   DCR_REQUIRE(g_index_stride >= 1, "%s: g_index_stride=%lld < 1", who, g_index_stride);
   RangePlan rp;
-  if (int rc = make_range_plan(nq, ng, d, n_parts, max_pairs, di->num_sms, di->max_smem_optin, &rp)) return rc;
+  if (int rc = make_range_plan(nq, ng, d, n_parts, cross, max_pairs, di->num_sms, di->max_smem_optin, &rp)) return rc;
   DCR_REQUIRE(ws != nullptr && ws_bytes >= rp.total, "%s: workspace too small (%zu < %zu)", who, ws_bytes, rp.total);
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "%s: workspace must be 256-byte aligned", who);
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0,
@@ -518,7 +544,9 @@ int range_search(const float* q, int nq, const float* g, int ng, int d, int n_pa
   } else {
     if (int rc = prepare_operands(q, nq, rp.nq_pad, g, ng, d, geo, di, o, stream)) return rc;
   }
-  if (int rc = launch(n_parts ? range_threshold_kernel<true> : range_threshold_kernel<false>, (nq + 3) / 4, 128, 0, stream,
+  auto threshold_kernel = rp.cross ? range_threshold_kernel<true, true>
+                                   : (n_parts ? range_threshold_kernel<true> : range_threshold_kernel<false>);
+  if (int rc = launch(threshold_kernel, (nq + 3) / 4, 128, 0, stream,
                       who, q, nq, d, geo.d_pad, n_parts, threshold, o.qnh, o.qnr, o.qnx, o.gmax, o.mu, o.nu, o.qflag, b.thr))
     return rc;
 
@@ -533,11 +561,13 @@ int range_search(const float* q, int nq, const float* g, int ng, int d, int n_pa
   p.row_cand = b.row_cand;
   p.cand_idx = b.cand_idx;
   p.kb_part = n_parts ? geo.num_kb / n_parts : 0;
-  auto sweep = [&](auto off, auto on, auto split) {
+  auto sweep = [&](auto off, auto on, auto split, auto cross_split) {
+    if (rp.cross) return launch(cross_split, rp.n_units, 32 + 128 * 2, rp.smem_bytes, stream, who, tq, tg, p);
     if (n_parts) return launch(split, rp.n_units, 32 + 128 * 2, rp.smem_bytes, stream, who, tq, tg, p);
     return launch_sweep(off, on, rp.n_units, 32 + 128, rp.smem_bytes, stream, who, tq, tg, p);
   };
-  if (int rc = sweep(sim_range_kernel<false, false>, sim_range_kernel<true, false>, sim_range_kernel<false, false, true>))
+  if (int rc = sweep(sim_range_kernel<false, false>, sim_range_kernel<true, false>, sim_range_kernel<false, false, true>,
+                     sim_range_kernel<false, false, true, true>))
     return rc;
   if (int rc = launch(range_slot_scan_kernel, (nq + 255) / 256, 256, 0, stream, who, b.seg, nq, rp.n_qtiles,
                       geo.n_gtiles, geo.gchunk, geo.n_chunks, rp.n_units, b.row_cnt, b.row_pcnt))
@@ -556,13 +586,19 @@ int range_search(const float* q, int nq, const float* g, int ng, int d, int n_pa
                      who, n_cand, max_pairs);
 
   if (n_pieces > 0) {
-    if (int rc = sweep(sim_range_kernel<false, true>, sim_range_kernel<true, true>, sim_range_kernel<false, true, true>))
+    if (int rc = sweep(sim_range_kernel<false, true>, sim_range_kernel<true, true>, sim_range_kernel<false, true, true>,
+                       sim_range_kernel<false, true, true, true>))
       return rc;
-    // split: the piece's running maxima, then one query part; dot product: the whole query row
-    const size_t rescore_smem = (n_parts ? static_cast<size_t>(kRangePiece) + pl : static_cast<size_t>(d)) * 8;
-    if (int rc = launch(n_parts ? range_rescore_kernel<true> : range_rescore_kernel<false>, static_cast<unsigned>(n_pieces),
-                        kRescoreThreads, rescore_smem, stream, who, q, g, nq, d, n_parts, threshold, b.row_cand,
-                        b.row_piece, b.cand_idx, b.cand_score, b.piece_kept))
+    // split: the piece's running maxima, then one query part; cross: then the staged query parts and the warps' running
+    // maxima; dot product: the whole query row
+    const int staged = rp.cross ? cross_staged_parts(n_parts, pl) : 0;
+    const size_t rescore_smem =
+        (rp.cross ? static_cast<size_t>(kRangePiece) + cross_stage_doubles(staged, pl, kRescoreThreads / 32)
+                  : (n_parts ? static_cast<size_t>(kRangePiece) + pl : static_cast<size_t>(d))) * 8;
+    auto rescore_kernel = rp.cross ? range_rescore_kernel<true, true>
+                                   : (n_parts ? range_rescore_kernel<true> : range_rescore_kernel<false>);
+    if (int rc = launch(rescore_kernel, static_cast<unsigned>(n_pieces), kRescoreThreads, rescore_smem, stream, who, q, g,
+                        nq, d, n_parts, threshold, b.row_cand, b.row_piece, b.cand_idx, b.cand_score, b.piece_kept, staged))
       return rc;
   }
   if (int rc = launch(exclusive_scan_kernel<int>, 1, 1024, 0, stream, who, b.piece_kept, n_pieces, b.piece_excl))
@@ -586,31 +622,31 @@ int range_search(const float* q, int nq, const float* g, int ng, int d, int n_pa
 }  // namespace
 
 size_t sim_range_workspace_size(int nq, int ng, int d, long long max_pairs) {
-  return range_workspace_size(nq, ng, d, 0, max_pairs);
+  return range_workspace_size(nq, ng, d, 0, false, max_pairs);
 }
 
 int sim_range(const float* q, int nq, const float* g, int ng, int d, float threshold, long long g_index_base,
               long long g_index_stride, long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,
               long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
-  return range_search(q, nq, g, ng, d, 0, threshold, g_index_base, g_index_stride, row_offsets, out_idx, out_scores,
+  return range_search(q, nq, g, ng, d, 0, false, threshold, g_index_base, g_index_stride, row_offsets, out_idx, out_scores,
                       max_pairs, counts, ws, ws_bytes, stream);
 }
 
 // one part is the dot product itself: the dot-product search, whose bits the split score must reproduce
-size_t sim_range_split_workspace_size(int nq, int ng, int d, int n_parts, long long max_pairs) {
+size_t sim_range_split_workspace_size(int nq, int ng, int d, int n_parts, long long max_pairs, bool cross) {
   if (n_parts < 1) {
-    set_error(-1, "sim_range_split: n_parts=%d < 1", n_parts);
+    set_error(-1, "%s: n_parts=%d < 1", range_name(1, cross), n_parts);
     return 0;
   }
-  return range_workspace_size(nq, ng, d, n_parts == 1 ? 0 : n_parts, max_pairs);
+  return range_workspace_size(nq, ng, d, n_parts == 1 ? 0 : n_parts, cross, max_pairs);
 }
 
 int sim_range_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, float threshold,
                     long long g_index_base, long long g_index_stride, long long* row_offsets, long long* out_idx,
                     float* out_scores, long long max_pairs, long long* counts, void* ws, size_t ws_bytes,
-                    cudaStream_t stream) {
-  DCR_REQUIRE(n_parts >= 1, "sim_range_split: n_parts=%d < 1", n_parts);
-  return range_search(q, nq, g, ng, d, n_parts == 1 ? 0 : n_parts, threshold, g_index_base, g_index_stride, row_offsets,
+                    cudaStream_t stream, bool cross) {
+  DCR_REQUIRE(n_parts >= 1, "%s: n_parts=%d < 1", range_name(1, cross), n_parts);
+  return range_search(q, nq, g, ng, d, n_parts == 1 ? 0 : n_parts, cross, threshold, g_index_base, g_index_stride, row_offsets,
                       out_idx, out_scores, max_pairs, counts, ws, ws_bytes, stream);
 }
 

@@ -6,6 +6,8 @@
 #pragma once
 #include <cuda_bf16.h>
 
+#include <algorithm>
+
 #include "host_util.cuh"
 #include "ptx.cuh"
 
@@ -158,9 +160,12 @@ struct FusedPipe {
 // TMA producer of a fused sweep.  The whole warp walks the loop (warp-uniform values stay in uniform registers) and one
 // elected lane issues.  Per segment: the query tile (resident mode), then warm + ntiles gallery tiles of num_kb k-blocks,
 // the first `warm` of them replayed from the segment start; warm_of(walker) says how many.
-template <class WarmOf>
+// kCross: the cross split score (DESIGN.md section 3).  A tile is n_parts^2 part pairs of kb_part k-blocks each, gallery
+// part b outer and query part a inner: step (b, a, kin) loads gallery k-block b kb_part + kin and, streamed, query k-block
+// a kb_part + kin.  Three nested int loops: the n_parts^2 kb_part steps of a tile are never one count.
+template <bool kCross = false, class WarmOf>
 DCR_DEVICE void fused_producer(const FusedPipe& pp, const CUtensorMap* tq, const CUtensorMap* tg, int stages, SegWalker& w,
-                               WarmOf warm_of) {
+                               WarmOf warm_of, int kb_part = 0) {
   uint32_t seg = 0;
   PipeState st(stages);
   while (w.next()) {
@@ -179,16 +184,24 @@ DCR_DEVICE void fused_producer(const FusedPipe& pp, const CUtensorMap* tq, const
     for (int j = 0; j < warm + ntiles; ++j) {
       const int gi = g_begin + (j < warm ? j : j - warm);
       const int g_row = gi * kBlockN;
-      for (int kb = 0; kb < pp.num_kb; ++kb, st.next()) {
+      // one stage: gallery k-block gkb, and with a streamed query tile query k-block qkb
+      auto issue = [&](int gkb, int qkb) {
         const uint32_t s = st.s, ph = st.ph;
         mbar_wait(&pp.b_empty[s], ph ^ 1);
         if (elect_one()) {
           mbar_arrive_expect_tx(&pp.b_full[s], pp.stage_bytes);
-          tma_load_2d(pp.smem_b + s * pp.stage_bytes, tg, &pp.b_full[s], kb * kBlockK, g_row, kEvictNormal);
+          tma_load_2d(pp.smem_b + s * pp.stage_bytes, tg, &pp.b_full[s], gkb * kBlockK, g_row, kEvictNormal);
           if (pp.stream_a)
-            tma_load_2d(pp.smem_b + s * pp.stage_bytes + kBTileBytes, tq, &pp.b_full[s], kb * kBlockK, q_row, kEvictNormal);
+            tma_load_2d(pp.smem_b + s * pp.stage_bytes + kBTileBytes, tq, &pp.b_full[s], qkb * kBlockK, q_row, kEvictNormal);
         }
         __syncwarp();
+      };
+      if constexpr (kCross) {
+        for (int gkb0 = 0; gkb0 < pp.num_kb; gkb0 += kb_part)
+          for (int qkb0 = 0; qkb0 < pp.num_kb; qkb0 += kb_part)
+            for (int kin = 0; kin < kb_part; ++kin, st.next()) issue(gkb0 + kin, qkb0 + kin);
+      } else {
+        for (int kb = 0; kb < pp.num_kb; ++kb, st.next()) issue(kb, kb);
       }
     }
     ++seg;
@@ -229,7 +242,9 @@ DCR_DEVICE void fused_tile_mma(WgAcc<kCols>& acc, PipeState& st, const FusedPipe
 // part's first k-block overwrites the part accumulator, and after its last one the accumulator is folded into `best`,
 // the running element-wise maximum over the parts (fmaxf: a NaN part is ignored, as in the exact split score).  A part
 // boundary waits for every MMA in flight, because the fold reads the accumulator, and then releases both stages it held.
-template <int kCols>
+// kCross: the cross split score, the same fold over the n_parts^2 part pairs in fused_producer<true>'s order (gallery part
+// outer, query part inner); a resident query tile supplies query part a's k-blocks.
+template <int kCols, bool kCross = false>
 DCR_DEVICE void fused_tile_mma_split(WgAcc<kCols>& best, PipeState& st, const FusedPipe& pp, uint32_t a_base,
                                      uint32_t b_base, int kb_part, bool last, uint32_t lane) {
   const uint32_t a_step = pp.stream_a ? 0u : static_cast<uint32_t>(kATileBytes);
@@ -241,7 +256,8 @@ DCR_DEVICE void fused_tile_mma_split(WgAcc<kCols>& best, PipeState& st, const Fu
   uint32_t prev_s = 0;
   bool held = false;   // stage prev_s is still read by an MMA that may be in flight
   int kin = 0;         // k-block within the current part
-  for (int kb = 0; kb < pp.num_kb; ++kb, st.next()) {
+  // one k-block of the current part (pair), whose query k-block is kb
+  auto step = [&](int kb) {
     const uint32_t s = st.s;
     mbar_wait(&pp.b_full[s], st.ph);
     const uint32_t a_addr = a_base + (pp.stream_a ? s * static_cast<uint32_t>(pp.stage_bytes) : static_cast<uint32_t>(kb) * a_step);
@@ -269,6 +285,13 @@ DCR_DEVICE void fused_tile_mma_split(WgAcc<kCols>& best, PipeState& st, const Fu
       held = true;
       prev_s = s;
     }
+  };
+  if constexpr (kCross) {
+    for (int gkb0 = 0; gkb0 < pp.num_kb; gkb0 += kb_part)
+      for (int qkb0 = 0; qkb0 < pp.num_kb; qkb0 += kb_part)
+        for (int i = 0; i < kb_part; ++i, st.next()) step(qkb0 + i);
+  } else {
+    for (int kb = 0; kb < pp.num_kb; ++kb, st.next()) step(kb);
   }
   if (lane == 0 && !pp.stream_a && last) mbar_arrive(pp.a_empty);   // num_kb is a whole number of parts: nothing held
 }
@@ -489,6 +512,121 @@ DCR_DEVICE RowBound split_row_bound(int n_parts, int p, int p_pad, int qrow, con
   rb.qmu = 0.0;
   rb.slack = slack;
   return rb;
+}
+
+// The same bound under the cross split score: the approximate score of pair (a, b) is the bf16 dot product of query part a
+// with gallery part b, bounded by the part formula above from query part a's norms and gallery part b's maxima, and
+// |max_ab a_ab - max_ab s_ab| <= max_ab |a_ab - s_ab|.  The exact maximum over the n_parts^2 pairs (lane-strided over a,
+// a broadcast walk over b): it is the tightest bound the norms allow, at n_parts^2 / 32 steps per lane, small next to the
+// sweep's n_parts^2 k-blocks per tile.  A NaN part norm makes eps NaN.  Whole warp.
+DCR_DEVICE RowBound cross_row_bound(int n_parts, int p, int p_pad, int qrow, const float* __restrict__ q_norm_hat,
+                                    const float* __restrict__ q_norm_res, const float* __restrict__ q_norm_x,
+                                    const unsigned int* __restrict__ g_max, uint32_t lane) {
+  float eps = 0.f;
+  double slack = 0.0;
+  bool nan = false;
+  for (int a = static_cast<int>(lane); a < n_parts; a += 32) {
+    const size_t i = static_cast<size_t>(qrow) * n_parts + a;
+    const float qh = q_norm_hat[i], qr = q_norm_res[i], qx = q_norm_x[i];
+    for (int b = 0; b < n_parts; ++b) {
+      const float g_norm = __uint_as_float(g_max[2 * b]), g_res = __uint_as_float(g_max[2 * b + 1]);
+      const float e = 1.001f * (qh * g_res + qr * g_norm) + p_pad * 2.4e-7f * qh * (g_norm + g_res) + 3e-7f * qx * g_norm + 1e-30f;
+      nan |= (e != e);
+      eps = fmaxf(eps, e);
+      slack = fmax(slack, 4.6e-16 * (p + 8) * static_cast<double>(qx) * static_cast<double>(g_norm));
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    eps = fmaxf(eps, __shfl_xor_sync(kFull, eps, o));
+    slack = fmax(slack, __shfl_xor_sync(kFull, slack, o));
+  }
+  RowBound rb;
+  rb.eps = __any_sync(kFull, nan) ? __int_as_float(0x7fc00000) : eps;
+  rb.qmu = 0.0;
+  rb.slack = slack;
+  return rb;
+}
+
+// Exact cross split scores of the gallery rows rows[0 .. n) against query row q (d = n_parts * pl values): best[c] = the
+// fmax fold from -inf of exact_dot(q_a, g_b) over query part a outer, gallery part b inner -- the order of
+// split_rescore_kernel's cross branch.  The query is staged `staged` parts at a time in qs (fp64, [staged][pl]); for each
+// candidate the warp walks the gallery parts once per staged group, scoring part b against every staged query part while
+// it sits in L1, so a row is read from L2 about ceil(n_parts / staged) times instead of n_parts times.  Per group the warp
+// keeps each staged part's running maximum over b in part_max ([warp][2][staged]) and folds them into best in part order:
+// exact_dot never returns -0 (its sums start at +0 and round to nearest) and fmax ignores NaN, so on its values fmax is
+// associative and this grouping is the bits of the single chain.  Every thread of the group calls this.
+template <int kThreads>
+DCR_DEVICE void cross_exact_scores(const float* __restrict__ q, const float* __restrict__ g, int d, int n_parts, int staged,
+                                   const int* __restrict__ rows, int n, double* __restrict__ best, double* __restrict__ qs,
+                                   double* __restrict__ part_max) {
+  constexpr int kWarps = kThreads / 32;
+  const int tid = static_cast<int>(threadIdx.x) % kThreads;
+  const uint32_t lane = threadIdx.x & 31;
+  const int warp = tid >> 5;
+  const int pl = d / n_parts;
+  double* pm = part_max + warp * 2 * staged;
+  for (int c = tid; c < n; c += kThreads) best[c] = -INFINITY;
+  for (int a0 = 0; a0 < n_parts; a0 += staged) {
+    const int na = min(staged, n_parts - a0);
+    group_sync<kThreads>();   // the previous group's readers of qs are done (and best initialised)
+    const float* qsrc = q + static_cast<size_t>(a0) * pl;
+    for (int c = tid * 4; c < na * pl; c += kThreads * 4) {   // pl % 4 == 0
+      const float4 v = *reinterpret_cast<const float4*>(qsrc + c);
+      *reinterpret_cast<double2*>(qs + c) = make_double2(static_cast<double>(v.x), static_cast<double>(v.y));
+      *reinterpret_cast<double2*>(qs + c + 2) = make_double2(static_cast<double>(v.z), static_cast<double>(v.w));
+    }
+    group_sync<kThreads>();
+    for (int c = 2 * warp; c < n; c += 2 * kWarps) {
+      const bool two = c + 1 < n;
+      const float* g0 = g + static_cast<size_t>(rows[c]) * d;
+      const float* g1 = two ? g + static_cast<size_t>(rows[c + 1]) * d : g0;
+      for (int i = static_cast<int>(lane); i < 2 * staged; i += 32) pm[i] = -INFINITY;
+      for (int l = static_cast<int>(lane) * 32; l < pl; l += 32 * 32) {   // part 0 of both rows, a lane per 128-byte line
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(g0 + l));
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(g1 + l));
+      }
+      __syncwarp();
+      for (int b = 0; b < n_parts; ++b) {
+        const size_t off = static_cast<size_t>(b) * pl;
+        if (b + 1 < n_parts)
+          for (int l = static_cast<int>(lane) * 32; l < pl; l += 32 * 32) {
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(g0 + off + pl + l));
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(g1 + off + pl + l));
+          }
+        for (int a = 0; a < na; ++a) {
+          double v0, v1 = 0.0;
+          if (two) exact_dot<2>(qs + static_cast<size_t>(a) * pl, g0 + off, g1 + off, pl, lane, v0, v1);
+          else exact_dot<1>(qs + static_cast<size_t>(a) * pl, g0 + off, nullptr, pl, lane, v0, v1);
+          if (lane == 0) {
+            pm[a] = fmax(pm[a], v0);
+            if (two) pm[staged + a] = fmax(pm[staged + a], v1);
+          }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) {
+        for (int a = 0; a < na; ++a) {
+          best[c] = fmax(best[c], pm[a]);
+          if (two) best[c + 1] = fmax(best[c + 1], pm[staged + a]);
+        }
+      }
+      __syncwarp();
+    }
+  }
+  group_sync<kThreads>();
+}
+
+// Query parts the cross re-score stages at once (cross_exact_scores) within kCrossStageBytes of shared memory, counting
+// each part's fp64 values and the running maxima of four warps; at least one part.
+constexpr size_t kCrossStageBytes = 44 * 1024;
+inline int cross_staged_parts(int n_parts, int pl) {
+  const size_t per_part = (static_cast<size_t>(pl) + 8) * sizeof(double);
+  return static_cast<int>(std::max<size_t>(1, std::min<size_t>(n_parts, kCrossStageBytes / per_part)));
+}
+// fp64 values cross_exact_scores needs at qs for `staged` parts of pl values, with kWarps warps' running maxima after them
+__host__ __device__ inline size_t cross_stage_doubles(int staged, int pl, int warps) {
+  return static_cast<size_t>(staged) * pl + 2 * static_cast<size_t>(warps) * staged;
 }
 
 // ------------------------------------------------------------------------------------------------------------

@@ -47,7 +47,7 @@ struct SimParams : SweepHead {
   unsigned int* gthr;      // [nq_pad] per query row: best threshold any unit has reached so far, as an order-preserving
                            // unsigned key (0 = none)
   unsigned long long* clk; // [4] clock64 / globaltimer at the start and end of CTA 0 (SM clock under this kernel); null = off
-  int kb_part;             // split score: k-blocks per descriptor part (kSplit kernels only)
+  int kb_part;             // split score: k-blocks per descriptor part (kSplit kernels only; n_parts = num_kb / kb_part)
 };
 
 // second-chance pass: copy the bf16 rows of the flagged queries into a compact matrix (zero rows up to n_pad)
@@ -246,11 +246,13 @@ DCR_DEVICE float seed_threshold(float (&slot)[32], int kp) {
 // that does not match the device-side decision (p.bias_flag) exits at once -- no host synchronisation needed.
 // kSplit: the split score (sim_topk_split): every tile's approximate score is the maximum over the descriptor parts
 // (fused_tile_mma_split); the filter and the lists see that maximum.  Built with kSets = 2 and without kBias only.
-template <bool kBias, int kSets, bool kSplit = false>
+// kCross: the cross split score (sim_topk_cross), the same kernel with the cross schedule of the part pairs.
+template <bool kBias, int kSets, bool kSplit = false, bool kCross = false>
 __global__ void __launch_bounds__(32 + 128 * kSets, 1)
     sim_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_g,
                     const SimParams p) {
   static_assert(!kSplit || (kSets == 2 && !kBias), "the split score runs on column halves, uncentred");
+  static_assert(!kCross || kSplit, "the cross score is a split score");
   if (((p.bias_flag != nullptr) && (*p.bias_flag != 0)) != kBias) return;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr int kSetCols = kBlockN / kSets;
@@ -279,8 +281,9 @@ __global__ void __launch_bounds__(32 + 128 * kSets, 1)
   if (warp == kProducerWarp) {
     // ===================================== TMA producer =====================================
     SegWalker w(p.n_qtiles, p.n_gtiles, p.gchunk, p.n_chunks, unit, n_units);
-    fused_producer(pp, &tmap_q, &tmap_g, p.stages, w,
-                   [&](const SegWalker& s) { return (p.thr_init || s.carried) ? 0 : min(kWarmTiles, s.ntiles); });
+    fused_producer<kCross>(pp, &tmap_q, &tmap_g, p.stages, w,
+                           [&](const SegWalker& s) { return (p.thr_init || s.carried) ? 0 : min(kWarmTiles, s.ntiles); },
+                           p.kb_part);
   } else {
     // ===================================== consumer warpgroups =====================================
     // kSets = 2: two warps per 32-row block, each owning one column half ("set") of every tile and its own candidate
@@ -330,7 +333,7 @@ __global__ void __launch_bounds__(32 + 128 * kSets, 1)
         unsigned int shared_key = 0;
         if (!kWarm && gslot) shared_key = *reinterpret_cast<volatile unsigned int*>(gslot);
         WgAcc<kSetCols> acc;
-        if constexpr (kSplit) fused_tile_mma_split(acc, st, pp, a_base, b_base, p.kb_part, last, lane);
+        if constexpr (kSplit) fused_tile_mma_split<kSetCols, kCross>(acc, st, pp, a_base, b_base, p.kb_part, last, lane);
         else fused_tile_mma(acc, st, pp, a_base, b_base, last, lane);
         if (!kWarm && gslot) {
           if (thr > published) {   // risen since the last publication (compaction): let the other units know
@@ -452,6 +455,8 @@ DCR_DEVICE void block_argbest(double& bs, long long& bi, int& bp, BlockBest<kWar
 // kSplit: the split score.  The exact score of a candidate is the maximum over the parts of exact_dot over that part, the
 // query staged in shared memory one part at a time (rows are far wider than shared memory), and the bound is
 // split_row_bound.
+// kCross: the cross split score.  The exact score folds every (query part, gallery part) pair (cross_exact_scores, the
+// query staged several parts at a time) and the bound is cross_row_bound.
 struct RescoreParams {
   const float* q;                   // the caller's query rows [*][d]
   const float* g;                   // [ng][d]
@@ -477,6 +482,7 @@ struct RescoreParams {
   int* n_flagged;
   float* thr_next;                  // per flagged entry: start threshold of the second-chance pass; null = last pass
   int n_parts;                      // split score (kSplit): descriptor parts of d / n_parts values; q_norm_* per part
+  int staged;                       // cross split score (kCross): query parts staged at once (cross_staged_parts)
 };
 
 // One query's shared memory: the query row widened to fp64, then four arrays of max_cand entries.  Every part is a
@@ -493,8 +499,9 @@ struct RescoreSmem {
   }
 };
 
-template <int kThreads, bool kSplit = false>
+template <int kThreads, bool kSplit = false, bool kCross = false>
 __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const RescoreParams p) {
+  static_assert(!kCross || kSplit, "the cross score is a split score");
   constexpr int kWarps = kThreads / 32;
   extern __shared__ __align__(16) uint8_t sm[];
   const int tid = static_cast<int>(threadIdx.x) % kThreads;
@@ -504,9 +511,12 @@ __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const R
   // crow indexes the (possibly compacted) query matrix the fused kernel saw; qrow is the caller's row
   const int crow = blockIdx.x * (kRescoreThreads / kThreads) + grp;
   if (crow >= p.nq) return;   // whole groups leave; nothing below synchronises across groups
-  const RescoreSmem L(kSplit ? p.d / p.n_parts : p.d, p.max_cand);
+  const RescoreSmem L(kCross ? static_cast<int>(cross_stage_doubles(p.staged, p.d / p.n_parts, kWarps))
+                             : (kSplit ? p.d / p.n_parts : p.d),
+                      p.max_cand);
   uint8_t* base = sm + grp * L.bytes;
-  double* qs = reinterpret_cast<double*>(base);          // [d] the query row, widened once ([d / n_parts]: one part)
+  double* qs = reinterpret_cast<double*>(base);          // [d] the query row, widened once ([d / n_parts]: one part;
+                                                         // cross: the staged parts and the warps' running maxima)
   double* sc = reinterpret_cast<double*>(base + L.sc);   // exact scores of the survivors
   int* ci = reinterpret_cast<int*>(base + L.ci);         // gallery rows of all candidates
   float* ap = reinterpret_cast<float*>(base + L.ap);     // approximate scores
@@ -591,7 +601,10 @@ __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const R
   // certificate: every gallery row that is not a candidate has approximate centred score <= thr, hence exact score
   // q.g <= thr + eps + q.mu + slack (row_bound; split_row_bound for the split score)
   const RowBound rb = [&] {
-    if constexpr (kSplit)
+    if constexpr (kCross)
+      return cross_row_bound(p.n_parts, d / p.n_parts, p.d_pad / p.n_parts, qrow, p.q_norm_hat, p.q_norm_res, p.q_norm_x,
+                             p.g_max, lane);
+    else if constexpr (kSplit)
       return split_row_bound(p.n_parts, d / p.n_parts, p.d_pad / p.n_parts, qrow, p.q_norm_hat, p.q_norm_res, p.q_norm_x,
                              p.g_max, lane);
     else
@@ -626,7 +639,11 @@ __global__ void __launch_bounds__(kRescoreThreads) rescore_select_kernel(const R
     m += kept;
   }
   group_sync<kThreads>();
-  if constexpr (kSplit) {
+  if constexpr (kCross) {
+    const int pl = d / p.n_parts;
+    cross_exact_scores<kThreads>(p.q + static_cast<size_t>(qrow) * d, p.g, d, p.n_parts, p.staged, kc, m, sc, qs,
+                                 qs + static_cast<size_t>(p.staged) * pl);
+  } else if constexpr (kSplit) {
     // ---- exact split scores of the survivors: per part, stage the query part, prefetch that part of every survivor, then
     // fold each part's dot product into the running maximum (the order of split_rescore_kernel: -inf, then parts 0, 1, ..)
     const int pl = d / p.n_parts;
@@ -822,7 +839,9 @@ __global__ void __launch_bounds__(256)
 }
 
 // the same under the split score: scores[f][g] = max over the parts of exact_dot over that part (the order of
-// split_rescore_kernel), the batch's query parts staged one part at a time
+// split_rescore_kernel), the batch's query parts staged one part at a time.  kCross: the cross split score, query part
+// `part` against every gallery part b in ascending order (split_rescore_kernel's cross branch: query part outer).
+template <bool kCross>
 __global__ void __launch_bounds__(256)
     split_scan_kernel(const float* __restrict__ q, const float* __restrict__ g, int ng, int d, int n_parts,
                       const int* __restrict__ flagged, int f_begin, const int* __restrict__ n_flagged,
@@ -842,13 +861,26 @@ __global__ void __launch_bounds__(256)
     }
     __syncthreads();
     for (int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < ng; row += warps) {
-      const float* gr = g + static_cast<size_t>(row) * d + static_cast<size_t>(part) * pl;
-      for (int f = 0; f < nb; ++f) {
-        double v;
-        exact_dot<1>(qs + f * pl, gr, nullptr, pl, lane, v, v);
-        if (lane == 0) {
-          double& s = scores[static_cast<size_t>(f) * ng + row];
-          s = fmax(part == 0 ? -INFINITY : s, v);
+      if constexpr (kCross) {
+        const float* gr = g + static_cast<size_t>(row) * d;
+        for (int f = 0; f < nb; ++f) {
+          double s = part == 0 ? -INFINITY : scores[static_cast<size_t>(f) * ng + row];
+          for (int b = 0; b < n_parts; ++b) {
+            double v;
+            exact_dot<1>(qs + f * pl, gr + static_cast<size_t>(b) * pl, nullptr, pl, lane, v, v);
+            s = fmax(s, v);
+          }
+          if (lane == 0) scores[static_cast<size_t>(f) * ng + row] = s;
+        }
+      } else {
+        const float* gr = g + static_cast<size_t>(row) * d + static_cast<size_t>(part) * pl;
+        for (int f = 0; f < nb; ++f) {
+          double v;
+          exact_dot<1>(qs + f * pl, gr, nullptr, pl, lane, v, v);
+          if (lane == 0) {
+            double& s = scores[static_cast<size_t>(f) * ng + row];
+            s = fmax(part == 0 ? -INFINITY : s, v);
+          }
         }
       }
     }
@@ -901,6 +933,7 @@ struct PassPlan {
 
 struct SimPlan : SweepGeometry {
   int n_parts;   // split score: descriptor parts (plan_split_geometry); 0 = dot product
+  bool cross;    // the cross split score (n_parts >= 2)
   int max_sets;  // upper bound for PassPlan::n_sets (1 or 2)
   int kp0, kp1;           // candidates kept by the first pass / by the second-chance pass (0 = no second pass)
   PassPlan p0, p1;        // p1 is sized for the worst case (every query flagged)
@@ -1008,23 +1041,26 @@ TopkBuffers carve_topk(const SimPlan& pl, int nq, int ng, int d, Carve& w) {
   return b;
 }
 
-// n_parts = 0: the dot product; >= 1: the split score over n_parts parts (sim_topk_split)
-int make_plan(int nq, int ng, int d, int k, int n_parts, int num_sms, size_t max_smem, SimPlan* pl) {
-  const char* who = n_parts ? "sim_topk_split" : "sim_topk";
+// n_parts = 0: the dot product; >= 1: the split score over n_parts parts (sim_topk_split; cross: sim_topk_cross)
+const char* topk_name(int n_parts, bool cross) { return n_parts ? (cross ? "sim_topk_cross" : "sim_topk_split") : "sim_topk"; }
+
+int make_plan(int nq, int ng, int d, int k, int n_parts, bool cross, int num_sms, size_t max_smem, SimPlan* pl) {
+  const char* who = topk_name(n_parts, cross);
   DCR_REQUIRE(nq >= 1 && ng >= 1 && d >= 1, "%s: empty problem (nq=%d ng=%d d=%d)", who, nq, ng, d);
   if (n_parts) {
     DCR_REQUIRE(n_parts >= 1 && d % n_parts == 0 && (d / n_parts) % 4 == 0,
-                "sim_topk_split: d=%d must split into %d parts whose length is a multiple of 4", d, n_parts);
+                "%s: d=%d must split into %d parts whose length is a multiple of 4", who, d, n_parts);
     const int p = d / n_parts;
-    DCR_REQUIRE(p <= kMaxDim, "sim_topk_split: part length %d > %d not supported", p, kMaxDim);
+    DCR_REQUIRE(p <= kMaxDim, "%s: part length %d > %d not supported", who, p, kMaxDim);
     DCR_REQUIRE(static_cast<long long>(n_parts) * ((p + kBlockK - 1) / kBlockK * kBlockK) <= (1ll << 30),
-                "sim_topk_split: %d parts of %d padded to 64 exceed 2^30 columns", n_parts, p);
+                "%s: %d parts of %d padded to 64 exceed 2^30 columns", who, n_parts, p);
   } else {
     DCR_REQUIRE(d <= kMaxDim, "sim_topk: descriptor dim %d > %d not supported", d, kMaxDim);
   }
   DCR_REQUIRE(k >= 1 && k <= 16, "%s: k=%d outside [1,16]", who, k);
   DCR_REQUIRE(k <= ng, "%s: k=%d > gallery size %d", who, k, ng);
   pl->n_parts = n_parts;
+  pl->cross = n_parts && cross;
   if (n_parts) plan_split_geometry(ng, n_parts, d / n_parts, pl);
   else plan_geometry(ng, d, pl);
   // Two consumer warpgroups (two warps per 32-row block, each with its own lists for one column half) when few
@@ -1068,6 +1104,9 @@ int launch_fused(const SimPlan& pl, const PassPlan& pp, const __nv_bfloat16* qb,
   p.gthr = gthr;
   p.kb_part = pl.n_parts ? pl.num_kb / pl.n_parts : 0;
   DCR_CUDA_CHECK(cudaMemsetAsync(gthr, 0, static_cast<size_t>(pp.nq_pad) * 4, stream));
+  if (pl.cross)
+    return launch(sim_topk_kernel<false, 2, true, true>, pp.n_units, 32 + 128 * 2, pp.smem_bytes, stream, "sim_topk_cross", tq,
+                  tg, p);
   if (pl.n_parts)
     return launch(sim_topk_kernel<false, 2, true>, pp.n_units, 32 + 128 * 2, pp.smem_bytes, stream, "sim_topk_split", tq, tg, p);
   const bool two = pp.n_sets == 2;
@@ -1077,16 +1116,16 @@ int launch_fused(const SimPlan& pl, const PassPlan& pp, const __nv_bfloat16* qb,
 }
 
 // The whole search: stage 1, the fused pass, the exact re-score, the second-chance pass and the brute-force path.
-// n_parts = 0: the dot product (sim_topk); >= 1: the split score over n_parts parts (sim_topk_split).
-int topk_search(const float* q, int nq, const float* g, int ng, int d, int n_parts, int k, long long g_index_base,
-                long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
-                cudaStream_t stream, SimStats* stats) {
-  const char* who = n_parts ? "sim_topk_split" : "sim_topk";
+// n_parts = 0: the dot product (sim_topk); >= 1: the split score over n_parts parts (sim_topk_split; cross: sim_topk_cross).
+int topk_search(const float* q, int nq, const float* g, int ng, int d, int n_parts, bool cross, int k,
+                long long g_index_base, long long g_index_stride, float* out_scores, long long* out_idx, void* ws,
+                size_t ws_bytes, cudaStream_t stream, SimStats* stats) {
+  const char* who = topk_name(n_parts, cross);
   const DeviceInfo* di = device_info();
   if (!di) return -2;
   if (int rc = require_sm90a(di, who)) return rc;
   SimPlan pl;
-  if (int rc = make_plan(nq, ng, d, k, n_parts, di->num_sms, di->max_smem_optin, &pl)) return rc;
+  if (int rc = make_plan(nq, ng, d, k, n_parts, cross, di->num_sms, di->max_smem_optin, &pl)) return rc;
   DCR_REQUIRE(ws != nullptr && ws_bytes >= pl.total, "%s: workspace too small (%zu < %zu)", who, ws_bytes, pl.total);
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "%s: workspace must be 256-byte aligned", who);
   DCR_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0 && d % 4 == 0,
@@ -1126,15 +1165,20 @@ int topk_search(const float* q, int nq, const float* g, int ng, int d, int n_par
     rp.q_norm_hat = o.qnh, rp.q_norm_res = o.qnr, rp.q_norm_x = o.qnx, rp.g_max = o.gmax;
     rp.g_index_base = g_index_base, rp.g_index_stride = g_index_stride, rp.out_scores = out_scores, rp.out_idx = out_idx;
     rp.flagged = flagged, rp.n_flagged = n_flagged, rp.thr_next = thr_next, rp.n_parts = n_parts;
+    rp.staged = pl.cross ? cross_staged_parts(n_parts, pl_len) : 0;
     // one warp per query when a q-tile's candidate slots fit a lane each and four queries' rows fit a block's shared memory
-    // (the block-wide form spends its time on barriers for such small candidate sets)
-    const size_t per_query = RescoreSmem(pl_len, pp.max_cand).bytes;
-    const bool warp_form = pp.kp > 0 && pp.max_cand / pp.kp <= 32 && pp.n_chunks <= 32 && 4 * per_query <= 56 * 1024 &&
-                           !tuning_flag("DCR_SIM_RESCORE_BLOCK");
+    // (the block-wide form spends its time on barriers for such small candidate sets).  The cross score always takes the
+    // block form: each survivor costs n_parts^2 part dot products, which four warps share.
+    const size_t per_query =
+        RescoreSmem(pl.cross ? static_cast<int>(cross_stage_doubles(rp.staged, pl_len, kRescoreThreads / 32)) : pl_len,
+                    pp.max_cand).bytes;
+    const bool warp_form = !pl.cross && pp.kp > 0 && pp.max_cand / pp.kp <= 32 && pp.n_chunks <= 32 &&
+                           4 * per_query <= 56 * 1024 && !tuning_flag("DCR_SIM_RESCORE_BLOCK");
     const int per_block = warp_form ? kRescoreThreads / 32 : 1;
     const size_t smem = per_block * per_query;
-    auto kern = n_parts ? (warp_form ? rescore_select_kernel<32, true> : rescore_select_kernel<kRescoreThreads, true>)
-                        : (warp_form ? rescore_select_kernel<32> : rescore_select_kernel<kRescoreThreads>);
+    auto kern = pl.cross ? rescore_select_kernel<kRescoreThreads, true, true>
+                : n_parts ? (warp_form ? rescore_select_kernel<32, true> : rescore_select_kernel<kRescoreThreads, true>)
+                          : (warp_form ? rescore_select_kernel<32> : rescore_select_kernel<kRescoreThreads>);
     return launch(kern, (pp.nq + per_block - 1) / per_block, kRescoreThreads, smem, stream, who, rp);
   };
   if (int rc = rescore(pl.p0, nullptr, b.flag0, b.counts + 0, b.thr1)) return rc;
@@ -1171,8 +1215,8 @@ int topk_search(const float* q, int nq, const float* g, int ng, int d, int n_par
     const size_t ex_smem = static_cast<size_t>(ex_batch) * pl_len * 4;
     const int* n_dev = (exact_list == b.flag0) ? b.counts + 0 : b.counts + 1;
     for (int done = 0; done < n_exact; done += ex_batch) {
-      const int rc = n_parts ? launch(split_scan_kernel, di->num_sms * 2, 256, ex_smem, stream, who, q, g, ng, d, n_parts,
-                                      exact_list, done, n_dev, b.exact, ex_batch)
+      const int rc = n_parts ? launch(pl.cross ? split_scan_kernel<true> : split_scan_kernel<false>, di->num_sms * 2, 256,
+                                      ex_smem, stream, who, q, g, ng, d, n_parts, exact_list, done, n_dev, b.exact, ex_batch)
                              : launch(exact_scan_kernel, di->num_sms * 2, 256, ex_smem, stream, who, q, g, ng, d, exact_list,
                                       done, n_dev, b.exact, ex_batch);
       if (rc) return rc;
@@ -1219,39 +1263,39 @@ int split_rescore(const float* q, const float* g, int nq, int d, int n_chunks, i
 }
 
 namespace {
-size_t workspace_size(int nq, int ng, int d, int n_parts, int k) {
+size_t workspace_size(int nq, int ng, int d, int n_parts, bool cross, int k) {
   const DeviceInfo* di = device_info();
   SimPlan pl;
-  if (make_plan(nq, ng, d, k, n_parts, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &pl) != 0)
+  if (make_plan(nq, ng, d, k, n_parts, cross, di ? di->num_sms : 132, di ? di->max_smem_optin : 232448, &pl) != 0)
     return 0;
   return pl.total;
 }
 }  // namespace
 
-size_t sim_topk_workspace_size(int nq, int ng, int d, int k) { return workspace_size(nq, ng, d, 0, k); }
+size_t sim_topk_workspace_size(int nq, int ng, int d, int k) { return workspace_size(nq, ng, d, 0, false, k); }
 
 int sim_topk(const float* q, int nq, const float* g, int ng, int d, int k, long long g_index_base,
              long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
              cudaStream_t stream, SimStats* stats) {
-  return topk_search(q, nq, g, ng, d, 0, k, g_index_base, g_index_stride, out_scores, out_idx, ws, ws_bytes, stream, stats);
+  return topk_search(q, nq, g, ng, d, 0, false, k, g_index_base, g_index_stride, out_scores, out_idx, ws, ws_bytes, stream, stats);
 }
 
 // one part is the dot product itself: the dot-product search, whose bits the split score must reproduce
-size_t sim_topk_split_workspace_size(int nq, int ng, int d, int n_parts, int k) {
-  if (n_parts == 1) return workspace_size(nq, ng, d, 0, k);
+size_t sim_topk_split_workspace_size(int nq, int ng, int d, int n_parts, int k, bool cross) {
+  if (n_parts == 1) return workspace_size(nq, ng, d, 0, false, k);
   if (n_parts < 1) {
-    set_error(-1, "sim_topk_split: n_parts=%d < 1", n_parts);
+    set_error(-1, "%s: n_parts=%d < 1", topk_name(1, cross), n_parts);
     return 0;
   }
-  return workspace_size(nq, ng, d, n_parts, k);
+  return workspace_size(nq, ng, d, n_parts, cross, k);
 }
 
 int sim_topk_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, int k, long long g_index_base,
                    long long g_index_stride, float* out_scores, long long* out_idx, void* ws, size_t ws_bytes,
-                   cudaStream_t stream, SimStats* stats) {
-  DCR_REQUIRE(n_parts >= 1, "sim_topk_split: n_parts=%d < 1", n_parts);
-  return topk_search(q, nq, g, ng, d, n_parts == 1 ? 0 : n_parts, k, g_index_base, g_index_stride, out_scores, out_idx, ws,
-                     ws_bytes, stream, stats);
+                   cudaStream_t stream, SimStats* stats, bool cross) {
+  DCR_REQUIRE(n_parts >= 1, "%s: n_parts=%d < 1", topk_name(1, cross), n_parts);
+  return topk_search(q, nq, g, ng, d, n_parts == 1 ? 0 : n_parts, cross, k, g_index_base, g_index_stride, out_scores,
+                     out_idx, ws, ws_bytes, stream, stats);
 }
 
 }  // namespace dcr

@@ -11,7 +11,8 @@ The reference has no function boundary here -- it is inline tensor code in `main
 `sim_topk(query, gallery, k)` returns exactly what `torch.mm(gallery, query.T).T.topk(k, dim=1)` would (values,
 indices), with a defined tie rule (lowest gallery index first) and without materialising the [Q,G] matrix.
 `sim_range(query, gallery, threshold)` returns the entries of that matrix that reach a threshold, as CSR.
-`sim_topk_split` and `sim_range_split` do the same under the 'splitloss' score (the best of the descriptor parts).
+`sim_topk_split` and `sim_range_split` do the same under the 'splitloss' score (the best of the descriptor parts), in
+its aligned and its cross form.
 All compute happens in libdcr_b200.so on the tensors' CUDA device.
 """
 from __future__ import annotations
@@ -134,13 +135,16 @@ def sim_range(query: torch.Tensor, gallery: torch.Tensor, threshold: float, *, i
 
 
 def sim_range_split(query: torch.Tensor, gallery: torch.Tensor, threshold: float, num_chunks: int, *,
-                    index_base: int = 0, index_stride: int = 1) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                    cross: bool = False, index_base: int = 0, index_stride: int = 1
+                    ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """Every (query i, gallery j) pair whose 'splitloss' score (diff_retrieval.py:393-400, aligned parts) reaches the
     threshold, in sim_range's CSR form: (offsets i64[Q+1], indices i64[P], scores f32[P]).  The score is
     max_c <q_c, g_c> over the C = num_chunks equal parts, bit for bit what sim_topk_split reports for the same pair; a
     NaN part is ignored, a pair whose parts are all NaN scores -inf, threshold = -inf reports every pair.  Part length
     p = D/C a multiple of 4 and at most 8192; num_chunks = 1 is sim_range.  Replaces the splitloss similarity.pth
-    (:411, :414) without the [G, Q, C] tensor of its einsum (dcr_sim_range_split)."""
+    (:411, :414) without the [G, Q, C] tensor of its einsum (dcr_sim_range_split).
+    cross=True: the cross score (`--stype cross`, max over every (query part, gallery part) pair), bit for bit what
+    sim_topk_split(cross=True) reports (dcr_sim_range_cross)."""
     lib = _lib.load()
     q = _check_cuda_f32("query", query)
     g = _check_cuda_f32("gallery", gallery)
@@ -151,6 +155,7 @@ def sim_range_split(query: torch.Tensor, gallery: torch.Tensor, threshold: float
     threshold = float(threshold)
     if math.isnan(threshold):
         raise _lib.DcrError("sim_range_split: threshold is NaN")
+    name = "dcr_sim_range_cross" if cross else "dcr_sim_range_split"
     nq, d = q.shape
     ng = g.shape[0]
     counts = (C.c_int64 * 2)()
@@ -158,20 +163,20 @@ def sim_range_split(query: torch.Tensor, gallery: torch.Tensor, threshold: float
     with torch.cuda.device(q.device):
         offsets = torch.empty(nq + 1, dtype=torch.int64, device=q.device)
         for attempt in range(2):
-            nbytes = lib.dcr_sim_range_split_workspace_size(nq, ng, d, num_chunks, cap)
+            nbytes = getattr(lib, name + "_workspace_size")(nq, ng, d, num_chunks, cap)
             if nbytes == 0:
-                raise _lib.DcrError(f"dcr_sim_range_split_workspace_size: {_lib.last_error()}")
+                raise _lib.DcrError(f"{name}_workspace_size: {_lib.last_error()}")
             ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=q.device)
             out_i = torch.empty(cap, dtype=torch.int64, device=q.device)
             out_s = torch.empty(cap, dtype=torch.float32, device=q.device)
             st = torch.cuda.current_stream().cuda_stream
-            rc = lib.dcr_sim_range_split(q.data_ptr(), nq, g.data_ptr(), ng, d, num_chunks, threshold, index_base,
-                                         index_stride, offsets.data_ptr(), out_i.data_ptr(), out_s.data_ptr(), cap,
-                                         counts, _aligned_ptr(ws), nbytes, st)
+            rc = getattr(lib, name)(q.data_ptr(), nq, g.data_ptr(), ng, d, num_chunks, threshold, index_base,
+                                    index_stride, offsets.data_ptr(), out_i.data_ptr(), out_s.data_ptr(), cap, counts,
+                                    _aligned_ptr(ws), nbytes, st)
             if rc == _lib.ERR_CAPACITY and attempt == 0:
                 cap = int(counts[1])   # the candidate count is a fixed function of the inputs: this capacity fits
                 continue
-            _lib.check(rc, "dcr_sim_range_split")
+            _lib.check(rc, name)
             break
     n = int(counts[0])
     if n < cap:   # do not keep the whole capacity alive behind the result
@@ -186,16 +191,12 @@ def sim_topk_split(q: torch.Tensor, g: torch.Tensor, k: int, num_chunks: int, cr
     One fused tensor-core sweep whose epilogue sees the maximum over the parts, then the exact split score of the
     candidates (dcr_sim_topk_split): any number of parts, part length p = D/C a multiple of 4 and at most 8192.
     Reported gallery indices are index_base + index_stride * row (a rank's gallery shard).
-    cross=True is `--stype cross` (einsum_in_chunks :643-662): score = max over every (gallery part, query part) pair.
-    Candidates then come from ONE fused pass over the part matrices [Q*C, D/C] x [G*C, D/C] with
-    k' = (k-1)*C + 1 rows per query part (fewer than k' part-rows can beat the best part-row of a true top-k gallery row)
-    while k' <= 16, otherwise from one pass per gallery part with k' = k (no limit on the number of parts)."""
+    cross=True is `--stype cross` (einsum_in_chunks :643-662): score = max over every (query part, gallery part) pair,
+    bit for bit what dcr_split_rescore(cross=1) reports.  The same fused sweep walks all C^2 part pairs
+    (dcr_sim_topk_cross), with the same limits: any number of parts, 1 <= k <= 16.  It is the only path: on an H100 it
+    took 0.31x the time of the old single-pass composition (one sim_topk over the part matrices, then
+    dcr_split_rescore) on 1k x 10k ViT-S/16 token rows at k = 1, and 0.59x that of the per-part one (DESIGN.md section 3)."""
     lib = _lib.load()
-    if cross and num_chunks > 1:
-        s, i = _sim_topk_cross(lib, q, g, k, num_chunks)
-        if index_base != 0 or index_stride != 1:
-            i = torch.where(i >= 0, index_base + index_stride * i, i)
-        return s, i
     if not (isinstance(q, torch.Tensor) and isinstance(g, torch.Tensor) and q.is_cuda and g.is_cuda):
         raise _lib.DcrError("sim_topk_split needs CUDA tensors")
     q = _check_cuda_f32("query", q.contiguous().float())
@@ -206,58 +207,18 @@ def sim_topk_split(q: torch.Tensor, g: torch.Tensor, k: int, num_chunks: int, cr
         raise _lib.DcrError(f"descriptor dims differ: {q.shape[1]} vs {g.shape[1]}")
     nq, d = q.shape
     ng = g.shape[0]
+    name = "dcr_sim_topk_cross" if cross else "dcr_sim_topk_split"
     with torch.cuda.device(q.device):
-        nbytes = lib.dcr_sim_topk_split_workspace_size(nq, ng, d, num_chunks, k)
+        nbytes = getattr(lib, name + "_workspace_size")(nq, ng, d, num_chunks, k)
         if nbytes == 0:
-            raise _lib.DcrError(f"dcr_sim_topk_split_workspace_size: {_lib.last_error()}")
+            raise _lib.DcrError(f"{name}_workspace_size: {_lib.last_error()}")
         ws = _workspace(nbytes, q.device)
         out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
         out_i = torch.empty((nq, k), dtype=torch.int64, device=q.device)
         st = torch.cuda.current_stream().cuda_stream
-        rc = lib.dcr_sim_topk_split(q.data_ptr(), nq, g.data_ptr(), ng, d, num_chunks, k, index_base, index_stride,
-                                    out_s.data_ptr(), out_i.data_ptr(), _aligned_ptr(ws), nbytes, st)
-        _lib.check(rc, "dcr_sim_topk_split")
-    return out_s, out_i
-
-
-def _sim_topk_cross(lib, q: torch.Tensor, g: torch.Tensor, k: int, c: int) -> Tuple[torch.Tensor, torch.Tensor]:
-    if not (q.is_cuda and g.is_cuda):
-        raise _lib.DcrError("sim_topk_split needs CUDA tensors")
-    q = q.contiguous().float()
-    g = g.contiguous().float()
-    nq, d = q.shape
-    ng = g.shape[0]
-    if d % c or (d // c) % 4:
-        raise _lib.DcrError(f"splitloss: descriptor dim {d} must split into {c} parts of a multiple of 4 dims")
-    kk = (k - 1) * c + 1
-    p = d // c
-    if kk <= 16:
-        # one fused pass over the part matrices: a gallery row of the true top-k is reached through its best
-        # (query part, gallery part) pair, and fewer than (k-1)*c + 1 part-rows can beat that part-row
-        kk = min(kk, ng * c)
-        _, idx = sim_topk(q.view(nq * c, p), g.view(ng * c, p), kk)            # rows of the part matrices
-        cand = (idx // c).reshape(nq, c * kk).contiguous()                      # gallery rows the part-rows belong to
-    else:
-        # any number of parts (the reference default topk = 10 with num_loss_chunks >= 2, diff_retrieval.py:643-662):
-        # one fused pass per GALLERY part against all query parts with k' = k.  Within the list of the pair
-        # (query part a, gallery part b) every row that beats a true top-k row also beats it in the cross score, so
-        # the union of the c*c per-pair top-k lists contains the true top-k.
-        if c * c * k > 4096:
-            raise _lib.DcrError(f"splitloss cross: {c} parts x top-{k} needs {c * c * k} candidates per query (max 4096)")
-        kq = min(k, ng)
-        cand = torch.full((nq, c, c, k), -1, dtype=torch.int64, device=q.device)
-        qparts = q.view(nq * c, p)
-        for b in range(c):
-            _, idx = sim_topk(qparts, g[:, b * p:(b + 1) * p].contiguous(), kq)   # [nq*c, kq] gallery rows
-            cand[:, :, b, :kq] = idx.view(nq, c, kq)
-        cand = cand.reshape(nq, c * c * k).contiguous()
-    out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
-    out_i = torch.empty((nq, k), dtype=torch.int64, device=q.device)
-    with torch.cuda.device(q.device):
-        st = torch.cuda.current_stream().cuda_stream
-        rc = lib.dcr_split_rescore(q.data_ptr(), g.data_ptr(), nq, d, c, 1, cand.data_ptr(), cand.shape[1], k,
-                                   out_s.data_ptr(), out_i.data_ptr(), st)
-        _lib.check(rc, "dcr_split_rescore")
+        rc = getattr(lib, name)(q.data_ptr(), nq, g.data_ptr(), ng, d, num_chunks, k, index_base, index_stride,
+                                out_s.data_ptr(), out_i.data_ptr(), _aligned_ptr(ws), nbytes, st)
+        _lib.check(rc, name)
     return out_s, out_i
 
 

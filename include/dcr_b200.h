@@ -117,17 +117,24 @@ int dcr_sim_topk_split(const float* q, int nq, const float* g, int ng, int d, in
                        int64_t g_index_stride, float* out_scores, int64_t* out_idx, void* workspace,
                        size_t workspace_bytes, void* stream);
 
-/* Final step of the 'splitloss' similarity in its 'cross' form, and of the per-part composition the aligned form used
- * before dcr_sim_topk_split (descriptors cut into n_chunks equal parts, pair
- * score = max over the parts of the per-part dot products).  The caller runs dcr_sim_topk once per part and passes
- * the union of the per-part top-k rows as cand [nq][n_cand] (duplicates allowed); this evaluates the exact split
- * score of every candidate (float64 accumulation, reported as fp32) and writes the k best per query ordered by
- * (score desc, row asc).  d %% n_chunks == 0, (d / n_chunks) %% 4 == 0, k <= n_cand <= 4096; negative entries of
- * cand are empty slots.
- * cross != 0: the 'cross' form (--stype cross, einsum_in_chunks diff_retrieval.py:643-662): score = max over EVERY pair
- * (gallery part, query part); the caller then collects candidates by running dcr_sim_topk on the part matrices
- * [nq * n_chunks, d / n_chunks] x [ng * n_chunks, d / n_chunks] with k' = (k - 1) * n_chunks + 1 (when k' <= 16), or once
- * per gallery part [nq * n_chunks, d / n_chunks] x [ng, d / n_chunks] with k' = k (any n_chunks; dcr_b200/similarity.py). */
+/* Top-k under the cross form of the 'splitloss' similarity (--stype cross, einsum_in_chunks diff_retrieval.py:643-662):
+ * a pair scores max over EVERY (query part a, gallery part b) of <q_a, g_b>.  The sweep of dcr_sim_topk_split walking all
+ * n_parts^2 part pairs, then the exact re-score: the fp64-accumulated part dot products folded with fmax from -inf, query
+ * part outer and gallery part inner, bit for bit what dcr_split_rescore(cross = 1) reports for the same pair.  Arguments,
+ * limits (no limit on d or n_parts), ordering, ties and workspace as dcr_sim_topk_split; n_parts = 1 returns the bits of
+ * dcr_sim_topk.  The sweep's work grows with n_parts^2 (n_parts times the aligned form's). */
+size_t dcr_sim_topk_cross_workspace_size(int nq, int ng, int d, int n_parts, int k);
+int dcr_sim_topk_cross(const float* q, int nq, const float* g, int ng, int d, int n_parts, int k, int64_t g_index_base,
+                       int64_t g_index_stride, float* out_scores, int64_t* out_idx, void* workspace,
+                       size_t workspace_bytes, void* stream);
+
+/* Exact split scores of given candidates: descriptors cut into n_chunks equal parts, pair score = max over the parts of
+ * the per-part dot products (cross != 0: over every (query part, gallery part) pair).  cand [nq][n_cand] lists gallery
+ * rows per query (duplicates allowed, negative entries are empty slots); this evaluates the exact split score of every
+ * candidate (float64 accumulation, folded with fmax from -inf -- query part outer, gallery part inner -- reported as fp32)
+ * and writes the k best per query ordered by (score desc, row asc).  d %% n_chunks == 0, (d / n_chunks) %% 4 == 0,
+ * k <= n_cand <= 4096.  It defines the bits dcr_sim_topk_split / dcr_sim_range_split (aligned) and dcr_sim_topk_cross /
+ * dcr_sim_range_cross (cross) report; those searches collect their own candidates in one fused sweep. */
 int dcr_split_rescore(const float* q, const float* g, int nq, int d, int n_chunks, int cross, const int64_t* cand,
                       int n_cand, int k, float* out_scores, int64_t* out_idx, void* stream);
 
@@ -214,6 +221,17 @@ int dcr_sim_range_sharded(const float* q, int nq, const float* g, int ng_local, 
  * without the [G, Q, C] tensor the einsum materialises. */
 size_t dcr_sim_range_split_workspace_size(int nq, int ng, int d, int n_parts, int64_t max_pairs);
 int dcr_sim_range_split(const float* q, int nq, const float* g, int ng, int d, int n_parts, float threshold,
+                        int64_t g_index_base, int64_t g_index_stride, int64_t* row_offsets, int64_t* out_idx,
+                        float* out_scores, int64_t max_pairs, int64_t* counts, void* workspace, size_t workspace_bytes,
+                        void* stream);
+
+/* Threshold search under the cross form of the 'splitloss' similarity (--stype cross, einsum_in_chunks
+ * diff_retrieval.py:643-662): every pair whose score max over every (query part a, gallery part b) of <q_a, g_b> reaches
+ * the threshold, bit for bit what dcr_split_rescore(cross = 1) and dcr_sim_topk_cross report for the same pair.  The
+ * arguments, CSR output, counts, DCR_ERR_CAPACITY protocol, determinism and limits of dcr_sim_range_split; n_parts = 1
+ * returns the bits of dcr_sim_range. */
+size_t dcr_sim_range_cross_workspace_size(int nq, int ng, int d, int n_parts, int64_t max_pairs);
+int dcr_sim_range_cross(const float* q, int nq, const float* g, int ng, int d, int n_parts, float threshold,
                         int64_t g_index_base, int64_t g_index_stride, int64_t* row_offsets, int64_t* out_idx,
                         float* out_scores, int64_t max_pairs, int64_t* counts, void* workspace, size_t workspace_bytes,
                         void* stream);
