@@ -270,9 +270,18 @@ TOPK_CASES = [
 ]
 
 
-def topk_case(name: str, d: int, centred: bool) -> Case:
+def topk_case(name: str, d: int, centred: bool, **build_kw) -> Case:
     _, k, n_b, shared, tie, _ = next(c for c in TOPK_CASES if c[0] == name)
-    return build(d, n_b, centred=centred, shared=shared, tie=tie)
+    return build(d, n_b, centred=centred, shared=shared, tie=tie, **build_kw)
+
+
+def stage_of(name: str) -> str:
+    return next(c for c in TOPK_CASES if c[0] == name)[5]
+
+
+# 258 queries, pairs at scales 1, 2, 1/2: query tiles of 128 + 128 + 2.  A power of two scales every score, norm and eps
+# exactly, so every query is decided by the stage its instance is built for.  Query r has scale MANY_SCALES[r // 2].
+MANY_SCALES = (1.0, 2.0, 0.5) * 43
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -339,7 +348,7 @@ def split_embed(case: Case, n_parts: int, part: int, layout: str = "quiet", othe
 def split_case(name: str, p: int, n_parts: int, part: int, layout: str = "quiet", other: int = -1, **build_kw) -> Case:
     """A TOPK_CASES instance (by name), or with name "range" the threshold-search instance build(p, 20, **build_kw)
     (tie=, scales=), in part `part` of n_parts."""
-    base = build(p, 20, centred=False, **build_kw) if name == "range" else topk_case(name, p, False)
+    base = build(p, 20, centred=False, **build_kw) if name == "range" else topk_case(name, p, False, **build_kw)
     return split_embed(base, n_parts, part, layout, other)
 
 
@@ -426,3 +435,189 @@ def split_realized(case: Case, op: SplitOperands) -> np.ndarray:
     c = case.info["n_parts"]
     rows = np.arange(case.q.shape[0])
     return split_exact(case.q, case.g, c)[rows, case.target] - split_approx(op, c)[rows, case.target].astype(np.float64)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Mixed stages in one call (the aligned split score)
+#
+# The first, second and brute-force instances of one k in three parts of one gallery (build() always gives 512 rows):
+# query r is of type r % 3 and holds instance (r % 3)'s query r in that instance's part, zeros elsewhere.  Its zero parts
+# score 0 and give terms of 1e-30, so its candidates, its eps and its stage are those of its own instance; the flagged
+# queries of a pass are then no prefix of the batch and span every query tile.
+
+MIXED = {1: ("k1_first", "k1_second", "k1_brute"), 10: ("k10_first", "k10_second", "k10_brute")}
+
+
+def mixed_case(k: int, p: int, n_parts: int, parts, scales=MANY_SCALES, seed: int = 0) -> Case:
+    assert len(set(parts)) == 3 and all(0 <= c < n_parts for c in parts)
+    cases = [topk_case(name, p, False, scales=scales) for name in MIXED[k]]
+    nq, ng = cases[0].q.shape[0], cases[0].g.shape[0]
+    rng = np.random.default_rng(seed + 1009 * n_parts + 17 * parts[0] + 5 * parts[1] + parts[2])
+    q = np.zeros((nq, n_parts * p), np.float32)
+    g = (rng.integers(-3, 4, size=(ng, n_parts * p)) * U).astype(np.float32)
+    for case, c in zip(cases, parts):
+        assert case.g.shape[0] == ng
+        g[:, c * p:(c + 1) * p] = case.g
+    types = np.arange(nq) % 3
+    for r in range(nq):
+        c = parts[types[r]]
+        q[r, c * p:(c + 1) * p] = cases[types[r]].q[r]
+    return Case(q=q, g=g, centred=False, target=np.array([cases[t].target[r] for r, t in enumerate(types)]),
+                comps=[cases[t].comps[r] for r, t in enumerate(types)], twin=np.full(nq, -1, np.int64),
+                info=dict(d=p, n_parts=n_parts, p=p, parts=tuple(parts), types=types, layout="mixed",
+                          stages=[stage_of(MIXED[k][t]) for t in types]))
+
+
+def nan_rows(nq: int) -> np.ndarray:
+    """Every 7th query, and the last row of the first query tile, the first of the second and the last of the batch."""
+    return np.array(sorted(set(range(0, nq, 7)) | {r for r in (127, 128, nq - 1) if 0 <= r < nq}), dtype=np.int64)
+
+
+def with_nan(case: Case, rows, part: int) -> Case:
+    """A NaN in the first value of query part `part` (a zero part of these queries) of every row in `rows`.  Its part
+    norms are NaN, so eps is NaN and the certificate fails in both passes: such a query is answered by the brute-force
+    path.  The pairs of the NaN part are ignored by the score, so the answer is the query's answer without it."""
+    p = case.info["p"]
+    q = case.q.copy()
+    assert not q[rows, part * p:(part + 1) * p].any()
+    q[rows, part * p] = np.nan
+    return Case(q=q, g=case.g, centred=False, target=case.target, comps=case.comps, twin=case.twin,
+                info=dict(case.info, nan_rows=np.asarray(rows), nan_part=part))
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# The cross split score: an instance in one (query part, gallery part) pair
+#
+# sim_topk_split(cross=True) and sim_range_split(cross=True) rank on the maximum over every (query part a, gallery part
+# b) of the bf16 dot product and trust cross_row_bound (sim_sweep.cuh): the largest over the pairs of row_bound's
+# expression, from query part a's norms (q_norm_*[qrow * n_parts + a]) and gallery part b's maxima (g_max[2b],
+# g_max[2b + 1]).  The operands are those of the split score (to_bf16_parts_kernel: split_operands).
+#
+# cross_embed puts a build() instance into the pair (a, b), a != b: the queries in query part a, the gallery in gallery
+# part b; the other query parts are zero and the other gallery parts hold tiny exact fillers x*2^-11 (|x| <= 3).  Every
+# other pair scores near 0 and has a term of at most 1e-3 of (a, b)'s, so eps comes from (a, b) alone: a bound read from
+# the aligned pairs (split_row_bound), from another query part's norms or from another gallery part's maxima collapses
+# below A's realized error.  The split layouts (split_embed) hold under the cross score too: their instance pairs are
+# the aligned ones, and a pair across two parts meets a filler.
+
+CROSS_PLACES = [(2, 64, 0, 1), (4, 516, 3, 0), (40, 64, 33, 1), (197, 64, 196, 0)]   # (C, p, a, b); 516 pads to 576
+# the threshold search's shapes: resident query tile (d_pad <= 512) and streamed
+CROSS_RANGE_SHAPES = ((2, 256), (4, 64), (8, 64), (4, 516), (40, 64), (197, 64))
+
+
+def cross_embed(case: Case, n_parts: int, a: int, b: int, seed: int = 0) -> Case:
+    """`case` (uncentred, dimension p): its queries in query part a, its gallery in gallery part b (see above)."""
+    assert not case.centred and a != b and 0 <= a < n_parts and 0 <= b < n_parts
+    nq, p = case.q.shape
+    ng = case.g.shape[0]
+    rng = np.random.default_rng(seed + 1009 * n_parts + 17 * a + b)
+    q = np.zeros((nq, n_parts * p), np.float32)
+    g = (rng.integers(-3, 4, size=(ng, n_parts * p)) * U).astype(np.float32)
+    q[:, a * p:(a + 1) * p] = case.q
+    g[:, b * p:(b + 1) * p] = case.g
+    return Case(q=q, g=g, centred=False, target=case.target, comps=case.comps, twin=case.twin,
+                info=dict(case.info, n_parts=n_parts, p=p, part=a, other=b, layout="pair"))
+
+
+def cross_pairs(n_parts: int):
+    """(a, b) of every pair a shape is tested at: the first query part against the last gallery part, the reverse, and
+    query part 33 against gallery part 1 and 196 against 0 when there are such parts (the second and the seventh lane
+    round of cross_row_bound's loop over a)."""
+    pairs = [(0, n_parts - 1), (n_parts - 1, 0)] + ([(33, 1)] if n_parts > 33 else []) + ([(196, 0)] if n_parts > 196 else [])
+    return list(dict.fromkeys(pairs))
+
+
+def cross_placements(n_parts: int):
+    """(layout, part, other): the pairs of cross_pairs, then the split layouts of split_placements."""
+    return [("pair", a, b) for a, b in cross_pairs(n_parts)] + split_placements(n_parts)
+
+
+def cross_case(name: str, p: int, n_parts: int, layout: str, part: int, other: int, **build_kw) -> Case:
+    """A TOPK_CASES instance (or with name "range" build(p, 20, **build_kw)) at a placement of cross_placements."""
+    if layout != "pair":
+        return split_case(name, p, n_parts, part, layout, other, **build_kw)
+    base = build(p, 20, centred=False, **build_kw) if name == "range" else topk_case(name, p, False, **build_kw)
+    return cross_embed(base, n_parts, part, other)
+
+
+def instance_pair(case: Case):
+    """(query part, gallery part) where A reaches its score."""
+    return (case.info["part"], case.info["other"]) if case.info["layout"] == "pair" else (case.info["part"],) * 2
+
+
+def cross_part_eps(op: SplitOperands, p_pad: int) -> np.ndarray:
+    """cross_row_bound's term of every (query part a, gallery part b), in the kernel's fp32 order of operations: query
+    part a's norms, gallery part b's maxima, split_part_eps's expression: [nq, C, C]."""
+    f = np.float32
+    qh, qr, qx = op.qnh[:, :, None], op.qnr[:, :, None], op.qnx[:, :, None]
+    gn, gr = op.g_norm[None, None, :], op.g_res[None, None, :]
+    e = f(1.001) * (qh * gr + qr * gn) + f(p_pad) * f(2.4e-7) * qh * (gn + gr) + f(3e-7) * qx * gn + f(1e-30)
+    return e.astype(np.float32)
+
+
+def cross_eps(op: SplitOperands, p_pad: int) -> np.ndarray:
+    """cross_row_bound's eps per query row: the largest pair term."""
+    return cross_part_eps(op, p_pad).max(axis=(1, 2))
+
+
+def cross_bf16_terms(op: SplitOperands) -> np.ndarray:
+    """The bf16 part of every pair's term, qh_a g_res_b + qr_a g_norm_b: [nq, C, C]."""
+    return (op.qnh[:, :, None] * op.g_res[None, None, :] + op.qnr[:, :, None] * op.g_norm[None, None, :]).astype(np.float32)
+
+
+def _cross_fold(q: np.ndarray, g: np.ndarray, n_parts: int, as_f32: bool) -> np.ndarray:
+    """max over every (query part, gallery part) of the fp64 dot product (rounded to fp32 first when as_f32), folded
+    with fmax (a NaN pair is ignored), a few query parts at a time: memory about max(nq * ng * C, 2^23) values."""
+    nq, d = q.shape
+    ng, p = g.shape[0], d // n_parts
+    q64 = q.astype(np.float64).reshape(nq, n_parts, p)
+    g64 = g.astype(np.float64).reshape(ng * n_parts, p)
+    best = np.full((nq, ng), -np.inf, np.float32 if as_f32 else np.float64)
+    step = max(1, 2 ** 23 // (nq * ng * n_parts))
+    for a in range(0, n_parts, step):
+        na = min(step, n_parts - a)
+        s = (q64[:, a:a + na].reshape(nq * na, p) @ g64.T).reshape(nq, na, ng, n_parts)
+        s = np.fmax.reduce(np.fmax.reduce(s.astype(np.float32) if as_f32 else s, axis=3), axis=1)
+        best = np.fmax(best, s)
+    return best
+
+
+def cross_approx(op: SplitOperands, n_parts: int) -> np.ndarray:
+    """The fused sweep's cross score: per pair the tensor-core product of the bf16 operands (exact here) as fp32, then
+    the maximum over the pairs."""
+    return _cross_fold(op.qh, op.gh, n_parts, True)
+
+
+def cross_exact(q: np.ndarray, g: np.ndarray, n_parts: int) -> np.ndarray:
+    """The fp64 cross score."""
+    return _cross_fold(q, g, n_parts, False)
+
+
+def cross_realized(case: Case, op: SplitOperands) -> np.ndarray:
+    """Per query: how far the target's approximate cross score lies below its exact cross score."""
+    c = case.info["n_parts"]
+    rows = np.arange(case.q.shape[0])
+    return cross_exact(case.q, case.g, c)[rows, case.target] - cross_approx(op, c)[rows, case.target].astype(np.float64)
+
+
+# The cross re-score (cross_exact_scores) stages the query `staged` parts at a time in kCrossStageBytes of shared
+# memory, (pl + 8) fp64 values per part: the restatement of cross_staged_parts.
+CROSS_STAGE_BYTES = 44 * 1024
+
+
+def cross_staged_parts(n_parts: int, pl: int) -> int:
+    return max(1, min(n_parts, CROSS_STAGE_BYTES // ((pl + 8) * 8)))
+
+
+def cross_groups(n_parts: int, pl: int):
+    """The sizes of the staged groups, in order."""
+    s = cross_staged_parts(n_parts, pl)
+    return [min(s, n_parts - a0) for a0 in range(0, n_parts, s)]
+
+
+# (C, p): the shapes whose groups the staged-group tests walk, with those groups
+STAGED_SHAPES = {(79, 64): [78, 1], (156, 64): [78, 78], (197, 64): [78, 78, 41], (3, 2808): [2, 1], (2, 4096): [1, 1],
+                 (3, 8192): [1, 1, 1]}
+
+# (C, p, parts of the first / second / brute instance, a part that is zero for every query): the mixed-stage shapes
+MIXED_PLACES = [(4, 64, (0, 1, 3), 2), (40, 64, (1, 33, 39), 0)]

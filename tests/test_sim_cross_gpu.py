@@ -146,21 +146,7 @@ def test_argument_errors_are_refused_with_a_message():
 # ------------------------------------------------------------------------------------------------------------------
 # the winning pair (query part a, gallery part b), a != b, at its bf16 error bound
 
-def _cross_embed(case, n_parts, a, b):
-    """`case` (uncentred, dimension p): its queries in query part a, its gallery in gallery part b.  Every other query
-    part is zero and every other gallery part a tiny exact filler, so the pair (a, b) decides every score and its norms
-    decide eps; the pair (a, a) meets only filler."""
-    nq, p = case.q.shape
-    ng = case.g.shape[0]
-    rng = np.random.default_rng(1009 * n_parts + 17 * a + b)
-    q = np.zeros((nq, n_parts * p), np.float32)
-    g = (rng.integers(-3, 4, size=(ng, n_parts * p)) * sbc.U).astype(np.float32)
-    q[:, a * p:(a + 1) * p] = case.q
-    g[:, b * p:(b + 1) * p] = case.g
-    return torch.from_numpy(q), torch.from_numpy(g)
-
-
-CROSS_PLACES = [(2, 64, 0, 1), (4, 516, 3, 0), (40, 64, 33, 1), (197, 64, 196, 0)]   # (C, p, a, b); 516 pads to 576
+CROSS_PLACES = sbc.CROSS_PLACES   # (C, p, a, b): the instance in the pair (a, b) (sbc.cross_embed)
 ADVERSARIAL = [(name, *place) for name, *_ in sbc.TOPK_CASES for place in CROSS_PLACES]
 
 
@@ -171,7 +157,8 @@ def test_pair_at_its_bf16_bound(name, c, p, a, b):
     instance is built for."""
     _, k, n_b, shared, tie, stage = next(x for x in sbc.TOPK_CASES if x[0] == name)
     case = sbc.topk_case(name, p, False)
-    q, g = _cross_embed(case, c, a, b)
+    e = sbc.cross_embed(case, c, a, b)
+    q, g = torch.from_numpy(e.q), torch.from_numpy(e.g)
     v, i, st = _check(q, g, k, c)
     nq = q.shape[0]
     assert (i[:, 0] == case.target).all()
