@@ -14,7 +14,7 @@ class DcrError(RuntimeError):
     pass
 
 
-ERR_CAPACITY = -3   # DCR_ERR_CAPACITY: dcr_sim_range(_split)(_sharded) found more candidate pairs than its capacities
+ERR_CAPACITY = -3   # DCR_ERR_CAPACITY: dcr_sim_range(_split|_cross)(_sharded) found more candidate pairs than its capacities
 
 
 # name -> (restype, argtypes); mirrors include/dcr_b200.h one to one (tests check the header against this table)
@@ -56,6 +56,11 @@ SIGNATURES = {
                                       C.c_void_p, C.c_size_t, C.c_void_p]),
     "dcr_sim_range_split_sharded_workspace_size": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64]),
     "dcr_sim_range_split_sharded": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float,
+                                              C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.POINTER(C.c_int64),
+                                              C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dcr_sim_range_cross_sharded_workspace_size": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64]),
+    "dcr_sim_range_cross_sharded": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float,
                                               C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.POINTER(C.c_int64),
                                               C.c_void_p, C.c_size_t, C.c_void_p]),

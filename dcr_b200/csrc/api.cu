@@ -199,6 +199,24 @@ int dcr_sim_range_split_sharded(const float* q, int nq, const float* g, int ng_l
                                       reinterpret_cast<long long*>(counts), workspace, workspace_bytes, as_stream(stream));
 }
 
+size_t dcr_sim_range_cross_sharded_workspace_size(int nq, int ng_local, int d, int n_parts, int world,
+                                                  int64_t max_local_pairs) {
+  return dcr::sim_range_split_sharded_workspace_size(nq, ng_local, d, n_parts, world, max_local_pairs, true);
+}
+
+int dcr_sim_range_cross_sharded(const float* q, int nq, const float* g, int ng_local, int d, int n_parts, float threshold,
+                                int64_t g_index_base, int64_t g_index_stride, int world, dcr_allgather_fn allgather,
+                                void* allgather_ctx, int64_t* row_offsets, int64_t* out_idx, float* out_scores,
+                                int64_t max_pairs, int64_t max_local_pairs, int64_t* counts, void* workspace,
+                                size_t workspace_bytes, void* stream) {
+  // argument checks happen inside, after the local search: a bad argument on one rank must still reach the exchange
+  return dcr::sim_range_split_sharded(q, nq, g, ng_local, d, n_parts, threshold, g_index_base, g_index_stride, world,
+                                      allgather, allgather_ctx, reinterpret_cast<long long*>(row_offsets),
+                                      reinterpret_cast<long long*>(out_idx), out_scores, max_pairs, max_local_pairs,
+                                      reinterpret_cast<long long*>(counts), workspace, workspace_bytes, as_stream(stream),
+                                      true);
+}
+
 int dcr_sim_topk_last_stats(int* out8) {
   DCR_REQUIRE(out8 != nullptr, "dcr_sim_topk_last_stats: null pointer");
   out8[0] = g_last_stats.cta_group;

@@ -59,12 +59,14 @@ int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int 
                       long long g_index_stride, int world, AllgatherFn allgather, void* allgather_ctx, long long* row_offsets,
                       long long* out_idx, float* out_scores, long long max_pairs, long long max_local_pairs,
                       long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream);
-size_t sim_range_split_sharded_workspace_size(int nq, int ng_local, int d, int n_parts, int world, long long max_local_pairs);
+// the split forms; cross: the cross split score (dcr_sim_range_cross_sharded)
+size_t sim_range_split_sharded_workspace_size(int nq, int ng_local, int d, int n_parts, int world, long long max_local_pairs,
+                                              bool cross = false);
 int sim_range_split_sharded(const float* q, int nq, const float* g, int ng_local, int d, int n_parts, float threshold,
                             long long g_index_base, long long g_index_stride, int world, AllgatherFn allgather,
                             void* allgather_ctx, long long* row_offsets, long long* out_idx, float* out_scores,
                             long long max_pairs, long long max_local_pairs, long long* counts, void* ws, size_t ws_bytes,
-                            cudaStream_t stream);
+                            cudaStream_t stream, bool cross = false);
 
 int split_rescore(const float* q, const float* g, int nq, int d, int n_chunks, int cross, const long long* cand, int n_cand,
                   int k, float* out_scores, long long* out_idx, cudaStream_t stream);

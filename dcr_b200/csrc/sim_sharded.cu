@@ -15,9 +15,10 @@
 //                       place in its row by binary search in the other ranks' pieces of that row.  No atomic decides an
 //                       order; a check pass before it refuses overlapping shards and malformed messages.
 // Every score is a function of its pair alone and the pieces are complete, so the merged rows are the rows sim_range
-// returns for the union of the shards.  The split form (dcr_sim_range_split_sharded) runs sim_range_split as the local
-// search; the exchange and the merge are the same, and header word [9] carries n_parts so that ranks running different
-// searches disagree instead of merging.
+// returns for the union of the shards.  The split forms (dcr_sim_range_split_sharded, dcr_sim_range_cross_sharded) run
+// sim_range_split, aligned or cross, as the local search; the exchange and the merge are the same, and header word [9]
+// carries the score (0 the dot product, n_parts aligned, -n_parts cross) so that ranks running different searches
+// disagree instead of merging.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -57,15 +58,38 @@ struct ShardLayout {
   size_t total;
 };
 
-// n_parts = 0: the dot product; >= 1: the split score (the local search is sim_range_split)
-int shard_layout(int nq, int ng_local, int d, int n_parts, int world, long long cap, void* base, ShardLayout* L) {
-  const char* who = n_parts ? "sim_range_split_sharded" : "sim_range_sharded";
+// The score a sharded threshold search computes.  One part of either split score is the dot product: such a rank plans,
+// searches and writes header word [9] as kDot, so it agrees with a dot-product peer.
+enum class Score { kDot, kAligned, kCross };
+
+const char* sharded_name(Score s) {
+  return s == Score::kDot ? "sim_range_sharded" : s == Score::kCross ? "sim_range_cross_sharded" : "sim_range_split_sharded";
+}
+
+// header word [9]: 0 the dot product, n_parts the aligned split score, -n_parts the cross split score (n_parts >= 2), so
+// that no two forms write the same word
+long long score_word(Score s, int n_parts) {
+  return s == Score::kDot ? 0 : s == Score::kCross ? -static_cast<long long>(n_parts) : n_parts;
+}
+
+// the form a header word names, for the disagreement message
+std::string score_of_word(long long w) {
+  if (w == 0) return "the dot product";
+  const unsigned long long parts = w < 0 ? 0ull - static_cast<unsigned long long>(w) : static_cast<unsigned long long>(w);
+  return std::string(w < 0 ? "the cross score over " : "the aligned score over ") + std::to_string(parts) + " parts";
+}
+
+// kDot: the local search is sim_range (n_parts unused); kAligned / kCross: sim_range_split over n_parts >= 2 parts
+int shard_layout(int nq, int ng_local, int d, Score score, int n_parts, int world, long long cap, void* base,
+                 ShardLayout* L) {
+  const char* who = sharded_name(score);
   DCR_REQUIRE(world >= 1 && world <= kMaxWorld, "%s: world=%d outside [1, %d]", who, world, kMaxWorld);
   DCR_REQUIRE(nq >= 1 && ng_local >= 0, "%s: bad problem (nq=%d ng_local=%d)", who, nq, ng_local);
   DCR_REQUIRE(cap >= 0 && cap <= kMaxLocalPairs, "%s: max_local_pairs=%lld outside [0, 2^40]", who, cap);
   // an empty shard runs no search, but its d is still checked by the same planner
   const int ng_plan = ng_local > 0 ? ng_local : 1;
-  L->inner = n_parts ? sim_range_split_workspace_size(nq, ng_plan, d, n_parts, cap) : sim_range_workspace_size(nq, ng_plan, d, cap);
+  L->inner = score == Score::kDot ? sim_range_workspace_size(nq, ng_plan, d, cap)
+                                  : sim_range_split_workspace_size(nq, ng_plan, d, n_parts, cap, score == Score::kCross);
   if (L->inner == 0) return -1;
   if (ng_local == 0) L->inner = 0;
   const size_t msg = msg_bytes(nq, cap);
@@ -257,14 +281,14 @@ int sim_topk_sharded(const float* q, int nq, const float* g, int ng_local, int d
 
 namespace {
 
-// The sharded threshold search.  split = false: the dot product (n_parts unused, header word [9] = 0); true: the split
-// score over n_parts parts, one part being the dot product itself (word [9] = 0 then too).
-int range_sharded(const float* q, int nq, const float* g, int ng_local, int d, bool split, int n_parts, float threshold,
+// The sharded threshold search.  score = kDot: the dot product (n_parts unused); kAligned / kCross: that split score over
+// n_parts parts, one part being the dot product itself (the search, and header word [9], of kDot then).
+int range_sharded(const float* q, int nq, const float* g, int ng_local, int d, Score score, int n_parts, float threshold,
                   long long g_index_base, long long g_index_stride, int world, AllgatherFn allgather, void* allgather_ctx,
                   long long* row_offsets, long long* out_idx, float* out_scores, long long max_pairs,
                   long long max_local_pairs, long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
-  const char* who = split ? "sim_range_split_sharded" : "sim_range_sharded";
-  const int parts = split && n_parts > 1 ? n_parts : 0;
+  const char* who = sharded_name(score);
+  const Score form = n_parts > 1 ? score : Score::kDot;   // one part is the dot product; n_parts < 1 is refused below
   // the only outcomes decided before the first exchange: without these there is nobody to agree with
   DCR_REQUIRE(world >= 1 && world <= kMaxWorld, "%s: world=%d outside [1, %d]", who, world, kMaxWorld);
   DCR_REQUIRE(world == 1 || allgather != nullptr, "%s: world=%d needs an all-gather callback", who, world);
@@ -272,17 +296,18 @@ int range_sharded(const float* q, int nq, const float* g, int ng_local, int d, b
   // 1. the local search; its outcome goes into the header, whatever it is
   uint32_t thr_bits;
   std::memcpy(&thr_bits, &threshold, 4);
-  long long hdr[kHdrWords] = {kHdrMagic, 0, 0, 0, max_local_pairs, max_pairs, nq, d, static_cast<long long>(thr_bits), parts};
+  long long hdr[kHdrWords] = {kHdrMagic, 0, 0, 0, max_local_pairs, max_pairs, nq, d, static_cast<long long>(thr_bits),
+                             score_word(form, n_parts)};
   ShardLayout L{};
   uint8_t* w = static_cast<uint8_t*>(ws);
   auto local = [&]() -> int {
     DCR_REQUIRE(q && (g || ng_local == 0) && row_offsets && counts && (max_pairs == 0 || (out_idx && out_scores)),
                 "%s: null pointer argument", who);
-    DCR_REQUIRE(!split || n_parts >= 1, "%s: n_parts=%d < 1", who, n_parts);
+    DCR_REQUIRE(score == Score::kDot || n_parts >= 1, "%s: n_parts=%d < 1", who, n_parts);
     DCR_REQUIRE(!std::isnan(threshold), "%s: threshold is NaN", who);
     DCR_REQUIRE(g_index_stride >= 1, "%s: g_index_stride=%lld < 1", who, g_index_stride);
     DCR_REQUIRE(max_pairs >= 0, "%s: max_pairs=%lld < 0", who, max_pairs);
-    if (int rc = shard_layout(nq, ng_local, d, parts, world, max_local_pairs, w, &L)) return rc;
+    if (int rc = shard_layout(nq, ng_local, d, form, n_parts, world, max_local_pairs, w, &L)) return rc;
     DCR_REQUIRE(w != nullptr && ws_bytes >= L.total, "%s: workspace too small (%zu < %zu)", who, ws_bytes, L.total);
     DCR_REQUIRE((reinterpret_cast<uintptr_t>(w) & 255) == 0, "%s: workspace must be 256-byte aligned", who);
     long long* send_off = reinterpret_cast<long long*>(L.send);
@@ -295,10 +320,12 @@ int range_sharded(const float* q, int nq, const float* g, int ng_local, int d, b
     long long* send_idx = send_off + nq + 1;
     float* tmp_scores = reinterpret_cast<float*>(L.recv);
     long long c[2] = {0, 0};
-    const int rc = parts ? sim_range_split(q, nq, g, ng_local, d, parts, threshold, g_index_base, g_index_stride, send_off,
-                                           send_idx, tmp_scores, max_local_pairs, c, L.inner_ws, L.inner, stream)
-                         : sim_range(q, nq, g, ng_local, d, threshold, g_index_base, g_index_stride, send_off, send_idx,
-                                     tmp_scores, max_local_pairs, c, L.inner_ws, L.inner, stream);
+    const int rc = form == Score::kDot
+                       ? sim_range(q, nq, g, ng_local, d, threshold, g_index_base, g_index_stride, send_off, send_idx,
+                                   tmp_scores, max_local_pairs, c, L.inner_ws, L.inner, stream)
+                       : sim_range_split(q, nq, g, ng_local, d, n_parts, threshold, g_index_base, g_index_stride, send_off,
+                                         send_idx, tmp_scores, max_local_pairs, c, L.inner_ws, L.inner, stream,
+                                         form == Score::kCross);
     hdr[H_CAND] = c[1];
     if (rc) return rc;
     hdr[H_PAIRS] = c[0];
@@ -343,9 +370,8 @@ int range_sharded(const float* q, int nq, const float* g, int ng_local, int d, b
                 "has nq=%lld d=%lld threshold bits 0x%llx",
                 who, h(0, H_NQ), h(0, H_D), h(0, H_THR), r, h(r, H_NQ), h(r, H_D), h(r, H_THR));
   for (int r = 1; r < world; ++r)
-    DCR_REQUIRE(h(r, H_PARTS) == h(0, H_PARTS),
-                "%s: ranks disagree on the score: rank 0 has n_parts=%lld, rank %d has n_parts=%lld (0: the dot product)",
-                who, h(0, H_PARTS), r, h(r, H_PARTS));
+    DCR_REQUIRE(h(r, H_PARTS) == h(0, H_PARTS), "%s: ranks disagree on the score: rank 0 computes %s, rank %d %s", who,
+                score_of_word(h(0, H_PARTS)).c_str(), r, score_of_word(h(r, H_PARTS)).c_str());
   // capacities: every local search finished, every receive buffer holds the largest message, every output the total
   bool finished = true;
   long long cand_need = 0, p_max = 0, total = 0, min_cap = h(0, H_CAND_CAP), min_out = h(0, H_MAX_PAIRS);
@@ -404,7 +430,7 @@ int range_sharded(const float* q, int nq, const float* g, int ng_local, int d, b
 
 size_t sim_range_sharded_workspace_size(int nq, int ng_local, int d, int world, long long max_local_pairs) {
   ShardLayout L;
-  if (shard_layout(nq, ng_local, d, 0, world, max_local_pairs, nullptr, &L) != 0) return 0;
+  if (shard_layout(nq, ng_local, d, Score::kDot, 0, world, max_local_pairs, nullptr, &L) != 0) return 0;
   return L.total;
 }
 
@@ -412,18 +438,21 @@ int sim_range_sharded(const float* q, int nq, const float* g, int ng_local, int 
                       long long g_index_stride, int world, AllgatherFn allgather, void* allgather_ctx, long long* row_offsets,
                       long long* out_idx, float* out_scores, long long max_pairs, long long max_local_pairs,
                       long long* counts, void* ws, size_t ws_bytes, cudaStream_t stream) {
-  return range_sharded(q, nq, g, ng_local, d, false, 0, threshold, g_index_base, g_index_stride, world, allgather,
+  return range_sharded(q, nq, g, ng_local, d, Score::kDot, 0, threshold, g_index_base, g_index_stride, world, allgather,
                        allgather_ctx, row_offsets, out_idx, out_scores, max_pairs, max_local_pairs, counts, ws, ws_bytes,
                        stream);
 }
 
-size_t sim_range_split_sharded_workspace_size(int nq, int ng_local, int d, int n_parts, int world, long long max_local_pairs) {
+size_t sim_range_split_sharded_workspace_size(int nq, int ng_local, int d, int n_parts, int world, long long max_local_pairs,
+                                              bool cross) {
+  const Score score = cross ? Score::kCross : Score::kAligned;
   if (n_parts < 1) {
-    set_error(-1, "sim_range_split_sharded: n_parts=%d < 1", n_parts);
+    set_error(-1, "%s: n_parts=%d < 1", sharded_name(score), n_parts);
     return 0;
   }
   ShardLayout L;
-  if (shard_layout(nq, ng_local, d, n_parts == 1 ? 0 : n_parts, world, max_local_pairs, nullptr, &L) != 0) return 0;
+  if (shard_layout(nq, ng_local, d, n_parts == 1 ? Score::kDot : score, n_parts, world, max_local_pairs, nullptr, &L) != 0)
+    return 0;
   return L.total;
 }
 
@@ -431,10 +460,10 @@ int sim_range_split_sharded(const float* q, int nq, const float* g, int ng_local
                             long long g_index_base, long long g_index_stride, int world, AllgatherFn allgather,
                             void* allgather_ctx, long long* row_offsets, long long* out_idx, float* out_scores,
                             long long max_pairs, long long max_local_pairs, long long* counts, void* ws, size_t ws_bytes,
-                            cudaStream_t stream) {
-  return range_sharded(q, nq, g, ng_local, d, true, n_parts, threshold, g_index_base, g_index_stride, world, allgather,
-                       allgather_ctx, row_offsets, out_idx, out_scores, max_pairs, max_local_pairs, counts, ws, ws_bytes,
-                       stream);
+                            cudaStream_t stream, bool cross) {
+  return range_sharded(q, nq, g, ng_local, d, cross ? Score::kCross : Score::kAligned, n_parts, threshold, g_index_base,
+                       g_index_stride, world, allgather, allgather_ctx, row_offsets, out_idx, out_scores, max_pairs,
+                       max_local_pairs, counts, ws, ws_bytes, stream);
 }
 
 }  // namespace dcr

@@ -178,7 +178,7 @@ def _allgather_callback(allgather: Optional[Callable], world: int, device: torch
 
 def sharded_range(query_all: torch.Tensor, gallery_local: torch.Tensor, threshold: float, gallery_base: int, *,
                   allgather: Optional[Callable] = None, world: Optional[int] = None, index_stride: int = 1,
-                  num_chunks: int = 1) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                  num_chunks: int = 1, cross: bool = False) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """Threshold search over a gallery sharded across ranks, through the C entry `dcr_sim_range_sharded`
     (include/dcr_b200.h): every rank searches ALL queries against its shard (global index of local row j =
     gallery_base + index_stride * j), the CSR pieces are exchanged and merged on the device, and every rank returns
@@ -188,7 +188,10 @@ def sharded_range(query_all: torch.Tensor, gallery_local: torch.Tensor, threshol
     sharded_topk_c (default: torch.distributed.all_gather_into_tensor).  The capacities start where sim_range's do; when
     some rank needs more, every rank gets DCR_ERR_CAPACITY with the needs and retries once, together.
     num_chunks > 1: the 'splitloss' score over that many aligned parts (`dcr_sim_range_split_sharded`), bit for bit
-    what similarity.sim_range_split returns for the union of the shards."""
+    what similarity.sim_range_split returns for the union of the shards.  cross=True with num_chunks > 1: the cross
+    score (`--stype cross`, `dcr_sim_range_cross_sharded`), bit for bit what similarity.sim_range_split(cross=True)
+    returns for the union of the shards; with num_chunks = 1 it is the dot product.  Every rank must pass the same
+    num_chunks and cross: ranks computing different scores raise DcrError ("disagree") instead of merging."""
     import ctypes as C
     from . import _lib
     from .similarity import _aligned_ptr, _check_cuda_f32
@@ -205,7 +208,7 @@ def sharded_range(query_all: torch.Tensor, gallery_local: torch.Tensor, threshol
     g_ptr = (g.data_ptr() if ng > 0 else None) if g_ok else None
     cb = _allgather_callback(allgather, world, q.device, "sharded_range")
     split = num_chunks > 1
-    what = "dcr_sim_range_split_sharded" if split else "dcr_sim_range_sharded"
+    what = ("dcr_sim_range_cross_sharded" if cross else "dcr_sim_range_split_sharded") if split else "dcr_sim_range_sharded"
     counts = (C.c_int64 * 3)()
     local_cap = out_cap = max(1 << 20, 16 * nq)   # sim_range's start; the exact needs come back with ERR_CAPACITY
     with torch.cuda.device(q.device):
@@ -213,8 +216,7 @@ def sharded_range(query_all: torch.Tensor, gallery_local: torch.Tensor, threshol
         for attempt in range(2):
             # 0 (invalid arguments) is passed on: the library reports the reason on every rank
             if split:
-                nbytes = lib.dcr_sim_range_split_sharded_workspace_size(nq, ng if g_ok else 1, d, num_chunks, world,
-                                                                        local_cap)
+                nbytes = getattr(lib, what + "_workspace_size")(nq, ng if g_ok else 1, d, num_chunks, world, local_cap)
             else:
                 nbytes = lib.dcr_sim_range_sharded_workspace_size(nq, ng if g_ok else 1, d, world, local_cap)
             ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=q.device) if nbytes else None
@@ -225,8 +227,7 @@ def sharded_range(query_all: torch.Tensor, gallery_local: torch.Tensor, threshol
                     out_i.data_ptr() or None, out_s.data_ptr() or None, out_cap, local_cap, counts,
                     _aligned_ptr(ws) if ws is not None else None, nbytes, st)
             if split:
-                rc = lib.dcr_sim_range_split_sharded(q.data_ptr(), nq, g_ptr, ng if g_ok else 1, d, num_chunks,
-                                                     float(threshold), *args)
+                rc = getattr(lib, what)(q.data_ptr(), nq, g_ptr, ng if g_ok else 1, d, num_chunks, float(threshold), *args)
             else:
                 rc = lib.dcr_sim_range_sharded(q.data_ptr(), nq, g_ptr, ng if g_ok else 1, d, float(threshold), *args)
             if rc == _lib.ERR_CAPACITY and attempt == 0:

@@ -175,10 +175,11 @@ int dcr_sim_range(const float* q, int nq, const float* g, int ng, int d, float t
  * int64 words):
  *     [0] 0x31474E52524344 ("DCRRNG1" in memory)   [1] status: 0, DCR_ERR_CAPACITY or the code of a local failure
  *     [2] local pairs   [3] local candidates (the max_local_pairs its search needs)   [4] max_local_pairs   [5] max_pairs
- *     [6] nq   [7] d   [8] the threshold's fp32 bits   [9] n_parts: 0 here (dcr_sim_range_split_sharded writes its own)
+ *     [6] nq   [7] d   [8] the threshold's fp32 bits   [9] the score: 0 here, the dot product (the split forms below
+ *     write n_parts for the aligned split score and -n_parts for the cross split score, n_parts >= 2)
  * so every rank returns the same code:
  *   - a local failure on any rank (bad argument, workspace too small, CUDA error): that rank's code on every rank
- *   - headers that disagree on nq, d or the threshold: -1
+ *   - headers that disagree on nq, d, the threshold or the score: -1
  *   - a local search over its candidate capacity, a largest local pair count above some rank's max_local_pairs, or a
  *     global pair total above some rank's max_pairs: DCR_ERR_CAPACITY with counts[1] = the largest local candidate count
  *     and counts[2] = the global total (when a search did not finish, a bound: its candidates stand for its pairs).  The
@@ -247,6 +248,23 @@ int dcr_sim_range_cross(const float* q, int nq, const float* g, int ng, int d, i
 size_t dcr_sim_range_split_sharded_workspace_size(int nq, int ng_local, int d, int n_parts, int world,
                                                   int64_t max_local_pairs);
 int dcr_sim_range_split_sharded(const float* q, int nq, const float* g, int ng_local, int d, int n_parts, float threshold,
+                                int64_t g_index_base, int64_t g_index_stride, int world, dcr_allgather_fn allgather,
+                                void* allgather_ctx, int64_t* row_offsets, int64_t* out_idx, float* out_scores,
+                                int64_t max_pairs, int64_t max_local_pairs, int64_t* counts, void* workspace,
+                                size_t workspace_bytes, void* stream);
+
+/* Gallery-sharded form of dcr_sim_range_cross: dcr_sim_range_split_sharded with dcr_sim_range_cross as the local search,
+ * the same arguments, exchange, agreement rules, messages and merge.  Header word [9] = -n_parts, a value no other form
+ * writes, so a cross rank disagrees (-1 on every rank, the message naming both scores) with an aligned rank of the same
+ * n_parts, with a dot-product rank and with a cross rank of another n_parts; n_parts = 1 is the dot product (word [9] =
+ * 0, the bits of dcr_sim_range_sharded, agreeing with its peers).  On success every rank holds the CSR
+ * dcr_sim_range_cross returns for the same queries against the union of the shards, bit for bit.  The cross form of the
+ * reference's splitloss similarity.pth (--stype cross, diff_retrieval.py:643-662) for a gallery spread over ranks.
+ * workspace: dcr_sim_range_cross_sharded_workspace_size(nq, ng_local, d, n_parts, world, max_local_pairs) bytes, laid out
+ * as dcr_sim_range_sharded's around the cross local search. */
+size_t dcr_sim_range_cross_sharded_workspace_size(int nq, int ng_local, int d, int n_parts, int world,
+                                                  int64_t max_local_pairs);
+int dcr_sim_range_cross_sharded(const float* q, int nq, const float* g, int ng_local, int d, int n_parts, float threshold,
                                 int64_t g_index_base, int64_t g_index_stride, int world, dcr_allgather_fn allgather,
                                 void* allgather_ctx, int64_t* row_offsets, int64_t* out_idx, float* out_scores,
                                 int64_t max_pairs, int64_t max_local_pairs, int64_t* counts, void* workspace,
